@@ -1,6 +1,6 @@
-"""bench.py -- Mpaths/s of the ReSTIR PT frame (1 spp, 1920x1080, Cornell Box) on N B200s.
+"""bench.py -- Mpaths/s of the ReSTIR PT frame (1 spp, 1920x1080, Cornell Box) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A step is one frame of the reference's frame graph for the emissive Cornell Box, steady state (temporal and
@@ -12,16 +12,16 @@ temporal + spatial path reuse) -> compositing + firefly filter -> TAA. Nothing i
           pinned host memory every frame and the anti-aliased RGBA16F image is read back to pinned host memory
   roofline        the judged bandwidth kernel -- the streaming merge of the spatial resample (k_spatial_merge): algorithmic
                   bytes / event-timed duration against the measured HBM peak; `dominant` names the kernel with the largest share
-                  of the frame (traversal / issue bound, no bandwidth claim); `traffic` = DRAM bytes per launch from the committed
-                  ncu capture, only if that capture was taken from the kernel sources that are being timed
+                  of the frame (traversal / issue bound, no bandwidth claim); `traffic` (DRAM bytes per launch) is not measured
   cpu_baseline    the CPU oracle (a port: the reference ships no CPU renderer) on a bounded sample of the workload
   c1_alias_table  config C1: alias-table build, device (zr_alias_table_build) next to the CPU reference-equivalent
+  --dump-outputs DIR  after the timed frames, writes the anti-aliased image of the last one (what Render hands its caller) as
+                  DIR/output.npy, float32 [1080][1920][4]; the inputs depend only on the arguments, so two builds can be compared
   --impl reference   the same CPU path with every host core (SURVEY 8d: the only CPU arm the reference's math has); this arm
                   does not map libzetaray_b200.so (ZETARAY_B200_STRUCTS_ONLY)
 """
 import argparse
 import ctypes as C
-import hashlib
 import json
 import os
 import subprocess
@@ -91,17 +91,6 @@ def _clock_summary(samples):
     return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": float(samples[0][1]), "reasons": reasons}
 
 
-def kernel_sources_hash():
-    """Identifies the kernels an ncu capture belongs to: sha256 over the CUDA sources + the compile flags."""
-    h = hashlib.sha256()
-    d = os.path.join(ROOT, "zetaray_b200", "csrc")
-    for f in sorted(os.listdir(d)) + ["../build.py", "../../include/zr_fpmath.h"]:
-        p = os.path.join(d, f)
-        if os.path.isfile(p):
-            h.update(f.encode()); h.update(open(p, "rb").read())
-    return h.hexdigest()[:16]
-
-
 def alias_table_leg(st):
     """Config C1 (BASELINE.md 3): alias-table build at N = 2 / 13 107 / 10^6 emissive triangles, device vs CPU.
     The device build is normalise + partition in parallel and the pairing loop on ONE lane: Vose's LIFO pairing order defines the
@@ -147,6 +136,15 @@ def alias_table_leg(st):
         out.append({"n": n, "gpu_ms": round(gpu_ms, 4), "cpu_port_ms": round(cpu_ms, 4), "identical": bool(same)})
     return {"what": "alias-table build (normalise + Vose), one call", "cpu": "oracle port, 1 thread (the reference's BuildAliasTable is scalar + AVX2 normalise)",
             "sizes": out}
+
+
+def dump_outputs(out_dir, img):
+    """--dump-outputs: the RGBA16F output image -> out_dir/output.npy as float32 [height][width][4]."""
+    import numpy as np
+    from zetaray_b200.passes import download_image_pitched
+    rgba = download_image_pitched(img, np.float16, 4).reshape(img.height, img.width, 4)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "output.npy"), rgba.astype(np.float32))
 
 
 def cpu_frames(w, h, nframes, nthreads, warm=3):
@@ -204,6 +202,7 @@ def main():
     ap.add_argument("--impl", default="ours")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--single-stream", action="store_true", help="record DirectLighting on the main stream instead of a second one")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed frame's output image to DIR/output.npy (float32)")
     ap.add_argument("--schedule-by-cost", action="store_true", help="N > 1: launch the lighting kernels' blocks most-expensive-tile-first (measured cost map)")
     args = ap.parse_args()
     if args.impl == "reference":
@@ -301,7 +300,7 @@ def main():
         for _ in range(args.warmup):
             frame(seq.next())
     # per-frame working set: G-buffers 2 x 36 B/px, PT reservoirs 2 x 64, DI 2 x 32, targets/finals ~ 90 B/px => ~0.8 GB
-    # at 1080p, larger than the 126 MB L2, so no explicit flush between frames is needed.
+    # at 1080p, larger than the H100's 50 MB L2, so no explicit flush between frames is needed.
 
     # ---- value: device-resident ----
     launches0 = lib.zr_kernel_launch_count()
@@ -319,6 +318,8 @@ def main():
     stop.set()
     ms = e0.elapsed_time(e1)
     launches = lib.zr_kernel_launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, output_image())
     t = torch.tensor([ms], dtype=torch.float64, device="cuda")
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -417,8 +418,8 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s (not measured)"
         tot = sum(kern.values())
         y0, y1 = (0, H) if plan is None else plan.rows(rank)      # rank 0's strip
         own_rows = y1 - y0
@@ -446,16 +447,7 @@ def main():
         by_name = {k["kernel"]: k for k in kernels}
         judged = by_name.get("k_spatial_merge") or by_name.get("k_spatial") or kernels[0]
         top = kernels[0]
-        traffic, traffic_note = None, "no ncu capture committed for these kernel sources"
-        try:        # dram__bytes_read.sum + dram__bytes_write.sum of one launch, from the committed ncu --set full capture
-            cap = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")))
-            if cap.get("kernel_sources_sha16") == kernel_sources_hash():
-                traffic = cap["kernels"][judged["kernel"]]["dram_bytes"]
-                traffic_note = "profiles/r2_ncu_traffic.json (same kernel sources as timed)"
-            else:
-                traffic_note = "profiles/r2_ncu_traffic.json was captured from other kernel sources: not reported"
-        except Exception:
-            pass
+        traffic, traffic_note = None, "not measured"
         spatial_ms = sum(by_name[k]["ms_per_frame"] for k in ("k_spatial_search", "k_sort", "k_spatial_classify", "k_shift", "k_spatial_merge", "k_spatial") if k in by_name)
         roofline = {"kernel": judged["kernel"], "bound": "hbm", "achieved": judged["achieved_gbs"], "peak": peak, "unit": "GB/s",
                     "frac": judged["frac"], "traffic": traffic, "traffic_source": traffic_note, "peak_source": peak_src,
@@ -489,7 +481,7 @@ def main():
             "config": {"workload": WORKLOAD, "resolution": [W, H], "spp": 1, "bounces": 3, "restir_pt": "temporal + 1 spatial pass",
                        "restir_di": "temporal + pairwise-MIS spatial", "parallelism": "1 frame / %d horizontal strips (32-row halos, grouped NCCL send/recv from C++, image gathered on rank 0)" % world if world > 1 else "single GPU",
                        "strips": plan_info, "block_order": "most expensive tile first" if (world > 1 and args.schedule_by_cost) else "plain", "kernel_ms_per_frame_by_rank": rank_kernel_ms, "halo_bytes_per_exchange_per_rank": halo_bytes, "streams": 1 if side is None else 2, 
-                       "l2": "per-frame working set ~0.8 GB >> 126 MB L2 (no flush needed)"},
+                       "l2": "per-frame working set ~0.8 GB >> 50 MB L2 (no flush needed)"},
             "e2e": {"value": round(e2e_value, 3), "unit": "Mpaths/s", "h2d_bytes_per_step": C.sizeof(_lib.FrameConstants),
                     "d2h_bytes_per_step": W * H * 8, "frames": n_e2e},
             "gpu_launches": int(launches),

@@ -1,5 +1,5 @@
 /*
- * zr_abi.h -- C-ABI of the B200-native ReSTIR path-tracing core (libzetaray_b200.so).
+ * zr_abi.h -- C-ABI of the H100-native ReSTIR path-tracing core (libzetaray_b200.so).
  *
  * Every entry point replaces one piece of ZetaRay's render-pass interface for the hot path
  * (G-buffer -> pre-lighting/alias table -> ReSTIR DI -> ReSTIR PT -> compositing/firefly/TAA).
@@ -192,7 +192,7 @@ typedef struct zr_frame_constants
 } zr_frame_constants;
 
 /* ------------------------------------------------------------------------------------------
- * Per-pixel state layouts in HBM (B200-native: AoS records sized for 128-bit accesses)
+ * Per-pixel state layouts in HBM (AoS records sized for 128-bit accesses)
  * ------------------------------------------------------------------------------------------ */
 
 /* G-buffer. The reference keeps 10 textures (ZetaRenderer/Default/DefaultRendererImpl.h:97-109);

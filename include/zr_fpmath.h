@@ -7,7 +7,7 @@
  * would make RNG-driven branch decisions diverge between a CPU oracle and a GPU kernel.
  * Both sides therefore call the SAME transcendental approximations below, built only from
  * IEEE-754 +,-,*,/,sqrt and fma so they are bit-identical on x86-64 (gcc, -ffp-contract=off)
- * and sm_100a (nvcc, -fmad=false). Nothing here restates the reference's algorithms; it plays
+ * and sm_90a (nvcc, -fmad=false). Nothing here restates the reference's algorithms; it plays
  * the role "the same libm on both sides" plays in a CPU-vs-CPU comparison.
  *
  * Accuracy: sin/cos <= 2 ulp on [-2pi, 4pi]; exp/log <= 2 ulp on normal range.

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -17,10 +17,3 @@ def oracle():
     """ctypes handle of the CPU oracle (built on demand; it is test infrastructure)."""
     from tests import orc
     return orc.load()
-
-
-@pytest.fixture(scope="session")
-def reflib():
-    """The reference's own alias-table code compiled into oracle/_ref (None if unavailable)."""
-    from tests import orc
-    return orc.load_ref()

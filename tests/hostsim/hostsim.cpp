@@ -1,7 +1,7 @@
 // hostsim.cpp -- TEST INFRASTRUCTURE. Compiles the product's own traversal source (zetaray_b200/csrc/zr_scene.cuh:
 // Traverse<0/1>, TriHit, the node decode) for the host with g++, so that the BVH builder + traversal pair can be checked
 // against brute force on scenes of the benchmark's size (10^5 - 10^6 triangles) in the CPU test tier, where no GPU exists.
-// Nothing here is shipped or used by the product; the product path is the same source compiled by nvcc for sm_100a.
+// Nothing here is shipped or used by the product; the product path is the same source compiled by nvcc for sm_90a.
 #include "prelude.h"
 struct ZrTraverseStats { unsigned long long nodes, tris; };
 static thread_local ZrTraverseStats g_stats;

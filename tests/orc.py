@@ -1,6 +1,7 @@
 """ctypes loader for the CPU oracle (oracle/liborc.so) and the compiled reference (oracle/_ref).
 
-Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may use this."""
+Only tests/, __graft_entry__.smoke(), bench.py's cpu_baseline / --impl reference legs and tools/make_reference_golden.py may use
+this; the compiled reference is for the tool alone (the tests read its stored outputs in tests/golden/)."""
 import ctypes as C
 import os
 import subprocess
@@ -35,8 +36,6 @@ def load_ref():
     global _ref
     if _ref is None:
         so = os.path.join(ORACLE_DIR, "_ref", "libref_alias.so")
-        if not os.path.exists(so) and os.path.isdir("/root/reference/Source"):
-            subprocess.call(["bash", os.path.join(ORACLE_DIR, "ref_alias", "build.sh")])
         if not os.path.exists(so):
             return None
         _ref = C.CDLL(so)

@@ -1,12 +1,20 @@
 """C1 -- alias-table correctness on the host (reference: Tests/TestAliasTable.cpp:14-121).
 
-Pins oracle/orc_alias.cpp against (a) the golden vector of SURVEY 8c, (b) the reference's own code
-compiled into oracle/_ref (bit-exact, including the pointer-alignment dependence of KahanSum), and
-re-states the reference's three doctest cases with fixed seeds."""
+Pins oracle/orc_alias.cpp against (a) the golden vector of SURVEY 8c, (b) the outputs of the reference's own code
+(oracle/_ref/libref_alias.so) stored in tests/golden/reference_alias.npz by tools/make_reference_golden.py (bit-exact,
+including the pointer-alignment dependence of KahanSum), and re-states the reference's three doctest cases with fixed seeds."""
 import ctypes as C
+import hashlib
+import os
 import numpy as np
 import pytest
 from tests.orc import ptr
+
+GOLDEN_REF = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_alias.npz")
+REF_SIZES = [1, 2, 6, 17, 50, 999, 13107, 100000]
+REF_PROLOGUES = [0, 3]
+REF_FULL_TABLE_MAX_N = 999      # larger tables are stored as their SHA-256
+RNG_STREAMS = (0xda3e39cb94b95bdb, 1, 12345)
 
 ENTRY = np.dtype([("P_Curr", "<f4"), ("P_Orig", "<f4"), ("Alias", "<u4")])
 GOLDEN_W = np.array([1, 22, 4, 8, 3.5, 10], dtype=np.float32)
@@ -97,48 +105,78 @@ def test_density_chi_squared(oracle, seed):
     assert chi <= 124.34211340400407
 
 
-@pytest.mark.parametrize("n", [1, 2, 6, 17, 50, 999, 13107, 100000])
-@pytest.mark.parametrize("prologue", [0, 3])
-def test_bit_exact_vs_reference(oracle, reflib, n, prologue):
-    if reflib is None:
-        pytest.skip("oracle/_ref not built (no /root/reference)")
+def ref_case_weights(n, prologue):
+    rng = np.random.default_rng(n * 7 + prologue)
+    w = (rng.random(n, dtype=np.float32) * np.float32(100.0)).astype(np.float32)
+    if n > 10:
+        w[rng.integers(0, n, size=n // 10)] = 0.0      # dead emitters
+    return w
+
+
+def reference_alias_outputs(reflib):
+    """What the reference's own code returns for the cases below; tools/make_reference_golden.py stores it."""
+    out = {}
+    for n in REF_SIZES:
+        for prologue in REF_PROLOGUES:
+            if prologue and n < prologue + 16:
+                continue
+            w = ref_case_weights(n, prologue)
+            buf = aligned(n, np.float32, prologue)
+            buf[:] = w
+            key = "n%d_p%d" % (n, prologue)
+            out[key + "_kahan"] = np.float32(reflib.ref_kahan_sum(ptr(buf), C.c_int64(n)))
+            t, _ = ref_build(reflib, w, prologue)
+            out[key + "_table"] = t if n <= REF_FULL_TABLE_MAX_N else np.array(hashlib.sha256(t.tobytes()).hexdigest())
+            idx = np.zeros(200, dtype=np.uint32); pdf = np.zeros(200, dtype=np.float32)
+            reflib.ref_alias_sample(ptr(t), C.c_int64(n), C.c_uint64(12345), 200, ptr(idx), ptr(pdf))
+            out[key + "_idx"], out[key + "_pdf"] = idx, pdf
+    for sid in RNG_STREAMS:
+        a = np.zeros(64, dtype=np.uint32)
+        reflib.ref_rng_stream(C.c_uint64(sid), 0, 0, 64, ptr(a), None)
+        out["rng_%x" % sid] = a
+    out["halton"] = np.array([[reflib.ref_halton(i, base) for base in (2, 3)] for i in range(1, 70)], dtype=np.float32)
+    return out
+
+
+@pytest.fixture(scope="module")
+def golden_ref():
+    with np.load(GOLDEN_REF) as z:
+        return {k: z[k] for k in z.files}
+
+
+@pytest.mark.parametrize("n", REF_SIZES)
+@pytest.mark.parametrize("prologue", REF_PROLOGUES)
+def test_bit_exact_vs_reference(oracle, golden_ref, n, prologue):
     if n < prologue + 16:
         # the reference's alignment prologue does not bound-check N (Common.cpp:82-90): with an
         # unaligned pointer and a short span it reads past the data -- undefined, nothing to pin
         if prologue:
             pytest.skip("reference reads out of bounds for short unaligned spans")
-    rng = np.random.default_rng(n * 7 + prologue)
-    w = (rng.random(n, dtype=np.float32) * np.float32(100.0)).astype(np.float32)
-    if n > 10:
-        w[rng.integers(0, n, size=n // 10)] = 0.0      # dead emitters
-    buf = aligned(n, np.float32, prologue)
-    buf[:] = w
-    ks_ref = reflib.ref_kahan_sum(ptr(buf), C.c_int64(n))
+    w = ref_case_weights(n, prologue)
+    key = "n%d_p%d" % (n, prologue)
     ks_orc = oracle.orc_kahan_sum(ptr(w.copy()), C.c_int64(n), prologue)
-    assert np.float32(ks_ref).tobytes() == np.float32(ks_orc).tobytes()
-    t_ref, w_ref = ref_build(reflib, w, prologue)
+    assert golden_ref[key + "_kahan"].tobytes() == np.float32(ks_orc).tobytes()
     t_orc, w_orc = orc_build(oracle, w, prologue)
-    assert (t_ref["Alias"] == t_orc["Alias"]).all()
-    assert t_ref["P_Curr"].tobytes() == t_orc["P_Curr"].tobytes()
-    assert t_ref["P_Orig"].tobytes() == t_orc["P_Orig"].tobytes()
-    idx_r = np.zeros(200, dtype=np.uint32); pdf_r = np.zeros(200, dtype=np.float32)
+    t_ref = golden_ref[key + "_table"]
+    if t_ref.dtype.kind == "U":
+        assert hashlib.sha256(t_orc.tobytes()).hexdigest() == str(t_ref)
+    else:
+        assert (t_ref["Alias"] == t_orc["Alias"]).all()
+        assert t_ref["P_Curr"].tobytes() == t_orc["P_Curr"].tobytes()
+        assert t_ref["P_Orig"].tobytes() == t_orc["P_Orig"].tobytes()
     idx_o = np.zeros(200, dtype=np.uint32); pdf_o = np.zeros(200, dtype=np.float32)
-    reflib.ref_alias_sample(ptr(t_ref), C.c_int64(n), C.c_uint64(12345), 200, ptr(idx_r), ptr(pdf_r))
     oracle.orc_alias_sample(ptr(t_orc), C.c_int64(n), C.c_uint64(12345), 200, ptr(idx_o), ptr(pdf_o))
-    assert (idx_r == idx_o).all() and pdf_r.tobytes() == pdf_o.tobytes()
+    assert (golden_ref[key + "_idx"] == idx_o).all() and golden_ref[key + "_pdf"].tobytes() == pdf_o.tobytes()
 
 
-def test_rng_and_halton_vs_reference(oracle, reflib):
-    if reflib is None:
-        pytest.skip("oracle/_ref not built (no /root/reference)")
-    for sid in (0xda3e39cb94b95bdb, 1, 12345):
-        a = np.zeros(64, dtype=np.uint32); b = np.zeros(64, dtype=np.uint32)
-        reflib.ref_rng_stream(C.c_uint64(sid), 0, 0, 64, ptr(a), None)
+def test_rng_and_halton_vs_reference(oracle, golden_ref):
+    for sid in RNG_STREAMS:
+        b = np.zeros(64, dtype=np.uint32)
         oracle.orc_rng64_stream(C.c_uint64(sid), 0, 0, 64, ptr(b), None)
-        assert (a == b).all()
+        assert (golden_ref["rng_%x" % sid] == b).all()
     for i in range(1, 70):
-        for base in (2, 3):
-            assert np.float32(reflib.ref_halton(i, base)).tobytes() == np.float32(oracle.orc_halton(i, base)).tobytes()
+        for j, base in enumerate((2, 3)):
+            assert golden_ref["halton"][i - 1, j].tobytes() == np.float32(oracle.orc_halton(i, base)).tobytes()
 
 
 def test_emissive_table_consistent_with_twin(oracle):

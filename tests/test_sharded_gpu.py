@@ -1,6 +1,6 @@
 """Strip-sharded frames on 2+ GPUs (one process per GPU, NCCL): every frame, each rank's strip of every pass output is
 byte-identical to the same rows of an unsharded render of the same frame on the same GPU, and the gathered image is
-the unsharded image. Needs >= 2 visible GPUs (`gpurun --gpus 2`); skipped on a 1-GPU box."""
+the unsharded image. Needs >= 2 visible GPUs; skipped on a 1-GPU machine."""
 import ctypes as C
 import os
 import socket

@@ -1,6 +1,6 @@
-"""In-tree build of libzetaray_b200.so for sm_100a (nvcc cross-compiles without a GPU).
+"""In-tree build of libzetaray_b200.so for sm_90a (H100) (nvcc cross-compiles without a GPU).
 
-    python -m zetaray_b200.build [--force]
+    python zetaray_b200/build.py [--force]
 
 Every .cu under zetaray_b200/csrc is compiled to an object (in parallel) and linked into
 zetaray_b200/libzetaray_b200.so next to this file, so the binary travels with the repo snapshot."""
@@ -12,16 +12,17 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # ZR_VARIANT=<name> ZR_EXTRA_FLAGS="-D..." builds an experimental libzetaray_b200_<name>.so beside the default one
-# (selected at run time with ZETARAY_B200_LIB); used for A/B measurements on the GPU box.
+# (selected at run time with ZETARAY_B200_LIB); used for A/B measurements.
 VARIANT = os.environ.get("ZR_VARIANT", "")
 OBJ = os.path.join(HERE, "build" + ("_" + VARIANT if VARIANT else ""))
 SO = os.path.join(HERE, "libzetaray_b200%s.so" % ("_" + VARIANT if VARIANT else ""))
-NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+NVCC = os.environ.get("NVCC", os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc"))
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 # -fmad=false / -ffp-contract=off: the numeric contract (DESIGN.md) -- fused multiply-adds appear only
 # where the code says fmaf(), exactly like the CPU oracle, so results are bit-comparable.
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    *GENCODE, "-lineinfo", "-O3", "-std=c++17",
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",
     "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=hidden,-O2",
     "-I" + os.path.join(os.path.dirname(HERE), "include"),
@@ -59,7 +60,7 @@ def build(force=False, verbose=True):
     objs = [o for o, _ in res]
     changed = any(c for _, c in res)
     if changed or not os.path.exists(SO):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", SO] + objs + ["-lcudart"]
+        cmd = [NVCC, "-shared", *GENCODE, "-o", SO] + objs + ["-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

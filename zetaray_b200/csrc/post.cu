@@ -4,7 +4,7 @@
 // TAA/TAA.hlsl:29-189 (+ Common.hlsli:65-102 Catmull-Rom history fetch) and their host passes
 // (Compositing.cpp:83-145, TAA.cpp:87-123).
 //
-// B200 notes: these kernels move bytes and nothing else. Compositing is elementwise, so when the
+// Notes: these kernels move bytes and nothing else. Compositing is elementwise, so when the
 // firefly filter is on it is fused into the 3x3 stencil (each tap recomposites from the two lighting
 // images; the neighbour taps are L1/L2 hits) which removes one 16 B/px write + one 16 B/px read of
 // the reference's two-dispatch sequence. The filter writes a second image instead of filtering in
@@ -267,7 +267,7 @@ namespace
     // TAA.hlsl:29-189. A block owns 32 x 8 pixels. The 3 x 3 neighbourhood is staged once per tile: every pixel of the 34 x 10 halo'd tile is
     // clamped to >= 0 and gets its tone-mapping weight 1 / (1 + luminance) ONCE (the per-tap form costs eight IEEE divisions per output
     // pixel), depth beside it; the taps then run out of shared memory in the reference's order with the reference's arithmetic.
-    // 5 blocks per SM = 48 registers: measured against 62 (4 blocks) and 40 (6 blocks), profiles/r2v_occupancy_ab.json
+    // 5 blocks per SM = 48 registers, chosen over 62 (4 blocks) and 40 (6 blocks)
     __global__ void __launch_bounds__(256, 5) k_taa(const float* __restrict__ depthPlane,
         const uint2* __restrict__ motionEmissive, const float4* __restrict__ signal,
         const uint2* __restrict__ prevOut, uint2* __restrict__ out, PostParams p)

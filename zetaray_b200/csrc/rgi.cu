@@ -13,11 +13,10 @@
 // temporal resampling.
 // D3D semantics kept: FindTemporalCandidate does not reject negative tap coordinates and out-of-bounds texture reads
 // return 0, so LoadPrev / the reservoir readers return zeros there.
-// Measured on B200 (profiles/r1e_ab_degenerate_ray.json): with the degenerate-ray cut of zr_scene.cuh::Traverse compiled into THIS
-// translation unit -- in either formulation, empty stack or early return -- ptxas lays k_rgi out so that warps run the traversal with
-// 6.9 instead of 12.4 active lanes (30.0 G instead of 16.7 G warp instructions, 116 ms instead of 60 ms on the 300 k-triangle atrium),
-// although the atrium's ReSTIR GI frame contains no degenerate ray at all. The other kernels are unaffected and the path tracer needs
-// the cut (3.5 s -> 0.12 s on the tunnel), so only this unit opts out. Cost: a zero-direction ray (2-3 per 14 400 pixels on scenes with glass) sweeps the tree here.
+// With the degenerate-ray cut of zr_scene.cuh::Traverse compiled into THIS translation unit -- in either formulation, empty stack or
+// early return -- ptxas has been seen to lay k_rgi out so that warps run the traversal with about half the active lanes, although
+// the atrium's ReSTIR GI frame contains no degenerate ray at all. The other kernels are unaffected and the path tracer needs the
+// cut (a zero-direction ray otherwise sweeps the whole tree), so only this unit opts out. Cost: a zero-direction ray (2-3 per 14 400 pixels on scenes with glass) sweeps the tree here.
 #define ZR_NO_DEGENERATE_RAY_EARLY_OUT
 #include "zr_pixel.cuh"
 #include "zr_rpt.cuh"       // ZR_PHASE

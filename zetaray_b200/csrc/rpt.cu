@@ -3,7 +3,7 @@
 // Replaces IndirectLighting/ReSTIR_PT/*.hlsl (24 compiled variants, IndirectLighting.h:257-289) and the
 // host sequencing of IndirectLighting.cpp:370-1025 for the emissive-light integrator.
 //
-// Dispatch structure (B200-first; the reference records 1 + 6 + 7 dispatches per frame):
+// Dispatch structure (the reference records 1 + 6 + 7 dispatches per frame):
 //   k_pathtrace        == ReSTIR_PT_PathTrace           one warp == one reference wave (16x2 pixels of a 16x8
 //                                                        group), bounce loop in lock-step so the Russian-roulette
 //                                                        wave-max is a warp max

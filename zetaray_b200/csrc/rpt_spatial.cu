@@ -418,7 +418,7 @@ zr_status SpatialQueued::Run(const SceneDev& sc, const FrameView& f, const RptPa
         const uint32_t tileRow0 = prm.rowBegin / 32, tileRow1 = (prm.rowEnd + 31) / 32;
         const uint32_t numTiles = tilesX * (tileRow1 - tileRow0);
         // A second form -- 512 threads x 2 co-resident blocks per SM, per-pixel state parked in shared memory between the phases -- was
-        // measured bit-identical and exactly as fast (profiles/r2p_merge_forms.json): the kernel waits for its global loads at 32 warps per
+        // bit-identical and no faster: the kernel waits for its global loads at 32 warps per
         // SM in either form. Removed again.
         const uint32_t grid = numTiles < (uint32_t)numSMs ? numTiles : (uint32_t)numSMs;
         ZR_PROF("k_spatial_merge", stream);

@@ -71,7 +71,7 @@ namespace
     }
 
     // 4 blocks per SM = 64 registers (84 bytes of spills): a latency-bound streaming pass gains more from 32 resident warps than it loses
-    // to the spills -- measured against 80 registers (3 blocks) and 48 (5 blocks), profiles/r2v_occupancy_ab.json
+    // to the spills -- chosen over 80 registers (3 blocks) and 48 (5 blocks)
     __global__ void __launch_bounds__(256, 4) k_temporal_merge(SceneDev sc, FrameView f, RptParams prm, zr_rpt_reservoir* __restrict__ resCurr,
         const zr_rpt_reservoir* __restrict__ resPrev, float4* __restrict__ target, float4* __restrict__ finalImg,
         const uint8_t* __restrict__ tflags, const ShiftResult* __restrict__ shiftRes)

@@ -41,7 +41,7 @@ namespace
         Reservoir r;
     };
     constexpr int PT_STATE_BYTES = 448;
-    // block size of the path-generation kernels: like k_pathtrace, 1024 threads x 1 block per SM (512 x 2 measured 20 % slower there)
+    // block size of the path-generation kernels: like k_pathtrace, 1024 threads x 1 block per SM
     constexpr int WF_THREADS = 1024, WF_MINBLOCKS = 1;
     static_assert(sizeof(PtState) <= PT_STATE_BYTES, "PtState outgrew its slot");
 

@@ -1,4 +1,4 @@
-// zr_common.cuh -- device math library of the B200 ReSTIR core.
+// zr_common.cuh -- device math library of the ReSTIR core.
 //
 // CUDA counterparts of ZetaRenderPass/Common/Math.hlsli, Sampling.hlsli and the DXGI storage
 // formats the reference relies on. Numeric contract (DESIGN.md "numerics"): IEEE ops only, HLSL

@@ -3,9 +3,10 @@
 // (zr_rpt.cuh Replay_kGt2_Sync / Shift2_Sync<CASE>) on real work. Used by the spatial pass (rpt_spatial.cu: current <-> neighbour
 // pixel of the same frame) and by the temporal pass (rpt_temporal.cu: current <-> reprojected pixel of the previous frame).
 //
-// Block size: 512 threads x 2 blocks per SM (64 registers). Measured on B200 (profiles/r2c_shift_block_size.json): 256 x 2 and 512 x 1
-// (128 registers) are 20 % slower on the Cornell frame and 17-52 % on the tunnel, 256 x 4 / 128 x 4 slower still -- the
-// block-synchronous phases want many warps behind each instruction-cache line.
+// Block size: 512 threads x 2 blocks per SM (64 registers): the block-synchronous phases want many warps behind each
+// instruction-cache line, so fewer, larger register budgets (256 x 2, 512 x 1 at 128 registers) or more, smaller blocks
+// (256 x 4, 128 x 4) trade away the wrong resource. The choice has not been re-measured on H100 (same register file and
+// thread limits per SM as the part it was tuned on).
 #pragma once
 #include "zr_rpt_spatial.h"
 

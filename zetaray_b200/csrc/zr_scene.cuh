@@ -75,10 +75,10 @@ ZR_F1 RayHit Traverse(const SceneDev& sc, float3 o, float3 d, float tmin, float 
     // Degenerate rays hit nothing under the hit rule (a zero direction makes every determinant 0, a NaN direction or origin makes
     // every barycentric NaN), but they pass every slab test below (0 * inf and NaN drop out of fminf / fmaxf), i.e. they would
     // sweep the whole tree: one such ray per ~1500 pixels comes out of the path tracer's BSDF-sampled emissive-hit query on
-    // transmissive surfaces (wi = 0 when the sampler returns pdf 0), and on a 195 k-node tree it stalled its whole 1024-thread block
-    // for tens of milliseconds (3.5 s per 4K frame of the 10^6-triangle tunnel). They start with an empty stack. One translation
+    // transmissive surfaces (wi = 0 when the sampler returns pdf 0), and such a ray holds its whole 1024-thread block
+    // for a full sweep of the tree. They start with an empty stack. One translation
     // unit, rgi.cu, opts out (ZR_NO_DEGENERATE_RAY_EARLY_OUT): with this cut compiled in -- as an empty stack or as an early return,
-    // both measured -- k_rgi runs with half the active lanes per warp (profiles/r1e_ab_degenerate_ray.json, DESIGN.md section 10).
+    // both tried -- k_rgi runs with half the active lanes per warp (see rgi.cu).
     const bool degenerate = (d.x == 0.0f && d.y == 0.0f && d.z == 0.0f) || d.x != d.x || d.y != d.y || d.z != d.z ||
         o.x != o.x || o.y != o.y || o.z != o.z;
 #if defined(ZR_DEGENERATE_RAY_RETURN)          /* A/B switches for measurements only */

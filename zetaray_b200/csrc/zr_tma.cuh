@@ -1,4 +1,4 @@
-// zr_tma.cuh -- Tensor Memory Accelerator plumbing for the streaming kernels (sm_100a).
+// zr_tma.cuh -- Tensor Memory Accelerator plumbing for the streaming kernels (sm_90a).
 //
 // Host: tensor maps over pitched 2D planes ([H][W] records of 8..64 bytes), encoded through the driver entry point
 // cuTensorMapEncodeTiled, which is fetched at run time with cudaGetDriverEntryPoint (the library links cudart only).

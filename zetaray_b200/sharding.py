@@ -260,8 +260,7 @@ class ShardedFrame:
 
     def end_cost_measurement(self, schedule=False):
         """Returns the cost of every 32-row band (for StripPlan.balanced). With schedule=True the per-tile costs also
-        become the lighting passes' block schedule (expensive tiles first; measured on B200: no gain over plain order,
-        the compact per-strip grid is what matters)."""
+        become the lighting passes' block schedule (expensive tiles first; no gain over plain order was seen, the compact per-strip grid is what matters)."""
         self.p["direct"].SetCostMap(0)
         self.p["indirect"].SetCostMap(0)
         c = self.cost.to(torch.float64)
