@@ -42,14 +42,32 @@ namespace
     // -------------------------------------------------------------------------------------------
     // PathTrace
     // -------------------------------------------------------------------------------------------
+// 768 threads at 80 registers with the parked state below (157 KB of shared memory per block). Measured on an H100 SXM (700 W):
+// 3.33 ms per bench frame, against 3.65 ms at 1024 x 64 registers, 3.52 ms at 512 x 128 and 4.40 ms at 512 x 2 blocks x 64
+// (DESIGN 4.1).
 #ifndef ZR_PT_THREADS
-#define ZR_PT_THREADS 1024
+#define ZR_PT_THREADS 768
 #endif
+    // The path's cold state: the reservoir under construction and the path's own reconnection vertex. Only reservoir updates,
+    // SetCase1/2/3 and Clear touch them, yet held in registers they competed with the hot state and spilled to local memory,
+    // whose reloads go to L2 once a full SM's spill area outgrows L1. They live in dynamic shared memory, one record per
+    // thread; the record's odd number of 32-bit words puts the 32 lanes of a warp in 32 different banks.
+    struct PtParked
+    {
+        Reservoir r;
+        Reconnection rc;
+        uint32_t pad;
+    };
+    static_assert(sizeof(PtParked) % 4 == 0 && (sizeof(PtParked) / 4) % 2 == 1, "PtParked must be an odd number of words");
+    constexpr size_t PT_SMEM_BYTES = (size_t)ZR_PT_THREADS * sizeof(PtParked);
+
     // A block is ZR_PT_THREADS/128 consecutive 16x8 groups of the reference's swizzled dispatch; each warp is one
     // reference wave. The warps of a block walk the bounce phases together (zr_rpt.cuh "block-synchronous phases").
+    // Dynamic shared memory: PT_SMEM_BYTES (PtParked per thread).
     __global__ void ZR_LB(ZR_PT_THREADS) k_pathtrace(SceneDev sc, FrameView f, RptParams prm, zr_rpt_reservoir* __restrict__ res,
         float4* __restrict__ target, float4* __restrict__ finalImg, uint32_t dispX, uint32_t dispY, const uint32_t* __restrict__ order)
     {
+        extern __shared__ PtParked s_ptParked[];
         const zr_frame_constants& fc = f.fc;
         const long long t0 = clock64();
         uint2 sg = make_uint2(0, 0);
@@ -77,8 +95,10 @@ namespace
         BSDF::BSDFSample bsdfSample = BSDF::BSDFSample::Init();
         HitEmissive nextHit;
         nextHit.hit = false;
-        Reconnection rc = Reconnection::Init();
-        Reservoir r = Reservoir::Init();
+        Reconnection& rc = s_ptParked[threadIdx.x].rc;
+        Reservoir& r = s_ptParked[threadIdx.x].r;
+        rc = Reconnection::Init();
+        r = Reservoir::Init();
         PrevHit prevHit;
         prevHit.alpha_lobe = 0; prevHit.wi = f3(0); prevHit.pdf = 0; prevHit.lobe = BSDF::DIFFUSE_R;
         float eta_curr = BSDF::ETA_AIR, eta_next = BSDF::DEFAULT_ETA_MAT;
@@ -954,6 +974,20 @@ struct zr_indirect_pass
         if (st != ZR_OK) return st;
         st = wavefront.Resize(w, h);
         if (st != ZR_OK) return st;
+        // k_pathtrace's parked state needs more than the 48 KB of static shared memory. The carveout asks for just the shared
+        // memory its resident blocks use (plus the 1 KB the system reserves per block); the rest of the 256 KB stays L1 for
+        // what still spills.
+        ZR_CUDA(cudaFuncSetAttribute(zr::k_pathtrace, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zr::PT_SMEM_BYTES));
+        int ptBlocks = 0;
+        ZR_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ptBlocks, zr::k_pathtrace, ZR_PT_THREADS, zr::PT_SMEM_BYTES));
+        if (ptBlocks < 1)
+        {
+            zr::set_error("zr_indirect_pass: k_pathtrace (%d threads, %zu B shared) cannot be resident", ZR_PT_THREADS, zr::PT_SMEM_BYTES);
+            return ZR_ERR_UNSUPPORTED;
+        }
+        const size_t ptSmem = (size_t)ptBlocks * (zr::PT_SMEM_BYTES + 1024);
+        ZR_CUDA(cudaFuncSetAttribute(zr::k_pathtrace, cudaFuncAttributePreferredSharedMemoryCarveout,
+            (int)((ptSmem * 100 + 228 * 1024 - 1) / (228 * 1024))));
         return ResetTemporal();
     }
 
@@ -1057,7 +1091,7 @@ struct zr_indirect_pass
             // the lock-step kernel (also while a cost map is being measured: it accounts the cycles of its blocks per tile)
             const uint32_t dispX = (width + 15) / 16, dispY = (height + 7) / 8;
             ZR_PROF("k_pathtrace", stream);
-            k_pathtrace<<<schedPathTrace.count, ZR_PT_THREADS, 0, stream>>>(in->scene->dev, f, prm, d_res[cur], d_target, d_final, dispX, dispY,
+            k_pathtrace<<<schedPathTrace.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, d_res[cur], d_target, d_final, dispX, dispY,
                 schedPathTrace.d_order);
             ZR_LAUNCH_CHECK();
         }

@@ -3,10 +3,9 @@
 // (zr_rpt.cuh Replay_kGt2_Sync / Shift2_Sync<CASE>) on real work. Used by the spatial pass (rpt_spatial.cu: current <-> neighbour
 // pixel of the same frame) and by the temporal pass (rpt_temporal.cu: current <-> reprojected pixel of the previous frame).
 //
-// Block size: 512 threads x 2 blocks per SM (64 registers): the block-synchronous phases want many warps behind each
-// instruction-cache line, so fewer, larger register budgets (256 x 2, 512 x 1 at 128 registers) or more, smaller blocks
-// (256 x 4, 128 x 4) trade away the wrong resource. The choice has not been re-measured on H100 (same register file and
-// thread limits per SM as the part it was tuned on).
+// Block size: 512 threads x 1 block per SM (128 registers). At 64 registers the replay classes spill ~1 KB per thread, more
+// than L1 holds at a full SM. Measured on an H100 SXM (700 W), spatial + temporal shift per bench frame: 0.88 + 0.78 ms at
+// 512 x 1, 0.87 + 0.85 at 768 x 1 (80 registers), 0.96 + 0.83 at 512 x 2 (64 registers), 0.99 + 0.87 at 1024 x 1 (DESIGN 4.1).
 #pragma once
 #include "zr_rpt_spatial.h"
 
@@ -15,7 +14,13 @@ namespace zr
 namespace
 {
     using namespace RPT;
-    constexpr int SHIFT_THREADS = 512, SHIFT_MINBLOCKS = 2;
+#ifndef ZR_SHIFT_THREADS
+#define ZR_SHIFT_THREADS 512
+#endif
+#ifndef ZR_SHIFT_MINBLOCKS
+#define ZR_SHIFT_MINBLOCKS 1
+#endif
+    constexpr int SHIFT_THREADS = ZR_SHIFT_THREADS, SHIFT_MINBLOCKS = ZR_SHIFT_MINBLOCKS;
     constexpr uint32_t NO_ITEM = 0xffffffffu;
 
     // queue class of a reservoir's sample from its metadata word: (case 1, 2, 3) x (k == 2, k > 2)
