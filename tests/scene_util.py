@@ -69,6 +69,70 @@ SCENES = {"cornell": cornell, "glossy": glossy_cornell, "glass": glass_cornell, 
 CAMERAS = {"atrium": (0.0, 1.7, -13.0), "atrium_lights": (0.0, 1.7, -13.0), "tunnel": (-1.6, 1.7, -4.0)}
 
 
+# ---- radiometric truth scenes (oracle/indep_radiometry.py) ----------------------------------------------------------------------
+# Every surface is an axis-aligned rectangle {p0, eu, ev, nu x nv cells}: a point is p0 + s eu + t ev, s, t in [0, 1], and
+# cross(eu, ev) is the side the vertex normals (and an emitter's emission) face. Material parameters are k / 255 so that the
+# 8-bit material and G-buffer encodings reproduce them exactly; emitter edges are dyadic and each triangle's two edges from its
+# first vertex run along eu and ev, so the emissive record's half-precision lengths are exact.
+def _k(v):
+    return tuple(float(np.float32(round(x * 255) / 255)) for x in v) if isinstance(v, tuple) else float(np.float32(round(v * 255) / 255))
+
+
+DIFFUSE = dict(base_color=_k((0.6, 0.6, 0.6)), roughness=1.0, double_sided=True)
+GLOSSY_ROUGH = dict(base_color=_k((0.5, 0.6, 0.7)), roughness=_k(0.5), double_sided=True)        # alpha 0.25: above both alpha_min
+GLOSSY_MID = dict(base_color=_k((0.7, 0.6, 0.5)), roughness=_k(0.12), double_sided=True)         # alpha (31/255)^2 = 0.0148: DI 0.0025 < alpha < PT 0.0306
+METAL = dict(base_color=_k((0.95, 0.64, 0.54)), metallic=1.0, roughness=_k(0.3), double_sided=True)
+COATED = dict(base_color=_k((0.2, 0.3, 0.7)), roughness=_k(0.6), coat_weight=1.0, coat_roughness=_k(0.1), coat_color=_k((0.9, 0.9, 0.9)),
+              coat_ior=1.6, double_sided=True)
+
+
+def _emitter(rgb, strength, double_sided=False):
+    return dict(base_color=(0, 0, 0), roughness=1.0, emissive_factor=_k(rgb), emissive_strength=strength, double_sided=double_sided)
+
+
+TRUTH_SCENES = {
+    # floor rough diffuse, back wall glossy; a one-sided light facing down (the wall above its plane sees only its back), a
+    # double-sided vertical light, and an occluder between the first light and the floor (umbra + penumbra)
+    "truth_a": [
+        dict(name="floor", p0=(-4, 0, -3), eu=(0, 0, 9), ev=(8, 0, 0), mat=DIFFUSE),
+        dict(name="wall", p0=(-4, 0, 3), eu=(0, 4, 0), ev=(8, 0, 0), mat=GLOSSY_ROUGH),
+        dict(name="light_down", p0=(-1.25, 2, 0.5), eu=(1, 0, 0), ev=(0, 0, 0.5), mat=_emitter((1.0, 0.9, 0.8), 8.0)),
+        dict(name="light_side", p0=(2, 0.5, 1), eu=(0, 0, 1), ev=(0, 1, 0), mat=_emitter((0.6, 0.8, 1.0), 2.0, double_sided=True)),
+        dict(name="occluder", p0=(-1.0, 1, 0.25), eu=(0, 0, 1), ev=(0.5, 0, 0), mat=DIFFUSE),
+    ],
+    # glossy floor (alpha between the two alpha_min), coated back wall, metal side wall; a 256-triangle dim panel and a small
+    # strong light: per-triangle powers differ by ~190x, so the alias table is far from uniform
+    "truth_b": [
+        dict(name="floor", p0=(-4, 0, -3), eu=(0, 0, 9), ev=(8, 0, 0), mat=GLOSSY_MID),
+        dict(name="wall", p0=(-4, 0, 3), eu=(0, 4, 0), ev=(8, 0, 0), mat=COATED),
+        dict(name="side", p0=(-3, 0, -3), eu=(0, 4, 0), ev=(0, 0, 6), mat=METAL),
+        dict(name="panel", p0=(0.5, 2.5, 1), eu=(2, 0, 0), ev=(0, 0, 1), nu=16, nv=8, mat=_emitter((1.0, 1.0, 1.0), 1.0)),
+        dict(name="light_small", p0=(-1.5, 1.5, 0), eu=(0.5, 0, 0), ev=(0, 0, 0.5), mat=_emitter((1.0, 0.7, 0.4), 16.0)),
+    ],
+}
+
+
+def truth_scene(name):
+    """Builds TRUTH_SCENES[name] with SceneBuilder; returns (FlatScene, the description)."""
+    desc = TRUTH_SCENES[name]
+    b = zscene.SceneBuilder()
+    for r in desc:
+        p0, eu, ev = (np.asarray(r[k], dtype=np.float64) for k in ("p0", "eu", "ev"))
+        nu, nv = r.get("nu", 1), r.get("nv", 1)
+        n = np.cross(eu, ev); n /= np.linalg.norm(n)
+        s, t = np.meshgrid(np.arange(nu + 1) / nu, np.arange(nv + 1) / nv, indexing="ij")
+        pos = p0 + s.reshape(-1, 1) * eu + t.reshape(-1, 1) * ev
+        uv = np.stack([s.reshape(-1), t.reshape(-1)], axis=1)
+        vid = lambda i, j: i * (nv + 1) + j
+        idx = []
+        for i in range(nu):
+            for j in range(nv):
+                # (c00, c10, c01) and (c11, c01, c10): both triangles' edges from vertex 0 run along +-eu / +-ev
+                idx += [vid(i, j), vid(i + 1, j), vid(i, j + 1), vid(i + 1, j + 1), vid(i, j + 1), vid(i + 1, j)]
+        b.add_mesh(pos, np.tile(n, (len(pos), 1)), uv, idx, b.add_material(zscene.make_material(**r["mat"])))
+    return b.finish(), desc
+
+
 _RHO_LUT = None
 
 
