@@ -48,7 +48,8 @@ ZR_API const char* zr_last_error(void);
 /* Library/ABI version: (major << 16) | minor. */
 /* (major << 16) | minor; additions bump the minor. 1.1 added zr_bvh_build_host, zr_renderer_set_integrator,
  * zr_renderer_get_gi_pass, zr_renderer_apply_scene_settings and zr_gi_pass_set_method; 1.2 the SVGF pass, zr_comm, the strip-sharded
- * renderer (zr_renderer_set_shard) and zr_gi_pass_set_rows / set_halo_exchange. */
+ * renderer (zr_renderer_set_shard) and zr_gi_pass_set_rows / set_halo_exchange. 1.3 removed two
+ * measurement and test hooks: the ReSTIR PT execution-model switch and the two-dispatch compositing entry point. */
 ZR_API uint32_t zr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -471,16 +472,7 @@ typedef enum zr_indirect_stage
 {
     ZR_RPT_STAGE_ALL = 0, ZR_RPT_STAGE_PATHTRACE = 1, ZR_RPT_STAGE_TEMPORAL = 2, ZR_RPT_STAGE_SPATIAL = 3
 } zr_indirect_stage;
-/* execution model of the pass (same results in every mode):
- *   QUEUED (default)  lock-step path generation (k_pathtrace) + temporal and spatial reuse through per-case shift queues and the
- *                     TMA-staged streaming merge
- *   FUSED             round 1: k_pathtrace + fused k_temporal / k_spatial (both shifts and the merge inline per pixel)
- *   WAVEFRONT         QUEUED, but path generation as one launch per bounce over a compacted queue of live paths (rpt_wavefront.cu);
- *                     measured slower than k_pathtrace on every scene (DESIGN.md 4.1c), kept for measurement
- * ZETARAY_B200_SPATIAL=fused|queued|wavefront sets the initial value. */
-typedef enum zr_indirect_execution { ZR_RPT_EXEC_FUSED = 0, ZR_RPT_EXEC_QUEUED = 1, ZR_RPT_EXEC_WAVEFRONT = 2 } zr_indirect_execution;
 ZR_API zr_status zr_indirect_pass_create(uint32_t width, uint32_t height, zr_indirect_pass** out);
-ZR_API zr_status zr_indirect_pass_set_execution(zr_indirect_pass* p, zr_indirect_execution mode);
 ZR_API zr_status zr_indirect_pass_resize(zr_indirect_pass* p, uint32_t width, uint32_t height);
 ZR_API zr_status zr_indirect_pass_reset_temporal(zr_indirect_pass* p);
 ZR_API zr_status zr_indirect_pass_default_params(zr_indirect_params* out);
@@ -548,10 +540,6 @@ ZR_API zr_status zr_compositing_pass_resize(zr_compositing_pass* p, uint32_t wid
 ZR_API zr_status zr_compositing_pass_set_params(zr_compositing_pass* p, const zr_compositing_params* params);
 /* d_direct / d_indirect: float4[w*h] (outputs of the lighting passes) or NULL */
 ZR_API zr_status zr_compositing_pass_render(zr_compositing_pass* p, const zr_frame_inputs* in,
-    const void* d_direct, const void* d_indirect, void* stream);
-/* the reference's two-dispatch sequence (compositing, then firefly on the stored image); the default
- * render() fuses both -- kept so tests can check the fusion changes nothing */
-ZR_API zr_status zr_compositing_pass_render_unfused(zr_compositing_pass* p, const zr_frame_inputs* in,
     const void* d_direct, const void* d_indirect, void* stream);
 ZR_API zr_status zr_compositing_pass_set_rows(zr_compositing_pass* p, uint32_t y0, uint32_t y1);
 ZR_API zr_status zr_compositing_pass_get_output(zr_compositing_pass* p, zr_image2d* out);

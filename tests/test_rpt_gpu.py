@@ -1,7 +1,7 @@
 """ReSTIR PT on the device vs the CPU oracle, frame by frame (bit-exact integer state AND radiance).
 
 Covers: initial path generation (frame 1), temporal reuse (frame 2+), spatial search, the StC thread map,
-fused CtS+StC spatial reuse with boiling suppression, ping-pong bookkeeping over several frames, on the
+CtS+StC spatial reuse with boiling suppression, ping-pong bookkeeping over several frames, on the
 Cornell box (k == 2 everywhere) and on the glossy variant (k > 2 replay, case 3, metals, coat)."""
 import ctypes as C
 import numpy as np
@@ -26,7 +26,7 @@ def _diff_report(name, a, b, fields=None):
     return "%s differs at %d/%d entries; first idx %d got %s want %s" % (name, len(d), len(a), d[0], a[d[0]], b[d[0]])
 
 
-def _run(which, w, h, nframes, params=None, jitter=True, dof=False, dump=None, cam_path=None, accumulate=False, presample=None, execution=None):
+def _run(which, w, h, nframes, params=None, jitter=True, dof=False, dump=None, cam_path=None, accumulate=False, presample=None):
     import torch
     from zetaray_b200 import lib, check, _lib
     from zetaray_b200.passes import Scene, GBuffers, GBufferRT, IndirectLighting, download_image
@@ -41,8 +41,6 @@ def _run(which, w, h, nframes, params=None, jitter=True, dof=False, dump=None, c
     gb = GBuffers(w, h)
     gpass = GBufferRT()
     ind = IndirectLighting(w, h)
-    if execution is not None:
-        ind.SetExecution(execution)
     if params:
         for k, v in params.items():
             setattr(R.params, k, v)
@@ -133,11 +131,18 @@ def test_rpt_glass_scene():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("which", ["glossy", "glass"])
-def test_rpt_moving_camera(which):
+@pytest.mark.parametrize("which,w,h,nframes,params", [
+    pytest.param("glossy", 320, 180, 5, None, id="glossy"),
+    pytest.param("glass", 320, 180, 5, None, id="glass"),
+    # odd size: partial 16x8 groups and 32x32 sort tiles at the right and bottom edges
+    pytest.param("glossy", 333, 187, 3, None, id="glossy-333-187"),
+    # 6 bounces so that the wave-wide Russian roulette runs on long transmissive paths, two spatial passes
+    pytest.param("glass", 256, 144, 4, dict(max_non_tr_bounces=5, max_glossy_tr_bounces=6, num_spatial_passes=2), id="glass-6-bounces"),
+])
+def test_rpt_moving_camera(which, w, h, nframes, params):
     # a translating camera: non-zero motion vectors, reprojection into other pixels, disocclusions at the box edges
     path = lambda f: (0.03 * f, 1.2 + 0.02 * f, -4.043 + 0.05 * f)
-    problems, _ = _run(which, 320, 180, 5, cam_path=path)
+    problems, _ = _run(which, w, h, nframes, params=params, cam_path=path)
     assert not problems, "\n".join(problems)
 
 
@@ -146,19 +151,6 @@ def test_rpt_accumulate_and_two_spatial_passes():
     problems, _ = _run("glossy", 256, 144, 4, accumulate=True)
     assert not problems, "\n".join(problems)
     problems, _ = _run("cornell", 256, 144, 4, params=dict(num_spatial_passes=2))
-    assert not problems, "\n".join(problems)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("execution", [0, 2])
-def test_rpt_execution_models_agree_with_the_oracle(execution):
-    # the default (queued reuse passes) runs in every other test; here the round-1 fused kernels (0) and wavefront path generation
-    # (2): glass + 6 bounces so that the wave-wide Russian roulette crosses the launch boundary, two spatial passes, moving camera
-    path = lambda f: (0.03 * f, 1.2 + 0.02 * f, -4.043 + 0.05 * f)
-    problems, _ = _run("glass", 256, 144, 4, params=dict(max_non_tr_bounces=5, max_glossy_tr_bounces=6, num_spatial_passes=2),
-                       cam_path=path, execution=execution)
-    assert not problems, "\n".join(problems)
-    problems, _ = _run("glossy", 333, 187, 3, execution=execution)
     assert not problems, "\n".join(problems)
 
 

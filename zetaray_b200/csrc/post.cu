@@ -56,68 +56,15 @@ namespace
         out[i] = f4(c.x, c.y, c.z, 0.0f);
     }
 
-    // Firefly filter over an image produced by `Load` (either a stored composited image or the
-    // on-the-fly composite).
-    template<bool Fused>
-    __global__ void __launch_bounds__(256) k_firefly(const uint4* __restrict__ core, const float* __restrict__ depth,
-        const float4* __restrict__ inOrDirect, const float4* __restrict__ indirect, float4* __restrict__ out,
-        PostParams p)
-    {
-        const int x = blockIdx.x * 32 + (threadIdx.x & 31);
-        const int y = (int)p.rowBegin + blockIdx.y * 8 + (threadIdx.x >> 5);
-        const int W = (int)p.W, H = (int)p.H;
-        if (x >= W || y >= (int)p.rowEnd) return;
-        const size_t idx = (size_t)y * W + x;
-        auto load = [&](size_t i) -> float3 {
-            if (Fused)
-                return composite_px(core, inOrDirect, indirect, i, p);
-            float4 c = __ldg(&inOrDirect[i]);
-            return f3(c.x, c.y, c.z);
-        };
-        const float z_view = __ldg(&depth[idx]);
-        const float3 currColor = load(idx);
-        if (z_view == FLT_MAX_)
-        {
-            out[idx] = f4(currColor.x, currColor.y, currColor.z, 0.0f);
-            return;
-        }
-        float minLum = FLT_MAX_;
-        float maxLum = 0.0f;
-        float3 minColor = currColor;
-        float3 maxColor = f3(0);
-        const float currLum = Math::Luminance(currColor);
-#pragma unroll
-        for (int i = -1; i <= 1; i++)
-        {
-#pragma unroll
-            for (int j = -1; j <= 1; j++)
-            {
-                if (i == 0 && j == 0) continue;
-                const int ax = x + j, ay = y + i;
-                if ((uint32_t)ax >= (uint32_t)W || (uint32_t)ay >= (uint32_t)H) continue;
-                const size_t n = (size_t)ay * W + ax;
-                if (__ldg(&depth[n]) == FLT_MAX_) continue;
-                const float3 neighborColor = load(n);
-                const float neighborLum = Math::Luminance(neighborColor);
-                if (neighborLum < minLum) { minLum = neighborLum; minColor = neighborColor; }
-                else if (neighborLum > maxLum) { maxLum = neighborLum; maxColor = neighborColor; }
-            }
-        }
-        float3 ret = currLum < minLum ? minColor : (currLum > maxLum ? maxColor : currColor);
-        ret = minLum <= maxLum ? ret : currColor;
-        out[idx] = f4(ret.x, ret.y, ret.z, 0.0f);
-    }
-
-    // Shared-memory-tiled form of the fused compositing + firefly stencil (the product path; k_firefly above stays as the
-    // reference-shaped two-dispatch sequence the tests compare it with). A block owns a 32 x 16 pixel tile: every pixel
-    // of the 34 x 18 halo'd tile is composited ONCE (1.2 composites per output pixel instead of 9 -- the untiled kernel
+    // Shared-memory-tiled fused compositing + firefly stencil. A block owns a 32 x 16 pixel tile: every pixel
+    // of the 34 x 18 halo'd tile is composited ONCE (1.2 composites per output pixel instead of 9 -- an untiled kernel
     // re-composites each tap, 27 IEEE divisions per pixel, and is issue-bound, not bandwidth-bound), its luminance and
     // "has geometry" flag are staged next to it, and the 3 x 3 min / max search then runs out of shared memory in the
-    // same tap order, so the result is bit-identical. Rows are read as contiguous 34-pixel segments (coalesced 128-bit loads).
+    // reference's tap order, so the result is bit-identical to the oracle. Rows are read as contiguous 34-pixel segments
+    // (coalesced 128-bit loads).
     constexpr int FF_TW = 32, FF_TH = 16, FF_SW = FF_TW + 2, FF_SH = FF_TH + 2;
-    template<bool Fused>
     __global__ void __launch_bounds__(FF_TW * FF_TH) k_firefly_tiled(const uint4* __restrict__ core, const float* __restrict__ depth,
-        const float4* __restrict__ inOrDirect, const float4* __restrict__ indirect, float4* __restrict__ out, PostParams p)
+        const float4* __restrict__ direct, const float4* __restrict__ indirect, float4* __restrict__ out, PostParams p)
     {
         __shared__ float4 tile[FF_SH][FF_SW];           // xyz = (composited) colour, w = its luminance
         __shared__ uint8_t geom[FF_SH][FF_SW];          // 1 = inside the image and depth != FLT_MAX
@@ -133,14 +80,7 @@ namespace
             if ((uint32_t)gx < (uint32_t)W && (uint32_t)gy < (uint32_t)H)
             {
                 const size_t i = (size_t)gy * W + gx;
-                float3 c;
-                if (Fused)
-                    c = composite_px(core, inOrDirect, indirect, i, p);
-                else
-                {
-                    const float4 c4 = __ldg(&inOrDirect[i]);
-                    c = f3(c4.x, c4.y, c4.z);
-                }
+                const float3 c = composite_px(core, direct, indirect, i, p);
                 v = f4(c.x, c.y, c.z, Math::Luminance(c));
                 g = __ldg(&depth[i]) != FLT_MAX_ ? 1 : 0;
             }
@@ -383,8 +323,7 @@ struct zr_compositing_pass
 {
     // Compositing (Compositing/Compositing.h): owns the LIGHT_ACCUM image (RGBA32F)
     uint32_t width = 0, height = 0;
-    float4* d_composited = nullptr;     // output of compositing (and of the fused firefly variant)
-    float4* d_scratch = nullptr;        // unfused path: compositing result before the filter
+    float4* d_composited = nullptr;     // output of compositing (fused with the firefly filter when it is on)
     zr_compositing_params params{ 1, 1, 1 };
     uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
     void SetRows(zr::PostParams& p, dim3& grid) const
@@ -399,14 +338,12 @@ struct zr_compositing_pass
         Release();
         width = w; height = h;
         ZR_CUDA(cudaMalloc(&d_composited, (size_t)w * h * sizeof(float4)));
-        ZR_CUDA(cudaMalloc(&d_scratch, (size_t)w * h * sizeof(float4)));
         return ZR_OK;
     }
     void Release()
     {
         if (d_composited) cudaFree(d_composited);
-        if (d_scratch) cudaFree(d_scratch);
-        d_composited = d_scratch = nullptr;
+        d_composited = nullptr;
     }
     zr_status Render(const zr_frame_inputs* in, const void* d_direct, const void* d_indirect, cudaStream_t stream)
     {
@@ -431,7 +368,7 @@ struct zr_compositing_pass
         {
             const dim3 tgrid((width + FF_TW - 1) / FF_TW, (p.rowEnd - p.rowBegin + FF_TH - 1) / FF_TH);
             ZR_PROF("k_firefly", stream);
-            k_firefly_tiled<true><<<tgrid, FF_TW * FF_TH, 0, stream>>>((const uint4*)in->curr.d_core, (const float*)in->curr.d_depth,
+            k_firefly_tiled<<<tgrid, FF_TW * FF_TH, 0, stream>>>((const uint4*)in->curr.d_core, (const float*)in->curr.d_depth,
                 direct, indirect, d_composited, p);
             ZR_LAUNCH_CHECK();
         }
@@ -441,23 +378,6 @@ struct zr_compositing_pass
             k_compositing<<<grid, 256, 0, stream>>>((const uint4*)in->curr.d_core, direct, indirect, d_composited, p);
             ZR_LAUNCH_CHECK();
         }
-        return ZR_OK;
-    }
-    // reference-shaped two-dispatch sequence (used by tests to check the fusion)
-    zr_status RenderUnfused(const zr_frame_inputs* in, const void* d_direct, const void* d_indirect, cudaStream_t stream)
-    {
-        using namespace zr;
-        PostParams p = make_params(in->frame);
-        dim3 grid;
-        SetRows(p, grid);
-        ZR_PROF("k_compositing", stream);
-        k_compositing<<<grid, 256, 0, stream>>>((const uint4*)in->curr.d_core, (const float4*)d_direct,
-            (const float4*)d_indirect, d_scratch, p);
-        ZR_LAUNCH_CHECK();
-        ZR_PROF("k_firefly", stream);
-        k_firefly<false><<<grid, 256, 0, stream>>>((const uint4*)in->curr.d_core, (const float*)in->curr.d_depth,
-            d_scratch, nullptr, d_composited, p);
-        ZR_LAUNCH_CHECK();
         return ZR_OK;
     }
 };
@@ -545,12 +465,6 @@ extern "C"
     {
         if (!p) return ZR_ERR_INVALID_ARG;
         return p->Render(in, d_direct, d_indirect, (cudaStream_t)stream);
-    }
-    zr_status zr_compositing_pass_render_unfused(zr_compositing_pass* p, const zr_frame_inputs* in, const void* d_direct,
-        const void* d_indirect, void* stream)
-    {
-        if (!p) return ZR_ERR_INVALID_ARG;
-        return p->RenderUnfused(in, d_direct, d_indirect, (cudaStream_t)stream);
     }
     zr_status zr_compositing_pass_set_rows(zr_compositing_pass* p, uint32_t y0, uint32_t y1)
     {

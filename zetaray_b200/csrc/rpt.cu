@@ -7,13 +7,13 @@
 //   k_pathtrace        == ReSTIR_PT_PathTrace           one warp == one reference wave (16x2 pixels of a 16x8
 //                                                        group), bounce loop in lock-step so the Russian-roulette
 //                                                        wave-max is a warp max
-//   k_temporal         == Sort x2 + Replay x2 + Reconnect_CtT + Reconnect_TtC fused. None of them has a
-//                         wave-scope op, so the sorted thread maps cannot change results: the kernel runs in
-//                         pixel order and keeps the replay context and the CtT-scaled w_sum in registers.
+//   temporal reuse     == Sort x2 + Replay x2 + Reconnect_CtT + Reconnect_TtC: classify -> per-case shift queues -> merge
+//                         (rpt_temporal.cu). None of them has a wave-scope op, so the sorted thread maps cannot change results.
 //   k_spatial_search   == ReSTIR_PT_SpatialSearch
 //   k_sort             == ReSTIR_PT_Sort (only the StC map is needed: it defines which 32 pixels share the
 //                         boiling-suppression wave sums)
-//   k_spatial          == Replay x2 + Reconnect_CtS + Reconnect_StC fused, run in the StC-sorted order
+//   spatial reuse      == Replay x2 + Reconnect_CtS + Reconnect_StC: classify -> per-case shift queues -> merge in the
+//                         StC-sorted order (rpt_spatial.cu)
 // Per-pixel state moves as 128-bit accesses: 64-byte reservoir records, float4 target/final, uint4 G-buffer.
 #include "zr_rpt_io.cuh"
 #include "zr_rpt_spatial.h"
@@ -327,186 +327,6 @@ namespace
     }
 
     // -------------------------------------------------------------------------------------------
-    // Temporal reuse: Reconnect_CtT then Reconnect_TtC for the same pixel (replay inline).
-    // A block is 32 x ZR_RPT_THREADS/32 pixels, one warp per 8x4 tile; block-synchronous phases throughout,
-    // so no thread leaves before the last barrier.
-    // -------------------------------------------------------------------------------------------
-#ifndef ZR_RPT_THREADS
-#define ZR_RPT_THREADS 1024
-#endif
-    __global__ void ZR_LB(ZR_RPT_THREADS) k_temporal(SceneDev sc, FrameView f, RptParams prm, zr_rpt_reservoir* __restrict__ resCurr,
-        const zr_rpt_reservoir* __restrict__ resPrev, float4* __restrict__ target, float4* __restrict__ finalImg,
-        uint32_t gridX, const uint32_t* __restrict__ order)
-    {
-        const zr_frame_constants& fc = f.fc;
-        const long long t0 = clock64();
-        const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        const uint32_t bid = order[blockIdx.x];
-        const int x = (int)((bid % gridX) * 32 + (warp & 3) * 8 + (lane & 7));
-        const int y = (int)((bid / gridX) * (ZR_RPT_THREADS / 32) + (warp >> 2) * 4 + (lane >> 3));
-        bool act = !(x >= (int)f.W || y >= (int)f.H || y < (int)prm.rowBegin || y >= (int)prm.rowEnd);
-        const size_t idx = act ? (size_t)y * f.W + x : 0;
-        if (act)
-        {
-            const GFlags flags = DecodeFlags(ld128(&f.core[idx]).w & 0xff);
-            if (flags.invalid || flags.emissive) act = false;
-        }
-
-        zr_rpt_reservoir rec;
-        Reservoir r_curr = Reservoir::Init();
-        int ppx = 0, ppy = 0;
-        bool ok = false, okReplay = false;
-        Pixel cur, prev;
-        if (act)
-        {
-            LoadRecord(&resCurr[idx], rec);
-            r_curr = Reservoir::Load_NonReconnection(rec);
-            const float4 tg = target[idx];
-            r_curr.target = f3(tg.x, tg.y, tg.z);
-            // temporal validity (identical tests in CtT, TtC and both replays; the replays use the tighter plane test)
-            ok = PrevPixel(f, x, y, ppx, ppy);
-            float prevViewDepth = FLT_MAX_;
-            if (ok)
-            {
-                prevViewDepth = asfloat(__ldg(&f.pcore[(size_t)ppy * f.W + ppx].x));
-                ok = prevViewDepth != FLT_MAX_;
-            }
-        }
-        ZR_PHASE();
-        if (ok)
-        {
-            cur = LoadPixel(f, sc, f.core, f.coat, x, y, false, x, y);
-            prev = LoadPixel(f, sc, f.pcore, f.pcoat, ppx, ppy, true, x, y);
-            ok = PlaneHeuristic(prev.pos, cur.normal, cur.pos, cur.z, 1.0f);
-            okReplay = ok && PlaneHeuristic(prev.pos, cur.normal, cur.pos, cur.z, 0.01f);
-            const bool matOk = !(prev.flags.emissive || (fabsf(prev.roughness - cur.roughness) > 0.3f) ||
-                (prev.flags.transmissive != cur.flags.transmissive));
-            ok = ok && matOk;
-            okReplay = okReplay && matOk;
-        }
-        if (act && !ok)
-        {
-            if (!prm.spatialFlag)
-                WriteOutputColor(fc, finalImg, idx, r_curr.target * r_curr.W);
-            act = false;
-        }
-        const size_t pidx = ok ? (size_t)ppy * f.W + ppx : 0;
-        zr_rpt_reservoir recPrev;
-        Reservoir r_prev = Reservoir::Init();
-        if (ok)
-        {
-            LoadRecord(&resPrev[pidx], recPrev);
-            r_prev = Reservoir::Load_NonReconnection(recPrev);
-        }
-
-        // ---- Reconnect_CtT: scale w_sum by the MIS weight of the current sample in the temporal domain ----
-        {
-            const bool doCtT = ok && r_curr.w_sum != 0 && r_prev.M > 0 && !r_curr.rc.Empty();
-            Reservoir rc_full = Reservoir::Init();
-            Reconnection rcOrig = Reconnection::Init();
-            if (doCtT)
-            {
-                rc_full = r_curr;
-                rc_full.Load_Reconnection(rec);
-                rcOrig = rc_full.rc;
-                if (rc_full.rc.IsCase1() || rc_full.rc.IsCase2())
-                    XkToPrev(sc, rc_full.rc);
-            }
-            const bool needCtx = doCtT && rc_full.rc.k > 2;
-            ZR_PHASE();
-            OffsetPathContext ctx = Replay_kGt2_Sync(needCtx && okReplay, sc, prev.pos, prev.normal, prev.eta_next, prev.surface, rcOrig, prm.alpha_min);
-            if (needCtx && okReplay)
-                ctx = ctx.Quantize();
-            const OffsetPath shift = Shift2_Sync(doCtT, sc, prev.pos, prev.normal, prev.eta_next, prev.surface, rc_full.rc, &ctx, prm.alpha_min);
-            if (doCtT)
-            {
-                const float target_prev = Math::Luminance(shift.target);
-                if (target_prev > 0)
-                {
-                    const float targetLum_curr = r_curr.W > 0 ? r_curr.w_sum / r_curr.W : 0;
-                    const float jacobian = rc_full.rc.partialJacobian > 0 ? shift.partialJacobian / rc_full.rc.partialJacobian : 0;
-                    const float m_curr = targetLum_curr / (targetLum_curr + (float)r_prev.M * target_prev * jacobian);
-                    r_curr.w_sum *= m_curr;
-                    rec.w_sum = r_curr.w_sum;
-                }
-            }
-        }
-
-        // ---- Reconnect_TtC ----
-        const uint32_t M_new = r_curr.M + r_prev.M;
-        const uint32_t M_max = prm.M_max_temporal;
-        if (ok && r_prev.rc.Empty())
-        {
-            const float targetLum = Math::Luminance(r_curr.target);
-            r_curr.W = targetLum > 0 ? r_curr.w_sum / targetLum : 0;
-            r_curr.M = M_new;
-            const uint32_t k = r_curr.rc.Empty() ? r_curr.rc.k : (r_curr.rc.k > 2 ? r_curr.rc.k : 2) - 2;
-            const uint32_t mm = r_curr.M < M_max ? r_curr.M : M_max;
-            rec.meta = (rec.meta & 0xffffff00u) | ((k | (mm << 4)) & 0xff);
-            rec.W = r_curr.W;
-            st128(&resCurr[idx], make_uint4(rec.meta, asuint(rec.w_sum), asuint(rec.W), rec.L_b));
-            if (!prm.spatialFlag)
-                WriteOutputColor(fc, finalImg, idx, r_curr.target * r_curr.W);
-            ok = false;
-        }
-        Reconnection rcReplay = Reconnection::Init();
-        if (ok)
-        {
-            r_prev.Load_Reconnection(recPrev);
-            rcReplay = r_prev.rc;
-            if (r_prev.rc.IsCase1() || r_prev.rc.IsCase2())
-                XkToCurr(sc, r_prev.rc);
-        }
-        const bool needCtx = ok && r_prev.rc.k > 2;
-        ZR_PHASE();
-        OffsetPathContext ctx = Replay_kGt2_Sync(needCtx && okReplay, sc, cur.pos, cur.normal, cur.eta_next, cur.surface, rcReplay, prm.alpha_min);
-        if (needCtx && okReplay)
-            ctx = ctx.Quantize();
-        const OffsetPath shift = Shift2_Sync(ok, sc, cur.pos, cur.normal, cur.eta_next, cur.surface, r_prev.rc, &ctx, prm.alpha_min);
-        AccountCost(prm.costMap, f.W, f.H, (uint32_t)x, (uint32_t)y, t0);
-        if (!ok)
-            return;         // past the last barrier
-        const float targetLum_curr = Math::Luminance(shift.target);
-        const float jacobian = r_prev.rc.partialJacobian > 0 ? shift.partialJacobian / r_prev.rc.partialJacobian : 0;
-        bool changed = false;
-        if (targetLum_curr > 1e-6f && jacobian > 1e-5f)
-        {
-            RNG rng = RNG::Init((uint32_t)y, (uint32_t)x, fc.FrameNum + 31);
-            const float targetLum_prev = r_prev.W > 0 ? r_prev.w_sum / r_prev.W : 0;
-            const float numerator = (float)r_prev.M * targetLum_prev;
-            const float denom = numerator / jacobian + targetLum_curr;
-            const float m_prev = denom > 0 ? numerator / denom : 0;
-            const float w_prev = m_prev * r_prev.W * targetLum_curr;
-            if (r_curr.Update(w_prev, shift.target, r_prev.rc, rng))
-            {
-                r_curr.rc.partialJacobian = shift.partialJacobian;
-                changed = true;
-            }
-        }
-        const float targetLum = Math::Luminance(r_curr.target);
-        r_curr.W = targetLum > 0 ? r_curr.w_sum / targetLum : 0;
-        r_curr.M = M_new;
-        if (changed)
-        {
-            zr_rpt_reservoir out;
-            r_curr.Write(out, M_max);
-            StoreRecord(&resCurr[idx], out);
-            if (prm.spatialFlag)
-            {
-                r_curr.target = Math::Sanitize(r_curr.target);
-                target[idx] = f4(r_curr.target.x, r_curr.target.y, r_curr.target.z, 0.0f);
-            }
-        }
-        else
-        {
-            r_curr.WriteReservoirData(rec, M_max);
-            st128(&resCurr[idx], make_uint4(rec.meta, asuint(rec.w_sum), asuint(rec.W), rec.L_b));
-        }
-        if (!prm.spatialFlag)
-            WriteOutputColor(fc, finalImg, idx, r_curr.target * r_curr.W);
-    }
-
-    // -------------------------------------------------------------------------------------------
     // Spatial search
     // -------------------------------------------------------------------------------------------
     __global__ void __launch_bounds__(256) k_spatial_search(FrameView f, RptParams prm, uint16_t* __restrict__ neighbor)
@@ -704,181 +524,6 @@ namespace
         }
     }
 
-    // -------------------------------------------------------------------------------------------
-    // Spatial reuse: Reconnect_CtS + Reconnect_StC for the same pixel, in the StC-sorted thread order
-    // -------------------------------------------------------------------------------------------
-    // A block is ZR_RPT_THREADS/64 consecutive 8x8 groups of the reference's swizzled dispatch (two waves each).
-    __global__ void ZR_LB(ZR_RPT_THREADS) k_spatial(SceneDev sc, FrameView f, RptParams prm, const zr_rpt_reservoir* __restrict__ resIn,
-        zr_rpt_reservoir* __restrict__ resOut, const float4* __restrict__ target, float4* __restrict__ finalImg,
-        const uint16_t* __restrict__ neighbor, const uint16_t* __restrict__ threadMap, uint32_t dispX, uint32_t dispY,
-        const uint32_t* __restrict__ order)
-    {
-        const zr_frame_constants& fc = f.fc;
-        const long long t0 = clock64();
-        uint2 sg = make_uint2(0, 0);
-        const uint32_t groupFlat = order[blockIdx.x] * (ZR_RPT_THREADS / 64) + (threadIdx.x >> 6);
-        const uint32_t tInGroup = threadIdx.x & 63;
-        uint2 sp = make_uint2(0xffffffffu, 0xffffffffu);
-        if (groupFlat < dispX * dispY)
-            sp = SwizzleThreadGroup(groupFlat, 0, tInGroup & 7, tInGroup >> 3, 8, 8, dispX, 16, 4, 16 * dispY, sg);
-        bool active = sp.x < f.W && sp.y < f.H;
-        int x = (int)sp.x, y = (int)sp.y;
-        if (active && prm.sortSpatial)
-        {
-            const uint16_t enc = __ldg(&threadMap[(size_t)sp.y * f.W + sp.x]);
-            if (enc & (1u << 15)) active = false;
-            x = (int)sp.x + (int)(enc & 0x3f) - 31;
-            y = (int)sp.y + (int)((enc >> 7) & 0x3f) - 31;
-        }
-        if (active && (y < (int)prm.rowBegin || y >= (int)prm.rowEnd)) active = false;
-        size_t idx = 0;
-        zr_rpt_reservoir rec;
-        Reservoir r_curr = Reservoir::Init();
-        Pixel p;
-        bool hasN = false;
-        int nx = 0, ny = 0;
-        if (active)
-        {
-            const GFlags flags = FlagsAt(f.core, f.W, x, y);
-            if (flags.invalid || flags.emissive) active = false;
-        }
-        if (active)
-        {
-            idx = (size_t)y * f.W + x;
-            p = LoadPixel(f, sc, f.core, f.coat, x, y, false, x, y);
-            LoadRecord(&resIn[idx], rec);
-            r_curr = Reservoir::Load_NonReconnection(rec);
-            const float4 tg = __ldg(&target[idx]);
-            r_curr.target = f3(tg.x, tg.y, tg.z);
-            hasN = NeighborOf(f, neighbor, x, y, nx, ny);
-        }
-        const float wsum0 = active ? r_curr.w_sum : 0.0f;
-        const float waveSum = WaveSum32(wsum0);
-        const float avgEx0 = (waveSum - wsum0) / 32.0f;
-        float waveAcc = WaveSum32(active && !hasN ? r_curr.w_sum : 0.0f);
-        uint32_t M_max = prm.M_max_spatial;
-        M_max = !r_curr.rc.Empty() && r_curr.rc.lobe_k_min_1 == BSDF::GLOSSY_T ? (M_max < 4 ? M_max : 4) : M_max;
-
-        if (active && !hasN)
-        {
-            if (prm.boilingSuppression) SuppressOutlier(avgEx0, r_curr);
-            WriteOutputColor(fc, finalImg, idx, r_curr.target * r_curr.W);
-            CopyToNextFrame(rec, &resOut[idx], r_curr, M_max);
-            active = false;
-        }
-        zr_rpt_reservoir recN;
-        Reservoir r_spatial = Reservoir::Init();
-        uint32_t M_new = 0;
-        {
-            // ---- Reconnect_CtS (its result only matters under the StC LoadWSum condition) ----
-            bool doCtS = false;
-            Reservoir rc_full = Reservoir::Init();
-            Pixel pn, pr;
-            if (active)
-            {
-                LoadRecord(&resIn[(size_t)ny * f.W + nx], recN);
-                r_spatial = Reservoir::Load_NonReconnection(recN);
-                doCtS = (r_curr.w_sum != 0) && !r_curr.rc.Empty() && (r_spatial.M > 0);
-            }
-            ZR_PHASE();
-            if (doCtS)
-            {
-                rc_full = r_curr;
-                rc_full.Load_Reconnection(rec);
-                pn = LoadPixel(f, sc, f.core, f.coat, nx, ny, false, x, y);
-            }
-            const bool needCtx = doCtS && rc_full.rc.k > 2;
-            if (needCtx)
-                pr = LoadPixel(f, sc, f.core, f.coat, nx, ny, false, nx, ny);
-            ZR_PHASE();
-            OffsetPathContext ctx = Replay_kGt2_Sync(needCtx, sc, pr.pos, pr.normal, pr.eta_next, pr.surface, rc_full.rc, prm.alpha_min);
-            if (needCtx)
-                ctx = ctx.Quantize();
-            const OffsetPath shift = Shift2_Sync(doCtS, sc, pn.pos, pn.normal, pn.eta_next, pn.surface, rc_full.rc, &ctx, prm.alpha_min);
-            if (doCtS)
-            {
-                const float target_spatial = Math::Luminance(shift.target);
-                if (target_spatial > 0)
-                {
-                    const float targetLum_curr = r_curr.W > 0 ? r_curr.w_sum / r_curr.W : 0;
-                    const float jacobian = rc_full.rc.partialJacobian > 0 ? shift.partialJacobian / rc_full.rc.partialJacobian : 0;
-                    const float numerator = (float)r_curr.M * targetLum_curr;
-                    const float denom = numerator + (float)r_spatial.M * target_spatial * jacobian;
-                    const float m_curr = denom > 0 ? numerator / denom : 0;
-                    r_curr.w_sum *= m_curr;
-                }
-            }
-            if (active)
-                M_new = r_curr.M + r_spatial.M;
-        }
-        waveAcc += WaveSum32(active && r_spatial.rc.Empty() ? r_curr.w_sum : 0.0f);
-        if (active && r_spatial.rc.Empty())
-        {
-            if (prm.boilingSuppression) SuppressOutlier(avgEx0, r_curr);
-            const float targetLum = Math::Luminance(r_curr.target);
-            r_curr.W = targetLum > 0 ? r_curr.w_sum / targetLum : 0;
-            r_curr.M = M_new;
-            CopyToNextFrame(rec, &resOut[idx], r_curr, M_max);
-            WriteOutputColor(fc, finalImg, idx, r_curr.target * r_curr.W);
-            active = false;
-        }
-        bool changed = false;
-        if (active)
-        {
-            M_max = r_spatial.rc.x_k_in_motion ? (M_max < 4 ? M_max : 4) : M_max;
-            r_spatial.rc.x_k_in_motion = false;
-            r_spatial.Load_Reconnection(recN);
-        }
-        const bool needCtx = active && r_spatial.rc.k > 2;
-        ZR_PHASE();
-        OffsetPathContext ctx = Replay_kGt2_Sync(needCtx, sc, p.pos, p.normal, p.eta_next, p.surface, r_spatial.rc, prm.alpha_min);
-        if (needCtx)
-            ctx = ctx.Quantize();
-        const OffsetPath shift = Shift2_Sync(active, sc, p.pos, p.normal, p.eta_next, p.surface, r_spatial.rc, &ctx, prm.alpha_min);
-        if (active)
-        {
-            const float targetLum_curr = Math::Luminance(shift.target);
-            const float targetLum_spatial = r_spatial.W > 0 ? r_spatial.w_sum / r_spatial.W : 0;
-            const float jacobian = r_spatial.rc.partialJacobian > 0 ? shift.partialJacobian / r_spatial.rc.partialJacobian : 0;
-            if (targetLum_curr > 1e-6f && jacobian > 1e-5f && jacobian < 100)
-            {
-                const uint3 h = RNG::PCG3d(make_uint3((uint32_t)x, (uint32_t)y, (uint32_t)y));
-                RNG rng = RNG::Init(h.x, h.z, fc.FrameNum + 511);
-                const float numerator = (float)r_spatial.M * targetLum_spatial;
-                const float denom = numerator / jacobian + (float)r_curr.M * targetLum_curr;
-                const float m_spatial = denom > 0 ? numerator / denom : 0;
-                const float w_spatial = m_spatial * r_spatial.W * targetLum_curr;
-                if (r_curr.Update(w_spatial, shift.target, r_spatial.rc, rng))
-                {
-                    r_curr.rc.partialJacobian = shift.partialJacobian;
-                    changed = true;
-                }
-            }
-            const float targetLum = Math::Luminance(r_curr.target);
-            r_curr.W = targetLum > 0 ? r_curr.w_sum / targetLum : 0;
-            r_curr.M = M_new;
-        }
-        if (prm.boilingSuppression)
-        {
-            const float total = waveAcc + WaveSum32(active ? r_curr.w_sum : 0.0f);
-            if (active)
-                SuppressOutlier((total - r_curr.w_sum) / 32.0f, r_curr);
-        }
-        AccountCost(prm.costMap, f.W, f.H, sp.x, sp.y, t0);
-        if (!active)
-            return;
-        if (changed)
-        {
-            const uint32_t mmax = shift.surfKMin1Tramsmissive ? (M_max < 4 ? M_max : 4) : M_max;
-            zr_rpt_reservoir out;
-            r_curr.Write(out, mmax);
-            StoreRecord(&resOut[idx], out);
-        }
-        else
-            CopyToNextFrame(rec, &resOut[idx], r_curr, M_max);
-        WriteOutputColor(fc, finalImg, idx, r_curr.target * r_curr.W);
-    }
-
     std::string asset_path2(const char* name)
     {
         Dl_info info;
@@ -914,24 +559,17 @@ struct zr_indirect_pass
     zr_halo_exchange_fn exchange = nullptr;
     void* exchangeUser = nullptr;
     unsigned long long* d_costMap = nullptr;
-    // block schedules (zr_schedule.h), rebuilt when the rows or the tile costs change
+    // k_pathtrace's block schedule (zr_schedule.h), rebuilt when the rows or the tile costs change
     zr::TileCosts tileCosts;
-    zr::BlockSchedule schedPathTrace, schedTemporal, schedSpatial;
-    // spatial reuse: per-case shift queues + TMA-staged streaming merge (rpt_spatial.cu) by default, the fused kernel on request
+    zr::BlockSchedule schedPathTrace;
+    // temporal and spatial reuse: per-case shift queues + streaming merge (rpt_temporal.cu, rpt_spatial.cu)
     zr::SpatialQueued spatialQueued;
     zr::TemporalQueued temporalQueued;
-    zr::WavefrontPT wavefront;
-    int execution = ZR_RPT_EXEC_QUEUED;
     zr_status UpdateSchedules()
     {
         const uint32_t y0 = rowBegin, y1 = rowEnd < height ? rowEnd : height, v = tileCosts.version;
         if (!schedPathTrace.UpToDate(y0, y1, v))
             ZR_CUDA(schedPathTrace.Upload(zr::ScheduleSwizzled((width + 15) / 16, (height + 7) / 8, 16, 8, ZR_PT_THREADS / 128, y0, y1, tileCosts), y0, y1, v));
-        if (!schedTemporal.UpToDate(y0, y1, v))
-            ZR_CUDA(schedTemporal.Upload(zr::ScheduleTiles((width + 31) / 32, (height + ZR_RPT_THREADS / 32 - 1) / (ZR_RPT_THREADS / 32), 32,
-                ZR_RPT_THREADS / 32, y0, y1, tileCosts), y0, y1, v));
-        if (!schedSpatial.UpToDate(y0, y1, v))
-            ZR_CUDA(schedSpatial.Upload(zr::ScheduleSwizzled((width + 7) / 8, (height + 7) / 8, 8, 8, ZR_RPT_THREADS / 64, y0, y1, tileCosts), y0, y1, v));
         return ZR_OK;
     }
     zr_indirect_params params{};
@@ -947,10 +585,9 @@ struct zr_indirect_pass
     void Release()
     {
         for (int i = 0; i < 2; i++) { if (d_res[i]) cudaFree(d_res[i]); d_res[i] = nullptr; if (d_threadMap[i]) cudaFree(d_threadMap[i]); d_threadMap[i] = nullptr; }
-        schedPathTrace.Release(); schedTemporal.Release(); schedSpatial.Release();
+        schedPathTrace.Release();
         spatialQueued.Release();
         temporalQueued.Release();
-        wavefront.Release();
         if (d_target) cudaFree(d_target); if (d_final) cudaFree(d_final); if (d_neighbor) cudaFree(d_neighbor);
         d_target = d_final = nullptr; d_neighbor = nullptr;
     }
@@ -971,8 +608,6 @@ struct zr_indirect_pass
         zr_status st = spatialQueued.Resize(w, h, d_res[0], d_res[1]);
         if (st != ZR_OK) return st;
         st = temporalQueued.Resize(w, h);
-        if (st != ZR_OK) return st;
-        st = wavefront.Resize(w, h);
         if (st != ZR_OK) return st;
         // k_pathtrace's parked state needs more than the 48 KB of static shared memory. The carveout asks for just the shared
         // memory its resident blocks use (plus the 1 KB the system reserves per block); the rest of the 256 KB stays L1 for
@@ -1081,34 +716,15 @@ struct zr_indirect_pass
         const uint32_t rows = prm.rowEnd - prm.rowBegin;
 
         int cur = currTemporalIdx;
-        if (execution == ZR_RPT_EXEC_WAVEFRONT && !d_costMap)
-        {
-            st = wavefront.Run(in->scene->dev, f, prm, d_res[cur], d_target, d_final, stream);
-            if (st != ZR_OK) return st;
-        }
-        else
-        {
-            // the lock-step kernel (also while a cost map is being measured: it accounts the cycles of its blocks per tile)
-            const uint32_t dispX = (width + 15) / 16, dispY = (height + 7) / 8;
-            ZR_PROF("k_pathtrace", stream);
-            k_pathtrace<<<schedPathTrace.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, d_res[cur], d_target, d_final, dispX, dispY,
-                schedPathTrace.d_order);
-            ZR_LAUNCH_CHECK();
-        }
+        const uint32_t dispX = (width + 15) / 16, dispY = (height + 7) / 8;
+        ZR_PROF("k_pathtrace", stream);
+        k_pathtrace<<<schedPathTrace.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, d_res[cur], d_target, d_final, dispX, dispY,
+            schedPathTrace.d_order);
+        ZR_LAUNCH_CHECK();
         if (doTemporal && lastStage != ZR_RPT_STAGE_PATHTRACE)
         {
-            if (execution != ZR_RPT_EXEC_FUSED)
-            {
-                st = temporalQueued.Run(spatialQueued, in->scene->dev, f, prm, d_res[cur], d_res[1 - cur], d_target, d_final, stream);
-                if (st != ZR_OK) return st;
-            }
-            else
-            {
-                ZR_PROF("k_temporal", stream);
-                k_temporal<<<schedTemporal.count, ZR_RPT_THREADS, 0, stream>>>(in->scene->dev, f, prm, d_res[cur], d_res[1 - cur],
-                    d_target, d_final, (width + 31) / 32, schedTemporal.d_order);
-                ZR_LAUNCH_CHECK();
-            }
+            st = temporalQueued.Run(spatialQueued, in->scene->dev, f, prm, d_res[cur], d_res[1 - cur], d_target, d_final, stream);
+            if (st != ZR_OK) return st;
         }
         // reservoirs written so far are read by neighbours (spatial pass) and by the next frame's temporal pass
         if (exchange)
@@ -1134,19 +750,8 @@ struct zr_indirect_pass
                     k_sort<<<dim3(sx, ty1 - ty0), 256, 0, stream>>>(f, 3, 1u, rin, nullptr, d_neighbor, d_threadMap[1], sx, sy, ty0);
                     ZR_LAUNCH_CHECK();
                 }
-                if (execution != ZR_RPT_EXEC_FUSED)
-                {
-                    st = spatialQueued.Run(in->scene->dev, f, prm, rin, rout, d_target, d_final, d_neighbor, d_threadMap[1], stream);
-                    if (st != ZR_OK) return st;
-                }
-                else
-                {
-                    const uint32_t dispX = (width + 7) / 8, dispY = (height + 7) / 8;
-                    ZR_PROF("k_spatial", stream);
-                    k_spatial<<<schedSpatial.count, ZR_RPT_THREADS, 0, stream>>>(in->scene->dev, f, prm, rin, rout, d_target, d_final, d_neighbor,
-                        d_threadMap[1], dispX, dispY, schedSpatial.d_order);
-                    ZR_LAUNCH_CHECK();
-                }
+                st = spatialQueued.Run(in->scene->dev, f, prm, rin, rout, d_target, d_final, d_neighbor, d_threadMap[1], stream);
+                if (st != ZR_OK) return st;
                 if (exchange)
                 {
                     const zr_image2d plane{ rout, width, height, width * 64u, 64u };
@@ -1168,8 +773,6 @@ extern "C"
         if (!out || !width || !height) { zr::set_error("zr_indirect_pass_create: bad args"); return ZR_ERR_INVALID_ARG; }
         zr_indirect_pass* p = new zr_indirect_pass();
         zr_indirect_pass::Defaults(&p->params);
-        if (const char* e = getenv("ZETARAY_B200_SPATIAL"))      // A/B switch for measurements: "fused" | "queued"
-            p->execution = std::string(e) == "fused" ? ZR_RPT_EXEC_FUSED : (std::string(e) == "wavefront" ? ZR_RPT_EXEC_WAVEFRONT : ZR_RPT_EXEC_QUEUED);
         zr_status s = p->OnWindowResized(width, height);
         if (s != ZR_OK) { p->Release(); delete p; return s; }
         *out = p;
@@ -1262,12 +865,6 @@ extern "C"
     {
         if (!p) return ZR_ERR_INVALID_ARG;
         p->d_costMap = (unsigned long long*)d_cycles;
-        return ZR_OK;
-    }
-    zr_status zr_indirect_pass_set_execution(zr_indirect_pass* p, zr_indirect_execution mode)
-    {
-        if (!p || (mode != ZR_RPT_EXEC_FUSED && mode != ZR_RPT_EXEC_QUEUED && mode != ZR_RPT_EXEC_WAVEFRONT)) { zr::set_error("zr_indirect_pass_set_execution: bad args"); return ZR_ERR_INVALID_ARG; }
-        p->execution = (int)mode;
         return ZR_OK;
     }
     zr_status zr_indirect_pass_set_rows(zr_indirect_pass* p, uint32_t y0, uint32_t y1)

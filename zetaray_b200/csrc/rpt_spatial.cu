@@ -1,9 +1,9 @@
 // rpt_spatial.cu -- ReSTIR PT spatial reuse as classify -> per-case shift queues -> TMA-staged streaming merge.
 //
-// Replaces the same reference dispatches as the fused k_spatial in rpt.cu (ReSTIR_PT_Replay x2, ReSTIR_PT_Reconnect_CtS.hlsl:46-230,
-// ReSTIR_PT_Reconnect_StC.hlsl:150-352) and produces the same bytes; only the execution model differs (zr_rpt_spatial.h).
+// Replaces ReSTIR_PT_Replay x2, ReSTIR_PT_Reconnect_CtS.hlsl:46-230 and ReSTIR_PT_Reconnect_StC.hlsl:150-352 and produces the oracle's
+// bytes; the execution model is described in zr_rpt_spatial.h.
 //
-// Why the split: the fused kernel evaluates two hybrid shifts inline per pixel, so a warp idles on sky pixels, on pixels without a
+// Why the split: a fused kernel evaluates two hybrid shifts inline per pixel, so a warp idles on sky pixels, on pixels without a
 // neighbour, on the other reconnection cases' phases (17 of 32 lanes active on the Cornell frame, 9 on the tunnel), and the 128 k
 // instructions of both shifts + merge share one register allocation. Here
 //   * the shifts run from queues holding (pixel, direction) items of ONE reconnection case and replay class, drained by
@@ -16,7 +16,6 @@
 #include "zr_rpt_spatial.h"
 #include "zr_rpt_shift.cuh"
 #include "zr_tma.cuh"
-#include <cstdlib>
 
 namespace zr
 {
@@ -379,15 +378,12 @@ zr_status SpatialQueued::Resize(uint32_t w, uint32_t h, const zr_rpt_reservoir* 
     ZR_CUDA(cudaGetDevice(&dev));
     ZR_CUDA(cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev));
     ZR_CUDA(cudaFuncSetAttribute(k_spatial_merge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MergeSmem)));
-    if (!getenv("ZETARAY_B200_SHIFT_ONE_STREAM"))        // A/B switch for measurements
+    for (int i = 0; i < 2; i++)
     {
-        for (int i = 0; i < 2; i++)
-        {
-            ZR_CUDA(cudaStreamCreateWithFlags(&aux[i], cudaStreamNonBlocking));
-            ZR_CUDA(cudaEventCreateWithFlags(&evJoin[i], cudaEventDisableTiming));
-        }
-        ZR_CUDA(cudaEventCreateWithFlags(&evFork, cudaEventDisableTiming));
+        ZR_CUDA(cudaStreamCreateWithFlags(&aux[i], cudaStreamNonBlocking));
+        ZR_CUDA(cudaEventCreateWithFlags(&evJoin[i], cudaEventDisableTiming));
     }
+    ZR_CUDA(cudaEventCreateWithFlags(&evFork, cudaEventDisableTiming));
     ready = true;
     return ZR_OK;
 }

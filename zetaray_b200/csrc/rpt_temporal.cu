@@ -1,7 +1,7 @@
 // rpt_temporal.cu -- ReSTIR PT temporal reuse as classify -> per-case shift queues -> merge.
 //
-// Same reference dispatches as the fused k_temporal in rpt.cu (Sort x2, Replay x2, ReSTIR_PT_Reconnect_CtT.hlsl, ReSTIR_PT_Reconnect_TtC.hlsl)
-// and the same bytes; the execution model is the one of the spatial pass (rpt_spatial.cu, zr_rpt_shift.cuh):
+// Replaces Sort x2, Replay x2, ReSTIR_PT_Reconnect_CtT.hlsl and ReSTIR_PT_Reconnect_TtC.hlsl and produces the oracle's bytes;
+// the execution model is the one of the spatial pass (rpt_spatial.cu, zr_rpt_shift.cuh):
 //   k_temporal_classify  per pixel: reprojection + the validity tests both reconnection kernels start with (plane distance, roughness,
 //                        transmissive flag; the replay's tighter plane test), which shifts are needed, their case / replay class;
 //                        one flag byte per pixel for the merge, (pixel, direction) items for the queues

@@ -1,5 +1,5 @@
-// zr_rpt_io.cuh -- ReSTIR PT per-pixel I/O shared by the fused kernels (rpt.cu) and the queued spatial path
-// (rpt_spatial.cu): kernel parameter block, 128-bit record accesses, neighbour lookup, the boiling-suppression rule
+// zr_rpt_io.cuh -- ReSTIR PT per-pixel I/O shared by path generation (rpt.cu) and the queued reuse passes
+// (rpt_temporal.cu, rpt_spatial.cu): kernel parameter block, 128-bit record accesses, neighbour lookup, the boiling-suppression rule
 // (ReSTIR_PT/Util.hlsli:58-67) and the "reservoir did not change" copy of Reconnect_StC (ReSTIR_PT_Reconnect_StC.hlsl:83-106).
 #pragma once
 #include "zr_rpt.cuh"
@@ -144,7 +144,7 @@ namespace
         rc.x_k_in_motion = rc.x_k_in_motion || dot(dScale, dScale) > 0;
     }
 
-    // ---- path generation helpers shared by the fused (rpt.cu) and the wavefront (rpt_wavefront.cu) kernels ----
+    // ---- path generation helpers (k_pathtrace, rpt.cu) ----
     struct PrevHit { float alpha_lobe; float3 wi; float pdf; BSDF::LOBE lobe; };
 
     ZR_D void MaybeSetCase2OrCase3(int pathVertex, float3 pos, float3 normal, float t, uint32_t ID, uint32_t meshIdx,

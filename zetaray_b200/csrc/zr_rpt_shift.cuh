@@ -136,14 +136,10 @@ namespace
         const zr_rpt_reservoir* resPrev, const uint16_t* neighbor, cudaStream_t stream)
     {
         const uint32_t grid = (uint32_t)q.numSMs * SHIFT_MINBLOCKS;
-        const bool fork = q.aux[0] && q.aux[1];
-        cudaStream_t s1 = fork ? q.aux[0] : stream, s2 = fork ? q.aux[1] : stream;
-        if (fork)
-        {
-            ZR_CUDA(cudaEventRecord(q.evFork, stream));
-            ZR_CUDA(cudaStreamWaitEvent(s1, q.evFork, 0));
-            ZR_CUDA(cudaStreamWaitEvent(s2, q.evFork, 0));
-        }
+        cudaStream_t s1 = q.aux[0], s2 = q.aux[1];
+        ZR_CUDA(cudaEventRecord(q.evFork, stream));
+        ZR_CUDA(cudaStreamWaitEvent(s1, q.evFork, 0));
+        ZR_CUDA(cudaStreamWaitEvent(s2, q.evFork, 0));
 #define ZR_LAUNCH_SHIFT(CASE, REPLAY, CLS, STREAM) \
         k_shift<CASE, REPLAY, TEMPORAL><<<grid, SHIFT_THREADS, 0, STREAM>>>(sc, f, prm, resIn, resPrev, neighbor, q.d_queue + (size_t)(CLS) * q.capacity, \
             q.d_counters, CLS, q.d_shift); \
@@ -155,13 +151,10 @@ namespace
         ZR_LAUNCH_SHIFT(2, true, 3, s2);
         ZR_LAUNCH_SHIFT(3, true, 5, stream);
 #undef ZR_LAUNCH_SHIFT
-        if (fork)
-        {
-            ZR_CUDA(cudaEventRecord(q.evJoin[0], s1));
-            ZR_CUDA(cudaEventRecord(q.evJoin[1], s2));
-            ZR_CUDA(cudaStreamWaitEvent(stream, q.evJoin[0], 0));
-            ZR_CUDA(cudaStreamWaitEvent(stream, q.evJoin[1], 0));
-        }
+        ZR_CUDA(cudaEventRecord(q.evJoin[0], s1));
+        ZR_CUDA(cudaEventRecord(q.evJoin[1], s2));
+        ZR_CUDA(cudaStreamWaitEvent(stream, q.evJoin[0], 0));
+        ZR_CUDA(cudaStreamWaitEvent(stream, q.evJoin[1], 0));
         return ZR_OK;
     }
 

@@ -7,7 +7,7 @@
 //                        full warp of work (no idle lanes for sky / empty / other-case pixels); result = 16 or 8 bytes per item
 //   k_spatial_merge      streaming merge in pixel order: TMA-staged 32x32 tiles of 64-byte reservoirs, the MIS weights, the
 //                        reservoir update, boiling-suppression wave sums taken in the sorted thread order through shared memory
-// Results are bit-identical to the fused k_spatial (and to the oracle).
+// Results are bit-identical to the oracle.
 #pragma once
 #include <cuda.h>
 #include "zr_rpt_io.cuh"
@@ -59,22 +59,5 @@ struct TemporalQueued
     void Release();
     zr_status Run(SpatialQueued& q, const SceneDev& sc, const FrameView& f, const RptParams& prm, zr_rpt_reservoir* resCurr,
         const zr_rpt_reservoir* resPrev, float4* target, float4* finalImg, cudaStream_t stream);
-};
-
-// Path generation as a wavefront: one launch per bounce over the compacted queue of live paths (rpt_wavefront.cu)
-struct WavefrontPT
-{
-    uint32_t width = 0, height = 0, wavesX = 0;
-    size_t numWaves = 0;
-    unsigned char* d_states = nullptr;          // 448 bytes of path state per pixel
-    uint32_t* d_queue[2] = { nullptr, nullptr };
-    uint32_t* d_counters = nullptr;             // [0], [1] entries of queue 0 / 1; [8], [9] claim cursors
-    uint32_t* d_waveMax[2] = { nullptr, nullptr };      // per reference wave (16 x 2 pixels): maximum throughput at the roulette
-    int numSMs = 0;
-    zr_status Resize(uint32_t w, uint32_t h);
-    zr_status Allocate();
-    void Release();
-    zr_status Run(const SceneDev& sc, const FrameView& f, const RptParams& prm, zr_rpt_reservoir* res, float4* target, float4* finalImg,
-        cudaStream_t stream);
 };
 } // namespace zr

@@ -105,20 +105,4 @@ inline std::vector<uint32_t> ScheduleSwizzled(uint32_t dispX, uint32_t dispY, ui
     SortByCost(blocks, key);
     return blocks;
 }
-
-// Kernels over a plain grid of gridX x gridY tiles of tileW x tileH pixels (block id = by * gridX + bx).
-inline std::vector<uint32_t> ScheduleTiles(uint32_t gridX, uint32_t gridY, uint32_t tileW, uint32_t tileH, uint32_t rowBegin, uint32_t rowEnd,
-    const TileCosts& costs)
-{
-    std::vector<uint32_t> blocks;
-    std::vector<double> key;
-    for (uint32_t by = 0; by < gridY; by++)
-    {
-        const uint32_t r0 = by * tileH;
-        if (!(r0 + tileH > rowBegin && r0 < rowEnd)) continue;
-        for (uint32_t bx = 0; bx < gridX; bx++) { blocks.push_back(by * gridX + bx); key.push_back(costs.At(bx * tileW, r0)); }
-    }
-    SortByCost(blocks, key);
-    return blocks;
-}
 } // namespace zr

@@ -247,12 +247,6 @@ class IndirectLighting(_Pass):
     def SetRows(self, y0, y1):
         check(lib.zr_indirect_pass_set_rows(self.handle, y0, y1))
 
-    FUSED, QUEUED, WAVEFRONT = 0, 1, 2
-
-    def SetExecution(self, mode):
-        """Execution model (same results): QUEUED (default), FUSED (round-1 kernels), WAVEFRONT (one launch per bounce)."""
-        check(lib.zr_indirect_pass_set_execution(self.handle, int(mode)))
-
     def SetHaloExchange(self, fn):
         self._halo_fn = fn
         check(lib.zr_indirect_pass_set_halo_exchange(self.handle, fn if fn is not None else _lib.HALO_EXCHANGE_FN(), None))
