@@ -192,9 +192,10 @@ zr_status scene_create(const zr_scene_desc* desc, zr_scene** out)
 
     BvhBuild w;
     build_bvh8(wt.data(), total, w);
-    if (w.maxStack > (uint32_t)BVH_STACK_ENTRIES)
+    if (w.maxDepth - 1 > (uint32_t)BVH_STACK_ENTRIES)
     {
-        set_error("zr_scene_create: the BVH needs a traversal stack of %u entries, the kernels hold %d", w.maxStack, BVH_STACK_ENTRIES);
+        set_error("zr_scene_create: the BVH is %u levels deep, the kernels' traversal stack holds %d levels below the root", w.maxDepth,
+            BVH_STACK_ENTRIES);
         zr_scene_destroy(sc);
         return ZR_ERR_INVALID_ARG;
     }

@@ -23,16 +23,23 @@ struct BVH8Node
 };
 static_assert(sizeof(BVH8Node) == 80, "BVH8Node must be 80 bytes");
 
-// Entries the traversal stack of zr_scene.cuh::Traverse holds. The builder computes the exact worst case of a tree
-// (BvhBuild::maxStack) and scene creation refuses a tree that needs more, so the device never drops a node.
-constexpr int BVH_STACK_ENTRIES = 96;
+// Entries the node-group stack of zr_scene.cuh::Traverse holds. One entry stands for the unvisited hit inner children of one
+// node and each tree level keeps at most one, so a tree of depth BvhBuild::maxDepth needs maxDepth - 1 entries (the 302 k-triangle
+// atrium 8, the 1.03 M-triangle tunnel 7). Scene creation refuses a deeper tree, so the device never drops a node.
+constexpr int BVH_STACK_ENTRIES = 32;
+// How many of those entries (the top ones) Traverse keeps in registers; the rest live in a local array.
+#ifndef ZR_BVH_STACK_REGS
+#define ZR_BVH_STACK_REGS 1
+#endif
+constexpr int BVH_STACK_REGS = ZR_BVH_STACK_REGS;
+static_assert(BVH_STACK_REGS >= 1 && BVH_STACK_REGS < BVH_STACK_ENTRIES, "BVH_STACK_REGS out of range");
 
 struct BvhBuild
 {
     std::vector<BVH8Node> nodes;
     std::vector<uint32_t> leafOrder;    // global triangle index per slot of the leaf-ordered triangle array
-    uint32_t maxDepth = 0;              // of the 8-wide tree
-    uint32_t maxStack = 0;              // worst-case occupancy of the traversal stack
+    uint32_t maxDepth = 0;              // of the 8-wide tree, the root at depth 1
+    uint32_t maxStack = 0;              // worst-case occupancy of a stack of single nodes (reported only; Traverse stacks node groups)
 };
 
 // worldTris: 9 floats per triangle {v0, e1 = v1 - v0, e2 = v2 - v0}, the arithmetic k_world_tris produced.

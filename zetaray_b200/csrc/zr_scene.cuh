@@ -67,6 +67,13 @@ ZR_D uint32_t TriID(const SceneDev& sc, uint32_t tri)
 }
 
 // Mode: 0 = closest hit, 1 = any hit whose ID differs from ignoreID (UINT32_MAX = none ignored)
+//
+// Everything per node stays in registers. The slab tests of the 8 slots are unrolled into a mask of hit leaves and one sort key per
+// hit inner child; the keys are sorted by a compare-exchange network, and one loop tests the hit leaves' triangles. The stack holds
+// node groups: a node's inner children sit at childBase + slot (bvh_build.cpp emit_wide), so one entry {childBase, slots} stands for
+// all its hit inner children not yet visited, as 4-bit fields (8 | slot) in near-to-far order, lowest first. Each tree level keeps at
+// most one non-empty entry, so the stack never holds more than BvhBuild::maxDepth - 1 entries, whatever the ray. The top
+// BVH_STACK_REGS entries live in registers (statically indexed, shifted on push and pop); deeper ones go to a local array.
 template<int Mode>
 ZR_F1 RayHit Traverse(const SceneDev& sc, float3 o, float3 d, float tmin, float tmax, uint32_t ignoreID)
 {
@@ -76,24 +83,24 @@ ZR_F1 RayHit Traverse(const SceneDev& sc, float3 o, float3 d, float tmin, float 
     // every barycentric NaN), but they pass every slab test below (0 * inf and NaN drop out of fminf / fmaxf), i.e. they would
     // sweep the whole tree: one such ray per ~1500 pixels comes out of the path tracer's BSDF-sampled emissive-hit query on
     // transmissive surfaces (wi = 0 when the sampler returns pdf 0), and such a ray holds its whole 1024-thread block
-    // for a full sweep of the tree. They start with an empty stack. One translation
-    // unit, rgi.cu, opts out (ZR_NO_DEGENERATE_RAY_EARLY_OUT): with this cut compiled in -- as an empty stack or as an early return,
-    // both tried -- k_rgi runs with half the active lanes per warp (see rgi.cu).
+    // for a full sweep of the tree. They visit no node. One translation unit, rgi.cu, opts out (ZR_NO_DEGENERATE_RAY_EARLY_OUT):
+    // with this cut compiled in, k_rgi runs with half the active lanes per warp (see rgi.cu).
     const bool degenerate = (d.x == 0.0f && d.y == 0.0f && d.z == 0.0f) || d.x != d.x || d.y != d.y || d.z != d.z ||
         o.x != o.x || o.y != o.y || o.z != o.z;
-#if defined(ZR_DEGENERATE_RAY_RETURN)          /* A/B switches for measurements only */
-    if (degenerate) return best;
-#endif
     const float3 invd = f3(1.0f / d.x, 1.0f / d.y, 1.0f / d.z);
-    uint32_t stack[BVH_STACK_ENTRIES];
-    int sp = 0;
-    stack[sp++] = 0;
-#if !defined(ZR_NO_DEGENERATE_RAY_EARLY_OUT) && !defined(ZR_DEGENERATE_RAY_RETURN)
-    sp = degenerate ? 0 : sp;
+    uint32_t topBase[BVH_STACK_REGS], topSlots[BVH_STACK_REGS];     // [0] = top of the stack; topSlots == 0: no entry
+#pragma unroll
+    for (int i = 0; i < BVH_STACK_REGS; i++) { topBase[i] = 0; topSlots[i] = 0; }
+    uint2 deep[BVH_STACK_ENTRIES - BVH_STACK_REGS];
+    int nDeep = 0;
+    uint32_t nodeIdx = 0;
+#if defined(ZR_NO_DEGENERATE_RAY_EARLY_OUT)
+    bool visit = true;
+#else
+    bool visit = !degenerate;
 #endif
-    while (sp > 0)
+    while (visit)
     {
-        const uint32_t nodeIdx = stack[--sp];
 #ifdef ZR_TRAVERSE_STATS        /* host test builds only (tests/hostsim): node visits / triangle tests per ray */
         ZR_TRAVERSE_STATS.nodes++;
 #endif
@@ -109,13 +116,14 @@ ZR_F1 RayHit Traverse(const SceneDev& sc, float3 o, float3 d, float tmin, float 
         const uint32_t metaLo = n1.z, metaHi = n1.w;
         // qlo[0] = n2.xy, qlo[1] = n2.zw, qlo[2] = n3.xy, qhi[0] = n3.zw, qhi[1] = n4.xy, qhi[2] = n4.zw
         const uint32_t q[12] = { n2.x, n2.y, n2.z, n2.w, n3.x, n3.y, n3.z, n3.w, n4.x, n4.y, n4.z, n4.w };
-        // children are visited far-to-near pushed, so near ones pop first
-        float childT[8];
-        uint32_t childNode[8];
-        int nPush = 0;
+        // key of a hit inner child: its entry distance with the slot in the low 3 bits (tn >= tmin >= 0, so unsigned order is
+        // distance order; the dropped bits only reorder near-ties). Missed and non-inner slots keep ~0 and sort last.
+        uint32_t key[8];
+        uint32_t innerMask = 0, leafMask = 0;
 #pragma unroll
         for (int c = 0; c < 8; c++)
         {
+            key[c] = 0xffffffffu;
             const uint32_t meta = ((c < 4 ? metaLo : metaHi) >> ((c & 3) * 8)) & 0xffu;
             if (meta == 0) continue;
             const int w = c >> 2, sh = (c & 3) * 8;
@@ -131,53 +139,98 @@ ZR_F1 RayHit Traverse(const SceneDev& sc, float3 o, float3 d, float tmin, float 
             const float tn = fmaxf(fmaxf(fminf(tx0, tx1), fminf(ty0, ty1)), fmaxf(fminf(tz0, tz1), tmin));
             const float tf = fminf(fminf(fmaxf(tx0, tx1), fmaxf(ty0, ty1)), fminf(fmaxf(tz0, tz1), best.t)) * 1.0000005f;
             if (!(tn <= tf)) continue;
-            if (meta & 0x20u)
+            if (meta & 0x20u)       // an inner child's offset from childBase is its slot
             {
-                childT[nPush] = tn;
-                childNode[nPush] = childBase + (meta & 0x1fu);
-                nPush++;
+                key[c] = (__float_as_uint(tn) & ~7u) | (uint32_t)c;
+                innerMask |= 1u << c;
             }
             else
+                leafMask |= 1u << c;
+        }
+        // the hit leaves' triangles, slot by slot
+        while (leafMask)
+        {
+            const int c = __ffs((int)leafMask) - 1;
+            leafMask &= leafMask - 1;
+            const uint32_t meta = ((c < 4 ? metaLo : metaHi) >> ((c & 3) * 8)) & 0xffu;
+            const uint32_t nt = meta >> 6;
+            const uint32_t first = triBase + (meta & 0x1fu);
+            for (uint32_t k = 0; k < nt; k++)
             {
-                const uint32_t nt = meta >> 6;
-                const uint32_t first = triBase + (meta & 0x1fu);
-                for (uint32_t k = 0; k < nt; k++)
-                {
-                    const float4* tp = sc.tris + (size_t)(first + k) * 3;
-                    const float4 a = __ldg(tp), b = __ldg(tp + 1), cc = __ldg(tp + 2);
-                    float t, u, v;
+                const float4* tp = sc.tris + (size_t)(first + k) * 3;
+                const float4 a = __ldg(tp), b = __ldg(tp + 1), cc = __ldg(tp + 2);
+                float t, u, v;
 #ifdef ZR_TRAVERSE_STATS
-                    ZR_TRAVERSE_STATS.tris++;
+                ZR_TRAVERSE_STATS.tris++;
 #endif
-                    if (TriHit(o, d, f3(a.x, a.y, a.z), f3(b.x, b.y, b.z), f3(cc.x, cc.y, cc.z), tmin, tmax, t, u, v))
+                if (TriHit(o, d, f3(a.x, a.y, a.z), f3(b.x, b.y, b.z), f3(cc.x, cc.y, cc.z), tmin, tmax, t, u, v))
+                {
+                    const uint32_t triGlobal = asuint(a.w);
+                    if (Mode == 1)
                     {
-                        const uint32_t triGlobal = asuint(a.w);
-                        if (Mode == 1)
-                        {
-                            if (ignoreID == 0xffffffffu || TriID(sc, triGlobal) != ignoreID)
-                            {
-                                best.hit = true; best.t = t; best.bary = f2(u, v); best.tri = triGlobal;
-                                return best;
-                            }
-                        }
-                        else if (!best.hit || t < best.t || (t == best.t && triGlobal < best.tri))
+                        if (ignoreID == 0xffffffffu || TriID(sc, triGlobal) != ignoreID)
                         {
                             best.hit = true; best.t = t; best.bary = f2(u, v); best.tri = triGlobal;
+                            return best;
                         }
+                    }
+                    else if (!best.hit || t < best.t || (t == best.t && triGlobal < best.tri))
+                    {
+                        best.hit = true; best.t = t; best.bary = f2(u, v); best.tri = triGlobal;
                     }
                 }
             }
         }
-        // push far-to-near (insertion sort, <= 8 entries)
-        for (int i = 1; i < nPush; i++)
+        // hit inner children near to far, as 4-bit fields (8 | slot), nearest in the low bits
+        uint32_t slots = 0;
+        if (innerMask & (innerMask - 1))
         {
-            float kt = childT[i]; uint32_t kn = childNode[i];
-            int j = i - 1;
-            while (j >= 0 && childT[j] < kt) { childT[j + 1] = childT[j]; childNode[j + 1] = childNode[j]; j--; }
-            childT[j + 1] = kt; childNode[j + 1] = kn;
+#define ZR_CSWAP(i, j) { const uint32_t lo_ = key[i] < key[j] ? key[i] : key[j]; key[j] = key[i] < key[j] ? key[j] : key[i]; key[i] = lo_; }
+            ZR_CSWAP(0, 2) ZR_CSWAP(1, 3) ZR_CSWAP(4, 6) ZR_CSWAP(5, 7)
+            ZR_CSWAP(0, 4) ZR_CSWAP(1, 5) ZR_CSWAP(2, 6) ZR_CSWAP(3, 7)
+            ZR_CSWAP(0, 1) ZR_CSWAP(2, 3) ZR_CSWAP(4, 5) ZR_CSWAP(6, 7)
+            ZR_CSWAP(2, 4) ZR_CSWAP(3, 5)
+            ZR_CSWAP(1, 4) ZR_CSWAP(3, 6)
+            ZR_CSWAP(1, 2) ZR_CSWAP(3, 4) ZR_CSWAP(5, 6)
+#undef ZR_CSWAP
+#pragma unroll
+            for (int i = 0; i < 8; i++)
+                slots |= (key[i] == 0xffffffffu ? 0u : 8u | (key[i] & 7u)) << (4 * i);
         }
-        for (int i = 0; i < nPush; i++)
-            if (sp < BVH_STACK_ENTRIES) stack[sp++] = childNode[i];      // never drops: scene creation checked BvhBuild::maxStack
+        else if (innerMask)
+            slots = 8u | (uint32_t)(__ffs((int)innerMask) - 1);
+        if (slots)
+        {
+            // descend into the nearest; the others become one entry
+            nodeIdx = childBase + (slots & 7u);
+            slots >>= 4;
+            if (slots)
+            {
+                if (topSlots[BVH_STACK_REGS - 1] && nDeep < BVH_STACK_ENTRIES - BVH_STACK_REGS)    // bounded: scene creation checked the depth
+                    deep[nDeep++] = make_uint2(topBase[BVH_STACK_REGS - 1], topSlots[BVH_STACK_REGS - 1]);
+#pragma unroll
+                for (int i = BVH_STACK_REGS - 1; i > 0; i--) { topBase[i] = topBase[i - 1]; topSlots[i] = topSlots[i - 1]; }
+                topBase[0] = childBase; topSlots[0] = slots;
+            }
+        }
+        else if (topSlots[0])
+        {
+            nodeIdx = topBase[0] + (topSlots[0] & 7u);
+            topSlots[0] >>= 4;
+            if (!topSlots[0])
+            {
+#pragma unroll
+                for (int i = 0; i < BVH_STACK_REGS - 1; i++) { topBase[i] = topBase[i + 1]; topSlots[i] = topSlots[i + 1]; }
+                topSlots[BVH_STACK_REGS - 1] = 0;
+                if (nDeep > 0)
+                {
+                    const uint2 e = deep[--nDeep];
+                    topBase[BVH_STACK_REGS - 1] = e.x; topSlots[BVH_STACK_REGS - 1] = e.y;
+                }
+            }
+        }
+        else
+            visit = false;
     }
     return best;
 }
