@@ -49,7 +49,8 @@ ZR_API const char* zr_last_error(void);
 /* (major << 16) | minor; additions bump the minor. 1.1 added zr_bvh_build_host, zr_renderer_set_integrator,
  * zr_renderer_get_gi_pass, zr_renderer_apply_scene_settings and zr_gi_pass_set_method; 1.2 the SVGF pass, zr_comm, the strip-sharded
  * renderer (zr_renderer_set_shard) and zr_gi_pass_set_rows / set_halo_exchange. 1.3 removed two
- * measurement and test hooks: the ReSTIR PT execution-model switch and the two-dispatch compositing entry point. */
+ * measurement and test hooks: the ReSTIR PT execution-model switch and the two-dispatch compositing entry point. 1.4 removed
+ * the stage-limited ReSTIR PT render and its stage enum, which nothing called. */
 ZR_API uint32_t zr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -467,19 +468,12 @@ typedef enum zr_indirect_output
     ZR_INDIRECT_FINAL = 0, ZR_INDIRECT_RESERVOIR_CURR, ZR_INDIRECT_RESERVOIR_PREV, ZR_INDIRECT_TARGET,
     ZR_INDIRECT_NEIGHBOR, ZR_INDIRECT_THREADMAP_CTN, ZR_INDIRECT_THREADMAP_NTC
 } zr_indirect_output;
-/* stages for parity tests: stop the frame after a stage (0 = whole frame) */
-typedef enum zr_indirect_stage
-{
-    ZR_RPT_STAGE_ALL = 0, ZR_RPT_STAGE_PATHTRACE = 1, ZR_RPT_STAGE_TEMPORAL = 2, ZR_RPT_STAGE_SPATIAL = 3
-} zr_indirect_stage;
 ZR_API zr_status zr_indirect_pass_create(uint32_t width, uint32_t height, zr_indirect_pass** out);
 ZR_API zr_status zr_indirect_pass_resize(zr_indirect_pass* p, uint32_t width, uint32_t height);
 ZR_API zr_status zr_indirect_pass_reset_temporal(zr_indirect_pass* p);
 ZR_API zr_status zr_indirect_pass_default_params(zr_indirect_params* out);
 ZR_API zr_status zr_indirect_pass_set_params(zr_indirect_pass* p, const zr_indirect_params* params);
 ZR_API zr_status zr_indirect_pass_render(zr_indirect_pass* p, const zr_frame_inputs* in, void* stream);
-ZR_API zr_status zr_indirect_pass_render_until(zr_indirect_pass* p, const zr_frame_inputs* in,
-    zr_indirect_stage last_stage, void* stream);
 ZR_API zr_status zr_indirect_pass_get_output(zr_indirect_pass* p, zr_indirect_output id, zr_image2d* out);
 ZR_API zr_status zr_indirect_pass_describe_io(zr_indirect_pass* p, zr_resource_use* uses, int* n);
 /* multi-GPU: rows [y0, y1) this rank owns; halo rows are read from the (all-gathered) planes */

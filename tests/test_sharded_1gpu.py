@@ -54,6 +54,29 @@ class ThreadHalo:
         self.barrier.wait()
 
 
+@pytest.mark.parametrize("pass_cls,has_schedule_costs", [("DirectLighting", True), ("IndirectLighting", True), ("IndirectLightingGI", False)])
+def test_lighting_pass_strip_setters_refuse_bad_input(pass_cls, has_schedule_costs):
+    """The lighting passes refuse an empty or out-of-image row range and a schedule-cost array of the wrong tile shape with
+    ZR_ERR_INVALID_ARG, and zr_last_error names the pass and the entry point."""
+    from zetaray_b200 import lib, passes
+    W, H = 96, 70
+    p = getattr(passes, pass_cls)(W, H)
+    set_rows = getattr(lib, p.prefix + "_set_rows")
+    for y0, y1 in ((0, 0), (40, 20), (H, H + 32), (H + 5, H + 40)):
+        assert set_rows(p.handle, y0, y1) == 1, (y0, y1)
+        assert lib.zr_last_error() == (p.prefix + "_set_rows: empty row range").encode()
+    assert set_rows(p.handle, 32, H + 100) == 0         # rows past the image are clipped when the pass renders
+    if not has_schedule_costs:
+        return
+    set_costs = getattr(lib, p.prefix + "_set_schedule_costs")
+    tx, ty = (W + 31) // 32, (H + 31) // 32
+    for bx, by in ((tx - 1, ty), (tx, ty + 1), (W // 8, H // 8)):
+        assert set_costs(p.handle, (C.c_double * (bx * by))(), bx, by) == 1, (bx, by)
+        assert lib.zr_last_error() == ("%s_set_schedule_costs: expected %u x %u tiles" % (p.prefix, tx, ty)).encode()
+    assert set_costs(p.handle, (C.c_double * (tx * ty))(*range(tx * ty)), tx, ty) == 0
+    assert set_costs(p.handle, None, 0, 0) == 0
+
+
 @pytest.mark.parametrize("which,bounds", [("glossy", [0, 96, 200]), ("glass", [0, 64, 128, 200])])
 def test_sharded_threads_equal_unsharded(which, bounds):
     import torch

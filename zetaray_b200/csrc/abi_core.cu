@@ -1,5 +1,6 @@
-// abi_core.cu -- error plumbing, launch accounting and host<->device helpers of the C-ABI.
+// abi_core.cu -- error plumbing, asset files, launch accounting and host<->device helpers of the C-ABI.
 #include "zr_common.cuh"
+#include <dlfcn.h>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -20,6 +21,28 @@ namespace zr
         va_start(ap, fmt);
         vsnprintf(g_err, sizeof(g_err), fmt, ap);
         va_end(ap);
+    }
+
+    zr_status read_asset(const char* who, const char* name, void* dst, size_t bytes)
+    {
+        Dl_info info;
+        std::string dir = ".";
+        if (dladdr((void*)&read_asset, &info) && info.dli_fname)
+        {
+            const std::string lib = info.dli_fname;
+            const size_t s = lib.find_last_of('/');
+            if (s != std::string::npos) dir = lib.substr(0, s);
+        }
+        const std::string path = dir + "/assets/" + name;
+        FILE* fp = fopen(path.c_str(), "rb");
+        const bool ok = fp && fread(dst, 1, bytes, fp) == bytes;
+        if (fp) fclose(fp);
+        if (!ok)
+        {
+            set_error("%s: cannot read %s (tools/extract_reference_tables.py writes it)", who, path.c_str());
+            return ZR_ERR_NOT_INITIALIZED;
+        }
+        return ZR_OK;
     }
 
     zr_status cuda_fail(cudaError_t e, const char* what)
@@ -59,8 +82,9 @@ namespace zr
 extern "C"
 {
     const char* zr_last_error(void) { return zr::g_err; }
+    // 1.4: - the stage-limited ReSTIR PT render and its stage enum (nothing called them)
     // 1.3: - zr_indirect_pass_set_execution, zr_compositing_pass_render_unfused (measurement and test hooks; nothing else called them)
-    uint32_t zr_abi_version(void) { return (1u << 16) | 3u; }     // 1.2: + SVGF pass, zr_comm, sharded renderer, zr_gi_pass_set_rows / set_halo_exchange; 1.1: + zr_bvh_build_host, zr_renderer_set_integrator / get_gi_pass / apply_scene_settings, zr_gi_pass_set_method
+    uint32_t zr_abi_version(void) { return (1u << 16) | 4u; }     // 1.2: + SVGF pass, zr_comm, sharded renderer, zr_gi_pass_set_rows / set_halo_exchange; 1.1: + zr_bvh_build_host, zr_renderer_set_integrator / get_gi_pass / apply_scene_settings, zr_gi_pass_set_method
     uint64_t zr_kernel_launch_count(void) { return zr::g_launches.load(); }
 
     zr_status zr_profile_enable(int on)

@@ -292,13 +292,9 @@ struct zr_gi_pass
     bool resetTemporalTextures = true;
     zr_gi_params params{};
     bool plainPathTracer = false;       // INTEGRATOR::PATH_TRACING instead of ReSTIR_GI (both read cb_ReSTIR_GI in the reference)
-    // strip-sharded frames (SURVEY 8e): owned rows + the hook that makes the reservoirs just written coherent across strips (they are
-    // next frame's temporal candidates, searched up to 16 px around the reprojected pixel: ReSTIR_GI/Params.hlsli:45)
-    uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
-    zr_halo_exchange_fn exchange = nullptr;
-    void* exchangeUser = nullptr;
-    zr::TileCosts tileCosts;
-    zr::BlockSchedule sched;
+    // the hook makes the reservoirs just written coherent across strips (they are next frame's temporal candidates, searched up to
+    // 16 px around the reprojected pixel: ReSTIR_GI/Params.hlsli:45); no tile costs are ever set, so blocks run in plain order
+    zr::LightingStrip strip{ "zr_gi_pass" };
 
     static void Defaults(zr_gi_params* p)
     {
@@ -311,7 +307,7 @@ struct zr_gi_pass
         for (int i = 0; i < 2; i++) { if (d_res[i]) cudaFree(d_res[i]); d_res[i] = nullptr; }
         if (d_final) cudaFree(d_final);
         d_final = nullptr;
-        sched.Release();
+        strip.Release();
     }
     zr_status OnWindowResized(uint32_t w, uint32_t h)
     {
@@ -335,27 +331,9 @@ struct zr_gi_pass
     zr_status Render(const zr_frame_inputs* in, cudaStream_t stream)
     {
         using namespace zr;
-        if (!in || !in->scene || !in->curr.d_core || !in->curr.d_motion_emissive || !in->curr.d_coat)
-        {
-            set_error("zr_gi_pass_render: missing scene or G-buffer");
-            return ZR_ERR_INVALID_ARG;
-        }
-        if (in->frame.RenderWidth != width || in->frame.RenderHeight != height)
-        {
-            set_error("zr_gi_pass_render: frame is %ux%u but the pass was sized %ux%u", in->frame.RenderWidth, in->frame.RenderHeight, width, height);
-            return ZR_ERR_INVALID_ARG;
-        }
-        if (in->scene->dev.numEmissives == 0 || !in->scene->aliasBuilt)
-        {
-            set_error("zr_gi_pass_render: the emissive variant needs emissive triangles and zr_prelighting_render first "
-                "(the sun/sky variant is not part of this build)");
-            return ZR_ERR_UNSUPPORTED;
-        }
-        if (in->scene->dev.sampleSetSize && !in->scene->samplesValid)
-        {
-            set_error("zr_gi_pass_render: presampling is enabled but zr_presample_emissives has not run");
-            return ZR_ERR_NOT_INITIALIZED;
-        }
+        FrameView f;
+        zr_status st = LightingFrame("zr_gi_pass", in, width, height, f);
+        if (st != ZR_OK) return st;
         if (in->scene->dev.lvg && in->scene->dev.sampleSetSize && !in->scene->lvgValid)
         {
             set_error("zr_gi_pass_render: the light voxel grid is enabled but zr_build_light_voxel_grid has not run");
@@ -367,19 +345,12 @@ struct zr_gi_pass
             set_error("zr_gi_pass_render: temporal reuse needs the previous G-buffer");
             return ZR_ERR_INVALID_ARG;
         }
-        FrameView f;
-        f.fc = in->frame;
-        f.core = (const uint4*)in->curr.d_core; f.depth = (const float*)in->curr.d_depth;
-        f.me = (const uint2*)in->curr.d_motion_emissive; f.coat = (const uint2*)in->curr.d_coat;
-        f.pcore = (const uint4*)in->prev.d_core; f.pcoat = (const uint2*)in->prev.d_coat;
-        f.W = width; f.H = height;
         GIParams prm{ params.max_non_tr_bounces, params.max_glossy_tr_bounces, params.russian_roulette, params.stochastic_multi_bounce,
-            params.boiling_suppression, params.M_max, doTemporal ? 1u : 0u, resetTemporalTextures ? 1u : 0u, rowBegin,
-            rowEnd < height ? rowEnd : height };
+            params.boiling_suppression, params.M_max, doTemporal ? 1u : 0u, resetTemporalTextures ? 1u : 0u, strip.rowBegin, strip.ClampedRowEnd(height) };
         const uint32_t dispX = (width + 7) / 8, dispY = (height + 7) / 8;
-        if (!sched.UpToDate(prm.rowBegin, prm.rowEnd, tileCosts.version))
-            ZR_CUDA(sched.Upload(ScheduleSwizzled(dispX, dispY, 8, 8, ZR_RGI_THREADS / 64, prm.rowBegin, prm.rowEnd, tileCosts), prm.rowBegin, prm.rowEnd,
-                tileCosts.version));
+        st = strip.Schedule(width, height, 8, 8, ZR_RGI_THREADS / 64);
+        if (st != ZR_OK) return st;
+        const BlockSchedule& sched = strip.sched;
         const int cur = currTemporalIdx;
         if (plainPathTracer)
         {
@@ -391,11 +362,7 @@ struct zr_gi_pass
         ZR_PROF("k_rgi", stream);
         k_rgi<false><<<sched.count, ZR_RGI_THREADS, 0, stream>>>(in->scene->dev, f, prm, d_res[cur], d_res[1 - cur], d_final, dispX, dispY, sched.d_order);
         ZR_LAUNCH_CHECK();
-        if (exchange)
-        {
-            const zr_image2d plane{ d_res[cur], width, height, width * (uint32_t)sizeof(zr_rgi_reservoir), (uint32_t)sizeof(zr_rgi_reservoir) };
-            exchange(exchangeUser, &plane, 1, stream);
-        }
+        strip.Exchange(d_res[cur], width, height, (uint32_t)sizeof(zr_rgi_reservoir), stream);
         isTemporalReservoirValid = true;
         currTemporalIdx = 1 - cur;
         resetTemporalTextures = false;
@@ -453,18 +420,8 @@ extern "C"
         p->plainPathTracer = plain;
         return p->ResetTemporal();
     }
-    zr_status zr_gi_pass_set_rows(zr_gi_pass* p, uint32_t y0, uint32_t y1)
-    {
-        if (!p || y0 >= y1 || y0 >= p->height) { zr::set_error("zr_gi_pass_set_rows: empty row range"); return ZR_ERR_INVALID_ARG; }
-        p->rowBegin = y0; p->rowEnd = y1;
-        return ZR_OK;
-    }
-    zr_status zr_gi_pass_set_halo_exchange(zr_gi_pass* p, zr_halo_exchange_fn fn, void* user)
-    {
-        if (!p) return ZR_ERR_INVALID_ARG;
-        p->exchange = fn; p->exchangeUser = user;
-        return ZR_OK;
-    }
+    zr_status zr_gi_pass_set_rows(zr_gi_pass* p, uint32_t y0, uint32_t y1) { return p ? p->strip.SetRows(y0, y1, p->height) : ZR_ERR_INVALID_ARG; }
+    zr_status zr_gi_pass_set_halo_exchange(zr_gi_pass* p, zr_halo_exchange_fn fn, void* user) { return p ? p->strip.SetHaloExchange(fn, user) : ZR_ERR_INVALID_ARG; }
     zr_status zr_gi_pass_render(zr_gi_pass* p, const zr_frame_inputs* in, void* stream)
     {
         if (!p) return ZR_ERR_INVALID_ARG;

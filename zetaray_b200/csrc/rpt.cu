@@ -18,23 +18,12 @@
 #include "zr_rpt_io.cuh"
 #include "zr_rpt_spatial.h"
 #include "zr_schedule.h"
-#include <cstdio>
-#include <string>
-#include <vector>
-#include <dlfcn.h>
 
 namespace zr
 {
 namespace
 {
     using namespace RPT;
-
-    // accounts the cycles a block took to the tile of its first pixel
-    ZR_D void AccountCost(unsigned long long* costMap, uint32_t W, uint32_t H, uint32_t x, uint32_t y, long long t0)
-    {
-        if (costMap && threadIdx.x == 0 && x < W && y < H)
-            atomicAdd(&costMap[(size_t)(y >> 5) * ((W + 31) >> 5) + (x >> 5)], (unsigned long long)(clock64() - t0));
-    }
 
     // 512 x float2, indexed per pixel by a random offset: a __constant__ table would serialise the 32 different addresses of a warp
     __device__ __align__(8) float c_disk512[1024];
@@ -523,19 +512,6 @@ namespace
             writeOutput(dxs[i], dys[i], (int)(rank & 31), (int)(rank >> 5), result[i]);
         }
     }
-
-    std::string asset_path2(const char* name)
-    {
-        Dl_info info;
-        std::string dir = ".";
-        if (dladdr((void*)&asset_path2, &info) && info.dli_fname)
-        {
-            std::string p = info.dli_fname;
-            size_t s = p.find_last_of('/');
-            if (s != std::string::npos) dir = p.substr(0, s);
-        }
-        return dir + "/assets/" + name;
-    }
 }
 } // namespace zr
 
@@ -554,24 +530,10 @@ struct zr_indirect_pass
     bool isTemporalReservoirValid = false;
     bool resetTemporalTextures = true;
     bool patternLoaded = false;
-    // strip-sharded frames (SURVEY 8e): owned rows, halo-exchange hook, optional cost map
-    uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
-    zr_halo_exchange_fn exchange = nullptr;
-    void* exchangeUser = nullptr;
-    unsigned long long* d_costMap = nullptr;
-    // k_pathtrace's block schedule (zr_schedule.h), rebuilt when the rows or the tile costs change
-    zr::TileCosts tileCosts;
-    zr::BlockSchedule schedPathTrace;
+    zr::LightingStrip strip{ "zr_indirect_pass" };  // the block schedule is k_pathtrace's
     // temporal and spatial reuse: per-case shift queues + streaming merge (rpt_temporal.cu, rpt_spatial.cu)
     zr::SpatialQueued spatialQueued;
     zr::TemporalQueued temporalQueued;
-    zr_status UpdateSchedules()
-    {
-        const uint32_t y0 = rowBegin, y1 = rowEnd < height ? rowEnd : height, v = tileCosts.version;
-        if (!schedPathTrace.UpToDate(y0, y1, v))
-            ZR_CUDA(schedPathTrace.Upload(zr::ScheduleSwizzled((width + 15) / 16, (height + 7) / 8, 16, 8, ZR_PT_THREADS / 128, y0, y1, tileCosts), y0, y1, v));
-        return ZR_OK;
-    }
     zr_indirect_params params{};
 
     static void Defaults(zr_indirect_params* p)
@@ -585,7 +547,7 @@ struct zr_indirect_pass
     void Release()
     {
         for (int i = 0; i < 2; i++) { if (d_res[i]) cudaFree(d_res[i]); d_res[i] = nullptr; if (d_threadMap[i]) cudaFree(d_threadMap[i]); d_threadMap[i] = nullptr; }
-        schedPathTrace.Release();
+        strip.Release();
         spatialQueued.Release();
         temporalQueued.Release();
         if (d_target) cudaFree(d_target); if (d_final) cudaFree(d_final); if (d_neighbor) cudaFree(d_neighbor);
@@ -648,47 +610,21 @@ struct zr_indirect_pass
     zr_status LoadPattern()
     {
         if (patternLoaded) return ZR_OK;
-        std::vector<float> pat(1024);
-        const std::string path = zr::asset_path2("disk512.bin");
-        FILE* fp = fopen(path.c_str(), "rb");
-        if (!fp || fread(pat.data(), 4, 1024, fp) != 1024)
-        {
-            if (fp) fclose(fp);
-            zr::set_error("zr_indirect_pass: cannot read %s (tools/extract_reference_tables.py writes it)", path.c_str());
-            return ZR_ERR_NOT_INITIALIZED;
-        }
-        fclose(fp);
-        ZR_CUDA(cudaMemcpyToSymbol(zr::c_disk512, pat.data(), 4096));
+        float pat[1024];
+        zr_status st = zr::read_asset("zr_indirect_pass", "disk512.bin", pat, sizeof(pat));
+        if (st != ZR_OK) return st;
+        ZR_CUDA(cudaMemcpyToSymbol(zr::c_disk512, pat, 4096));
         patternLoaded = true;
         return ZR_OK;
     }
 
-    zr_status Render(const zr_frame_inputs* in, int lastStage, cudaStream_t stream)
+    zr_status Render(const zr_frame_inputs* in, cudaStream_t stream)
     {
         using namespace zr;
-        if (!in || !in->scene || !in->curr.d_core || !in->curr.d_motion_emissive || !in->curr.d_coat)
-        {
-            set_error("zr_indirect_pass_render: missing scene or G-buffer");
-            return ZR_ERR_INVALID_ARG;
-        }
-        if (in->frame.RenderWidth != width || in->frame.RenderHeight != height)
-        {
-            set_error("zr_indirect_pass_render: frame is %ux%u but the pass was sized %ux%u", in->frame.RenderWidth,
-                in->frame.RenderHeight, width, height);
-            return ZR_ERR_INVALID_ARG;
-        }
-        if (in->scene->dev.numEmissives == 0 || !in->scene->aliasBuilt)
-        {
-            set_error("zr_indirect_pass_render: emissive integrator needs emissive triangles and zr_prelighting_render first "
-                "(the sun/sky variant is not part of this build)");
-            return ZR_ERR_UNSUPPORTED;
-        }
-        if (in->scene->dev.sampleSetSize && !in->scene->samplesValid)
-        {
-            set_error("zr_indirect_pass_render: presampling is enabled but zr_presample_emissives has not run");
-            return ZR_ERR_NOT_INITIALIZED;
-        }
-        zr_status st = LoadPattern();
+        FrameView f;
+        zr_status st = LightingFrame("zr_indirect_pass", in, width, height, f);
+        if (st != ZR_OK) return st;
+        st = LoadPattern();
         if (st != ZR_OK) return st;
 
         const bool doTemporal = params.temporal_resample && isTemporalReservoirValid;
@@ -698,41 +634,31 @@ struct zr_indirect_pass
             set_error("zr_indirect_pass_render: temporal reuse needs the previous G-buffer");
             return ZR_ERR_INVALID_ARG;
         }
-        FrameView f;
-        f.fc = in->frame;
-        f.core = (const uint4*)in->curr.d_core; f.depth = (const float*)in->curr.d_depth;
-        f.me = (const uint2*)in->curr.d_motion_emissive; f.coat = (const uint2*)in->curr.d_coat;
-        f.pcore = (const uint4*)in->prev.d_core; f.pcoat = (const uint2*)in->prev.d_coat;
-        f.W = width; f.H = height;
         RptParams prm;
         prm.maxNonTrBounces = params.max_non_tr_bounces; prm.maxGlossyTrBounces = params.max_glossy_tr_bounces;
         prm.russianRoulette = params.russian_roulette; prm.M_max_temporal = params.M_max_temporal; prm.M_max_spatial = params.M_max_spatial;
         prm.boilingSuppression = params.boiling_suppression; prm.sortSpatial = params.sort_spatial; prm.alpha_min = params.alpha_min;
         prm.temporalResample = doTemporal; prm.resetTemporal = resetTemporalTextures; prm.spatialFlag = doSpatial;
-        prm.rowBegin = rowBegin; prm.rowEnd = rowEnd < height ? rowEnd : height;
-        prm.costMap = d_costMap;
-        st = UpdateSchedules();
+        prm.rowBegin = strip.rowBegin; prm.rowEnd = strip.ClampedRowEnd(height);
+        prm.costMap = strip.d_costMap;
+        st = strip.Schedule(width, height, 16, 8, ZR_PT_THREADS / 128);
         if (st != ZR_OK) return st;
         const uint32_t rows = prm.rowEnd - prm.rowBegin;
 
         int cur = currTemporalIdx;
         const uint32_t dispX = (width + 15) / 16, dispY = (height + 7) / 8;
         ZR_PROF("k_pathtrace", stream);
-        k_pathtrace<<<schedPathTrace.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, d_res[cur], d_target, d_final, dispX, dispY,
-            schedPathTrace.d_order);
+        k_pathtrace<<<strip.sched.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, d_res[cur], d_target, d_final, dispX, dispY,
+            strip.sched.d_order);
         ZR_LAUNCH_CHECK();
-        if (doTemporal && lastStage != ZR_RPT_STAGE_PATHTRACE)
+        if (doTemporal)
         {
             st = temporalQueued.Run(spatialQueued, in->scene->dev, f, prm, d_res[cur], d_res[1 - cur], d_target, d_final, stream);
             if (st != ZR_OK) return st;
         }
         // reservoirs written so far are read by neighbours (spatial pass) and by the next frame's temporal pass
-        if (exchange)
-        {
-            const zr_image2d plane{ d_res[cur], width, height, width * 64u, 64u };
-            exchange(exchangeUser, &plane, 1, stream);
-        }
-        if (doSpatial && lastStage != ZR_RPT_STAGE_PATHTRACE && lastStage != ZR_RPT_STAGE_TEMPORAL)
+        strip.Exchange(d_res[cur], width, height, 64u, stream);
+        if (doSpatial)
         {
             for (uint32_t pass = 0; pass < params.num_spatial_passes; pass++)
             {
@@ -752,11 +678,7 @@ struct zr_indirect_pass
                 }
                 st = spatialQueued.Run(in->scene->dev, f, prm, rin, rout, d_target, d_final, d_neighbor, d_threadMap[1], stream);
                 if (st != ZR_OK) return st;
-                if (exchange)
-                {
-                    const zr_image2d plane{ rout, width, height, width * 64u, 64u };
-                    exchange(exchangeUser, &plane, 1, stream);
-                }
+                strip.Exchange(rout, width, height, 64u, stream);
             }
         }
         isTemporalReservoirValid = true;
@@ -805,12 +727,7 @@ extern "C"
     zr_status zr_indirect_pass_render(zr_indirect_pass* p, const zr_frame_inputs* in, void* stream)
     {
         if (!p) return ZR_ERR_INVALID_ARG;
-        return p->Render(in, ZR_RPT_STAGE_ALL, (cudaStream_t)stream);
-    }
-    zr_status zr_indirect_pass_render_until(zr_indirect_pass* p, const zr_frame_inputs* in, zr_indirect_stage last_stage, void* stream)
-    {
-        if (!p) return ZR_ERR_INVALID_ARG;
-        return p->Render(in, (int)last_stage, (cudaStream_t)stream);
+        return p->Render(in, (cudaStream_t)stream);
     }
     zr_status zr_indirect_pass_get_output(zr_indirect_pass* p, zr_indirect_output id, zr_image2d* out)
     {
@@ -842,36 +759,12 @@ extern "C"
         *n = 5;
         return ZR_OK;
     }
-    zr_status zr_indirect_pass_set_halo_exchange(zr_indirect_pass* p, zr_halo_exchange_fn fn, void* user)
-    {
-        if (!p) return ZR_ERR_INVALID_ARG;
-        p->exchange = fn; p->exchangeUser = user;
-        return ZR_OK;
-    }
+    zr_status zr_indirect_pass_set_halo_exchange(zr_indirect_pass* p, zr_halo_exchange_fn fn, void* user) { return p ? p->strip.SetHaloExchange(fn, user) : ZR_ERR_INVALID_ARG; }
     zr_status zr_indirect_pass_set_schedule_costs(zr_indirect_pass* p, const double* h_tile_cost, uint32_t tiles_x, uint32_t tiles_y)
     {
-        if (!p) return ZR_ERR_INVALID_ARG;
-        if (h_tile_cost && (tiles_x != (p->width + 31) / 32 || tiles_y != (p->height + 31) / 32))
-        {
-            zr::set_error("zr_indirect_pass_set_schedule_costs: expected %u x %u tiles", (p->width + 31) / 32, (p->height + 31) / 32);
-            return ZR_ERR_INVALID_ARG;
-        }
-        p->tileCosts.cost.assign(h_tile_cost ? h_tile_cost : nullptr, h_tile_cost ? h_tile_cost + (size_t)tiles_x * tiles_y : nullptr);
-        p->tileCosts.tilesX = h_tile_cost ? tiles_x : 0;
-        p->tileCosts.version++;
-        return ZR_OK;
+        return p ? p->strip.SetScheduleCosts(h_tile_cost, tiles_x, tiles_y, p->width, p->height) : ZR_ERR_INVALID_ARG;
     }
-    zr_status zr_indirect_pass_set_cost_map(zr_indirect_pass* p, void* d_cycles)
-    {
-        if (!p) return ZR_ERR_INVALID_ARG;
-        p->d_costMap = (unsigned long long*)d_cycles;
-        return ZR_OK;
-    }
-    zr_status zr_indirect_pass_set_rows(zr_indirect_pass* p, uint32_t y0, uint32_t y1)
-    {
-        if (!p || y0 >= y1 || y0 >= p->height) { zr::set_error("zr_indirect_pass_set_rows: empty row range"); return ZR_ERR_INVALID_ARG; }
-        p->rowBegin = y0; p->rowEnd = y1;
-        return ZR_OK;
-    }
+    zr_status zr_indirect_pass_set_cost_map(zr_indirect_pass* p, void* d_cycles) { return p ? p->strip.SetCostMap(d_cycles) : ZR_ERR_INVALID_ARG; }
+    zr_status zr_indirect_pass_set_rows(zr_indirect_pass* p, uint32_t y0, uint32_t y1) { return p ? p->strip.SetRows(y0, y1, p->height) : ZR_ERR_INVALID_ARG; }
     void zr_indirect_pass_destroy(zr_indirect_pass* p) { if (p) { p->Release(); delete p; } }
 }

@@ -10,10 +10,7 @@
 #include <vector>
 #include <algorithm>
 #include <cmath>
-#include <cstdio>
 #include <cstring>
-#include <string>
-#include <dlfcn.h>
 
 namespace zr
 {
@@ -60,19 +57,6 @@ namespace
         if (i >= n) return;
         const float* r = rays + (size_t)i * 8;
         flags[i] = TraceAnyExcept(sc, f3(r[0], r[1], r[2]), f3(r[4], r[5], r[6]), r[3], r[7], 0xffffffffu) ? 1u : 0u;
-    }
-
-    std::string asset_path(const char* name)
-    {
-        Dl_info info;
-        std::string dir = ".";
-        if (dladdr((void*)&asset_path, &info) && info.dli_fname)
-        {
-            std::string p = info.dli_fname;
-            size_t s = p.find_last_of('/');
-            if (s != std::string::npos) dir = p.substr(0, s);
-        }
-        return dir + "/assets/" + name;
     }
 }
 
@@ -165,16 +149,7 @@ zr_status scene_create(const zr_scene_desc* desc, zr_scene** out)
     // directional-albedo table
     {
         std::vector<uint16_t> rho(64 * 32 * 16);
-        const std::string path = asset_path("rho_lut.bin");
-        FILE* f = fopen(path.c_str(), "rb");
-        if (!f || fread(rho.data(), 2, rho.size(), f) != rho.size())
-        {
-            if (f) fclose(f);
-            set_error("zr_scene_create: cannot read %s (tools/extract_reference_tables.py writes it)", path.c_str());
-            zr_scene_destroy(sc);
-            return ZR_ERR_NOT_INITIALIZED;
-        }
-        fclose(f);
+        if ((st = read_asset("zr_scene_create", "rho_lut.bin", rho.data(), rho.size() * sizeof(uint16_t))) != ZR_OK) { zr_scene_destroy(sc); return st; }
         UP(rho, rho.data(), rho.size());
     }
 

@@ -502,7 +502,7 @@ namespace BSDF
 
     struct BSDFEval { float3 f; float3 Fr_g; bool tir; };
 
-    ZR_F1 BSDFEval Unified(const ShadingData& surface)
+    ZR_D BSDFEval Unified(const ShadingData& surface)
     {
         BSDFEval ret;
         ret.f = f3(0); ret.Fr_g = f3(0); ret.tir = false;
@@ -565,7 +565,7 @@ namespace BSDF
     };
     struct BSDFSamplerEval { float pdf; float3 bsdfOverPdf; float3 f; };
 
-    ZR_F2 BSDFSample SampleBSDF_NoDiffuse(float3 normal, ShadingData surface, float2 u_c, float2 u_g,
+    ZR_D BSDFSample SampleBSDF_NoDiffuse(float3 normal, ShadingData surface, float2 u_c, float2 u_g,
         float u_wrs_0, float u_wrs_1)
     {
         BSDFSample ret = BSDFSample::Init();
@@ -627,7 +627,7 @@ namespace BSDF
         return ret;
     }
 
-    ZR_F2 BSDFSample SampleBSDF_NoDiffuse(float3 normal, const ShadingData& surface, RNG& rng)
+    ZR_D BSDFSample SampleBSDF_NoDiffuse(float3 normal, const ShadingData& surface, RNG& rng)
     {
         float2 u_c = rng.Uniform2D();
         float2 u_g = rng.Uniform2D();
@@ -636,7 +636,7 @@ namespace BSDF
         return SampleBSDF_NoDiffuse(normal, surface, u_c, u_g, u_wrs_0, u_wrs_1);
     }
 
-    ZR_F2 BSDFSample SampleBSDF_NoSpecTr(float3 normal, ShadingData surface, float2 u_coat, float2 u_g, float2 u_d,
+    ZR_D BSDFSample SampleBSDF_NoSpecTr(float3 normal, ShadingData surface, float2 u_coat, float2 u_g, float2 u_d,
         float u_wrs_g, float u_wrs_dr, float u_wrs_dt)
     {
         BSDFSample ret = BSDFSample::Init();
@@ -732,7 +732,7 @@ namespace BSDF
         return SampleBSDF_NoDiffuse(normal, surface, u_c, u_g, u_wrs_0, u_wrs_1);
     }
 
-    ZR_F2 BSDFSamplerEval EvalBSDFSampler_NoSpecTr(float3 normal, ShadingData surface, float3 wi, LOBE lobe,
+    ZR_D BSDFSamplerEval EvalBSDFSampler_NoSpecTr(float3 normal, ShadingData surface, float3 wi, LOBE lobe,
         float2 u_c, float2 u_g, float2 u_d)
     {
         BSDFSamplerEval ret;
@@ -798,7 +798,7 @@ namespace BSDF
         return ret;
     }
 
-    ZR_F2 BSDFSamplerEval EvalBSDFSampler_NoDiffuse(float3 normal, ShadingData surface, float3 wi, LOBE lobe)
+    ZR_D BSDFSamplerEval EvalBSDFSampler_NoDiffuse(float3 normal, ShadingData surface, float3 wi, LOBE lobe)
     {
         float3 wh = surface.SetWi(wi, normal);
         BSDFEval eval = Unified(surface);
@@ -861,7 +861,7 @@ namespace BSDF
         return EvalBSDFSampler_NoDiffuse(normal, surface, wi, lobe);
     }
 
-    ZR_F2 float BSDFSamplerPdf_NoDiffuse(float3 normal, ShadingData surface, float3 wi)
+    ZR_D float BSDFSamplerPdf_NoDiffuse(float3 normal, ShadingData surface, float3 wi)
     {
         float3 wh = surface.SetWi(wi, normal);
         float pdf_base = 1;
@@ -904,7 +904,7 @@ namespace BSDF
         return pdf_g;
     }
 
-    ZR_F2 float BSDFSamplerPdf(float3 normal, ShadingData surface, float3 wi_z, RNG& rng)
+    ZR_D float BSDFSamplerPdf(float3 normal, ShadingData surface, float3 wi_z, RNG& rng)
     {
         if (surface.specTr)
             return BSDFSamplerPdf_NoDiffuse(normal, surface, wi_z);

@@ -10,14 +10,9 @@
 #include "../../include/zr_abi.h"
 #include "../../include/zr_fpmath.h"
 
+// Every device function is inlined into the kernel's phase structure: real calls were slower, their ABI spills the live
+// state around every call (DESIGN 4.1).
 #define ZR_D __device__ __forceinline__
-// Call-graph shaping: the lighting kernels inline into megabytes of SASS if everything is forced inline, which
-// thrashes the instruction cache (ncu: ~80% of stall cycles "no instruction"). ZR_Fn functions become real calls
-// when ZR_NI_LEVEL >= n. Inlining does not change results (no fused contraction, no fast math).
-#ifndef ZR_NI_LEVEL
-#define ZR_NI_LEVEL 0
-#endif
-#define ZR_NI static __device__ __noinline__
 // Register budget of the lighting kernels: ZR_MAXREGS caps registers/thread through __launch_bounds__'s
 // min-blocks argument (0 = let ptxas take what it wants).
 #ifndef ZR_MAXREGS
@@ -27,21 +22,6 @@
 #define ZR_LB(threads) __launch_bounds__(threads, 65536 / ((threads) * ZR_MAXREGS))
 #else
 #define ZR_LB(threads) __launch_bounds__(threads)
-#endif
-#if ZR_NI_LEVEL >= 1
-#define ZR_F1 ZR_NI
-#else
-#define ZR_F1 ZR_D
-#endif
-#if ZR_NI_LEVEL >= 2
-#define ZR_F2 ZR_NI
-#else
-#define ZR_F2 ZR_D
-#endif
-#if ZR_NI_LEVEL >= 3
-#define ZR_F3 ZR_NI
-#else
-#define ZR_F3 ZR_D
 #endif
 
 namespace zr
@@ -59,6 +39,8 @@ constexpr float FLT16_MAX = 65504.0f;
 // host-side error plumbing
 // ---------------------------------------------------------------------------------------------
 void set_error(const char* fmt, ...);
+// Reads the first `bytes` bytes of <directory of this library>/assets/<name> into dst; `who` prefixes the error message.
+zr_status read_asset(const char* who, const char* name, void* dst, size_t bytes);
 zr_status cuda_fail(cudaError_t e, const char* what);
 void count_launch(uint64_t n = 1);
 #define ZR_CUDA(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return zr::cuda_fail(e__, #expr); } while (0)

@@ -32,6 +32,47 @@ struct FrameView
     uint32_t W, H;
 };
 
+// Checks the lighting passes share before a render, then the FrameView over the frame's G-buffers: scene and current G-buffer
+// present, a frame of the pass's size, emissive triangles with their alias table, the presampled light sets when enabled.
+// `pass` ("zr_direct_pass", ...) prefixes the error messages.
+inline zr_status LightingFrame(const char* pass, const zr_frame_inputs* in, uint32_t width, uint32_t height, FrameView& f)
+{
+    if (!in || !in->scene || !in->curr.d_core || !in->curr.d_motion_emissive || !in->curr.d_coat)
+    {
+        set_error("%s_render: missing scene or G-buffer", pass);
+        return ZR_ERR_INVALID_ARG;
+    }
+    if (in->frame.RenderWidth != width || in->frame.RenderHeight != height)
+    {
+        set_error("%s_render: frame is %ux%u but the pass was sized %ux%u", pass, in->frame.RenderWidth, in->frame.RenderHeight, width, height);
+        return ZR_ERR_INVALID_ARG;
+    }
+    if (in->scene->dev.numEmissives == 0 || !in->scene->aliasBuilt)
+    {
+        // PathTracer.cpp:274-284: the emissive variants only run when the scene has emissive triangles
+        set_error("%s_render: needs emissive triangles and zr_prelighting_render first (the sun/sky variants are not part of this build)", pass);
+        return ZR_ERR_UNSUPPORTED;
+    }
+    if (in->scene->dev.sampleSetSize && !in->scene->samplesValid)
+    {
+        set_error("%s_render: presampling is enabled but zr_presample_emissives has not run", pass);
+        return ZR_ERR_NOT_INITIALIZED;
+    }
+    f.fc = in->frame;
+    f.core = (const uint4*)in->curr.d_core; f.depth = (const float*)in->curr.d_depth;
+    f.me = (const uint2*)in->curr.d_motion_emissive; f.coat = (const uint2*)in->curr.d_coat;
+    f.pcore = (const uint4*)in->prev.d_core; f.pcoat = (const uint2*)in->prev.d_coat;
+    f.W = width; f.H = height;
+    return ZR_OK;
+}
+
+// accounts the cycles a block took to the tile of its first pixel
+ZR_D void AccountCost(unsigned long long* costMap, uint32_t W, uint32_t H, uint32_t x, uint32_t y, long long t0)
+{
+    if (costMap && threadIdx.x == 0 && x < W && y < H)
+        atomicAdd(&costMap[(size_t)(y >> 5) * ((W + 31) >> 5) + (x >> 5)], (unsigned long long)(clock64() - t0));
+}
+
 struct Pixel
 {
     GFlags flags; float roughness; float z; float3 pos, normal, origin; float2 lensSample;
@@ -49,7 +90,7 @@ ZR_D GFlags FlagsAt(const uint4* __restrict__ core, uint32_t W, int x, int y, fl
 }
 
 // prev == false: current camera / jitter / frame number; true: previous frame's
-ZR_F2 Pixel LoadPixel(const FrameView& f, const SceneDev& sc, const uint4* __restrict__ core, const uint2* __restrict__ coat,
+ZR_D Pixel LoadPixel(const FrameView& f, const SceneDev& sc, const uint4* __restrict__ core, const uint2* __restrict__ coat,
     int px, int py, bool prev, int coatX, int coatY)
 {
     const zr_frame_constants& fc = f.fc;

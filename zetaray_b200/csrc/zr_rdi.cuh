@@ -18,11 +18,6 @@ namespace
         uint32_t rowBegin, rowEnd;              // rows this device owns (strip-sharded frames)
         unsigned long long* costMap;            // optional: SM cycles spent per 32x32-pixel tile
     };
-    ZR_D void AccountCost(unsigned long long* costMap, uint32_t W, uint32_t H, uint32_t x, uint32_t y, long long t0)
-    {
-        if (costMap && threadIdx.x == 0 && x < W && y < H)
-            atomicAdd(&costMap[(size_t)(y >> 5) * ((W + 31) >> 5) + (x >> 5)], (unsigned long long)(clock64() - t0));
-    }
 
     __constant__ float c_disk32[64];
 

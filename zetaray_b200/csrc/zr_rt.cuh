@@ -46,7 +46,7 @@ struct HitEmissive
 };
 
 // RayQuery.hlsli:213-299 (ToHitInfo) == the attribute part of Hit::FindClosest
-ZR_F2 Hit HitAttributes(const SceneDev& sc, uint32_t meshIdx, uint32_t primIdx, float2 bary, float t)
+ZR_D Hit HitAttributes(const SceneDev& sc, uint32_t meshIdx, uint32_t primIdx, float2 bary, float t)
 {
     Hit ret;
     const zr_mesh_instance meshData = LoadInstance(sc, meshIdx);
@@ -178,7 +178,7 @@ ZR_D bool Visibility_Segment_Precise(const SceneDev& sc, float3 origin, float3 w
 }
 
 // GetMaterialData (RayQuery.hlsli:452-510), textures unsupported (factors only)
-ZR_F2 bool GetMaterialData(const SceneDev& sc, float3 wo, float eta_curr, Hit& hitInfo, BSDF::ShadingData& surface, float& eta)
+ZR_D bool GetMaterialData(const SceneDev& sc, float3 wo, float eta_curr, Hit& hitInfo, BSDF::ShadingData& surface, float& eta)
 {
     const zr_material mat = LoadMaterial(sc, hitInfo.matIdx);
     const bool hitBackface = dot(wo, hitInfo.normal) < 0;

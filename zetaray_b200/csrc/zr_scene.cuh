@@ -75,7 +75,7 @@ ZR_D uint32_t TriID(const SceneDev& sc, uint32_t tri)
 // most one non-empty entry, so the stack never holds more than BvhBuild::maxDepth - 1 entries, whatever the ray. The top
 // BVH_STACK_REGS entries live in registers (statically indexed, shifted on push and pop); deeper ones go to a local array.
 template<int Mode>
-ZR_F1 RayHit Traverse(const SceneDev& sc, float3 o, float3 d, float tmin, float tmax, uint32_t ignoreID)
+ZR_D RayHit Traverse(const SceneDev& sc, float3 o, float3 d, float tmin, float tmax, uint32_t ignoreID)
 {
     RayHit best;
     best.hit = false; best.t = tmax; best.bary = f2(0, 0); best.tri = 0xffffffffu;

@@ -11,6 +11,7 @@
 #include <cstdint>
 #include <vector>
 #include <cuda_runtime.h>
+#include "zr_common.cuh"
 
 namespace zr
 {
@@ -105,4 +106,69 @@ inline std::vector<uint32_t> ScheduleSwizzled(uint32_t dispX, uint32_t dispY, ui
     SortByCost(blocks, key);
     return blocks;
 }
+
+// What a lighting pass keeps for strip-sharded frames (SURVEY 8e): the rows it owns, the hook that makes rows it just wrote
+// coherent across strips, the optional cost map and tile costs, and its kernels' block table. `pass` ("zr_direct_pass", ...)
+// prefixes the error messages of the pass's set_* entry points.
+struct LightingStrip
+{
+    const char* pass;
+    uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
+    zr_halo_exchange_fn exchange = nullptr;
+    void* exchangeUser = nullptr;
+    unsigned long long* d_costMap = nullptr;
+    TileCosts tileCosts;
+    BlockSchedule sched;
+
+    explicit LightingStrip(const char* passName) : pass(passName) {}
+    void Release() { sched.Release(); }
+    uint32_t ClampedRowEnd(uint32_t height) const { return rowEnd < height ? rowEnd : height; }
+
+    zr_status SetRows(uint32_t y0, uint32_t y1, uint32_t height)
+    {
+        if (y0 >= y1 || y0 >= height) { set_error("%s_set_rows: empty row range", pass); return ZR_ERR_INVALID_ARG; }
+        rowBegin = y0; rowEnd = y1;
+        return ZR_OK;
+    }
+    zr_status SetHaloExchange(zr_halo_exchange_fn fn, void* user)
+    {
+        exchange = fn; exchangeUser = user;
+        return ZR_OK;
+    }
+    zr_status SetCostMap(void* d_cycles)
+    {
+        d_costMap = (unsigned long long*)d_cycles;
+        return ZR_OK;
+    }
+    // h_tile_cost: ceil(width/32) x ceil(height/32) tiles, row-major, or nullptr for plain order
+    zr_status SetScheduleCosts(const double* h_tile_cost, uint32_t tiles_x, uint32_t tiles_y, uint32_t width, uint32_t height)
+    {
+        if (h_tile_cost && (tiles_x != (width + 31) / 32 || tiles_y != (height + 31) / 32))
+        {
+            set_error("%s_set_schedule_costs: expected %u x %u tiles", pass, (width + 31) / 32, (height + 31) / 32);
+            return ZR_ERR_INVALID_ARG;
+        }
+        tileCosts.cost.assign(h_tile_cost ? h_tile_cost : nullptr, h_tile_cost ? h_tile_cost + (size_t)tiles_x * tiles_y : nullptr);
+        tileCosts.tilesX = h_tile_cost ? tiles_x : 0;
+        tileCosts.version++;
+        return ZR_OK;
+    }
+    // hands the hook one width x height plane of texelBytes-sized texels; nothing happens without a hook
+    void Exchange(void* d_plane, uint32_t width, uint32_t height, uint32_t texelBytes, cudaStream_t stream) const
+    {
+        if (!exchange) return;
+        const zr_image2d plane{ d_plane, width, height, width * texelBytes, texelBytes };
+        exchange(exchangeUser, &plane, 1, stream);
+    }
+    // sched for a kernel whose blocks are groupsPerBlock swizzled groups of groupW x groupH pixels; the table is rebuilt and
+    // uploaded only when the rows or the tile costs changed
+    zr_status Schedule(uint32_t width, uint32_t height, uint32_t groupW, uint32_t groupH, uint32_t groupsPerBlock)
+    {
+        const uint32_t y0 = rowBegin, y1 = ClampedRowEnd(height), v = tileCosts.version;
+        if (!sched.UpToDate(y0, y1, v))
+            ZR_CUDA(sched.Upload(ScheduleSwizzled((width + groupW - 1) / groupW, (height + groupH - 1) / groupH, groupW, groupH, groupsPerBlock,
+                y0, y1, tileCosts), y0, y1, v));
+        return ZR_OK;
+    }
+};
 } // namespace zr

@@ -258,11 +258,8 @@ class IndirectLighting(_Pass):
         arr = None if tile_costs is None else (C.c_double * (tiles_x * tiles_y))(*tile_costs)
         check(lib.zr_indirect_pass_set_schedule_costs(self.handle, arr, tiles_x, tiles_y))
 
-    def Render(self, fi, stream=None, until=0):
-        if until:
-            check(lib.zr_indirect_pass_render_until(self.handle, C.byref(fi), until, stream))
-        else:
-            check(lib.zr_indirect_pass_render(self.handle, C.byref(fi), stream))
+    def Render(self, fi, stream=None):
+        check(lib.zr_indirect_pass_render(self.handle, C.byref(fi), stream))
 
     def GetOutput(self, which=0):
         img = _lib.Image2D()
