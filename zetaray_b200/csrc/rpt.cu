@@ -32,8 +32,9 @@ namespace
     // PathTrace
     // -------------------------------------------------------------------------------------------
 // 768 threads at 80 registers with the parked state below (157 KB of shared memory per block). Measured on an H100 SXM (700 W):
-// 3.33 ms per bench frame, against 3.65 ms at 1024 x 64 registers, 3.52 ms at 512 x 128 and 4.40 ms at 512 x 2 blocks x 64
-// (DESIGN 4.1).
+// 2.61 ms per bench frame, against 2.60 ms at 640 x 96 registers and 2.68 ms at 512 x 128; 640 threads spill far less but are no
+// faster. An earlier sweep, before the traversal rewrite: 3.33 ms, against 3.65 ms at 1024 x 64, 3.52 ms at 512 x 128 and 4.40 ms
+// at 512 x 2 blocks x 64 (DESIGN 4.1).
 #ifndef ZR_PT_THREADS
 #define ZR_PT_THREADS 768
 #endif
@@ -176,10 +177,8 @@ namespace
             // phase: BSDF-sampled light hit, then light sample + BSDF value (NEE_Emissive, ReSTIR_PT_NEE.hlsli:224-302)
             NeeLightState nee;
             nee.facing = false; nee.ld = f3(0);
-            BSDF::ShadingData surfNee;
             bool lightSample = false;
             uint32_t seed_nee = 0;
-            RaySetup seg; seg.go = false;
             if (alive)
             {
                 nextHit = FinishClosestEmissive(sc, rs, rh, nextBsdfSample.wi);
@@ -197,16 +196,16 @@ namespace
                 if (lightSample)
                 {
                     seed_nee = rngThread.State;
-                    surfNee = surface;
+                    BSDF::ShadingData surfNee = surface;
                     nee = NEE_Emissive_Begin(sc, pos, hitInfo.normal, surfNee, sampleSetIdx, rngThread);
-                    if (nee.facing && dot(nee.ld, nee.ld) > 0)
-                        seg = SetupSegment(pos, nee.ret.wi, nee.t, hitInfo.normal, nee.ret.ID, surfNee.Transmissive());
                 }
             }
             ZR_PHASE();
-            // phase: shadow segment
+            // phase: shadow segment. The segment is set up here rather than carried across the barrier; SetWi leaves
+            // Transmissive() as it was, so `surface` answers for the copy NEE_Emissive_Begin shaded with.
             if (lightSample && nee.facing && dot(nee.ld, nee.ld) > 0)
             {
+                const RaySetup seg = SetupSegment(pos, nee.ret.wi, nee.t, hitInfo.normal, nee.ret.ID, surface.Transmissive());
                 const bool visible = seg.go ? !TraceAnyExcept(sc, seg.o, nee.ret.wi, seg.tmin, seg.tmax, nee.ret.ID) : false;
                 nee.ld *= visible ? 1.0f : 0.0f;
             }
@@ -217,6 +216,10 @@ namespace
                 float bsdfPdf = 0;
                 if (nee.facing && dot(nee.ld, nee.ld) > 0)
                 {
+                    // the shading copy NEE_Emissive_Begin evaluated the light sample with, rebuilt by the same SetWi instead of
+                    // carried through the shadow-segment traversal
+                    BSDF::ShadingData surfNee = surface;
+                    surfNee.SetWi(nee.ret.wi, hitInfo.normal);
                     bsdfPdf = BSDF::BSDFSamplerPdf(hitInfo.normal, surfNee, nee.ret.wi, rngThread);
                     bsdfPdf *= nee.dwdA;
                 }
