@@ -409,6 +409,14 @@ typedef enum zr_resource_id
 } zr_resource_id;
 typedef struct zr_resource_use { uint32_t id; uint32_t write; } zr_resource_use;
 
+/* ---- Pass lifetime ----
+ * zr_*_pass_create / _resize take a non-zero width and height. A resize is all-or-nothing: the pass allocates and clears a
+ * complete new set of planes and frees the old ones only when that succeeded, so while it runs both sets are allocated, and on
+ * failure the pass is exactly as it was (same size, same planes, same history). A successful resize drops the temporal history
+ * and forgets what described the old size: set_rows returns to the whole frame, the cost map and the schedule costs are unset.
+ * A halo-exchange hook stays. A failed device allocation returns ZR_ERR_OUT_OF_MEMORY (ZR_ERR_CUDA for other CUDA errors),
+ * with zr_last_error naming the pass and the bytes asked for. */
+
 /* ---- GBufferRT (GBuffer/GBufferRT.h, GBufferRT.cpp:99-160) ---- */
 typedef struct zr_gbuffer_pass zr_gbuffer_pass;
 ZR_API zr_status zr_gbuffer_pass_create(zr_gbuffer_pass** out);
@@ -466,7 +474,7 @@ typedef struct zr_indirect_params
 typedef enum zr_indirect_output
 {
     ZR_INDIRECT_FINAL = 0, ZR_INDIRECT_RESERVOIR_CURR, ZR_INDIRECT_RESERVOIR_PREV, ZR_INDIRECT_TARGET,
-    ZR_INDIRECT_NEIGHBOR, ZR_INDIRECT_THREADMAP_CTN, ZR_INDIRECT_THREADMAP_NTC
+    ZR_INDIRECT_NEIGHBOR, ZR_INDIRECT_THREADMAP_NTC = 6
 } zr_indirect_output;
 ZR_API zr_status zr_indirect_pass_create(uint32_t width, uint32_t height, zr_indirect_pass** out);
 ZR_API zr_status zr_indirect_pass_resize(zr_indirect_pass* p, uint32_t width, uint32_t height);

@@ -51,6 +51,13 @@ namespace zr
         return ZR_ERR_CUDA;
     }
 
+    zr_status check_frame_size(const char* pass, const zr_frame_constants& frame, uint32_t width, uint32_t height)
+    {
+        if (frame.RenderWidth == width && frame.RenderHeight == height) return ZR_OK;
+        set_error("%s_render: frame is %ux%u but the pass was sized %ux%u", pass, frame.RenderWidth, frame.RenderHeight, width, height);
+        return ZR_ERR_INVALID_ARG;
+    }
+
     void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
     // Optional per-kernel timing (bench.py's roofline leg): an event pair around every launch while enabled.
@@ -82,9 +89,11 @@ namespace zr
 extern "C"
 {
     const char* zr_last_error(void) { return zr::g_err; }
+    // 1.5: - ZR_INDIRECT_THREADMAP_CTN (never written; ZR_INDIRECT_THREADMAP_NTC keeps its id 6); resize is all-or-nothing and
+    //        allocation failures return ZR_ERR_OUT_OF_MEMORY
     // 1.4: - the stage-limited ReSTIR PT render and its stage enum (nothing called them)
     // 1.3: - zr_indirect_pass_set_execution, zr_compositing_pass_render_unfused (measurement and test hooks; nothing else called them)
-    uint32_t zr_abi_version(void) { return (1u << 16) | 4u; }     // 1.2: + SVGF pass, zr_comm, sharded renderer, zr_gi_pass_set_rows / set_halo_exchange; 1.1: + zr_bvh_build_host, zr_renderer_set_integrator / get_gi_pass / apply_scene_settings, zr_gi_pass_set_method
+    uint32_t zr_abi_version(void) { return (1u << 16) | 5u; }     // 1.2: + SVGF pass, zr_comm, sharded renderer, zr_gi_pass_set_rows / set_halo_exchange; 1.1: + zr_bvh_build_host, zr_renderer_set_integrator / get_gi_pass / apply_scene_settings, zr_gi_pass_set_method
     uint64_t zr_kernel_launch_count(void) { return zr::g_launches.load(); }
 
     zr_status zr_profile_enable(int on)

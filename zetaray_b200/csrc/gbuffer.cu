@@ -326,11 +326,18 @@ extern "C"
         if (!out || !width || !height) { zr::set_error("zr_gbuffer_alloc: bad args"); return ZR_ERR_INVALID_ARG; }
         const size_t n = (size_t)width * height;
         memset(out, 0, sizeof(*out));
-        ZR_CUDA(cudaMalloc(&out->d_core, n * 16));
-        ZR_CUDA(cudaMalloc(&out->d_depth, n * 4));
-        ZR_CUDA(cudaMalloc(&out->d_motion_emissive, n * 8));
-        ZR_CUDA(cudaMalloc(&out->d_coat, n * 8));
-        if (with_tridiff) ZR_CUDA(cudaMalloc(&out->d_tridiff, n * 24));
+        cudaError_t e = cudaMalloc(&out->d_core, n * 16);
+        if (e == cudaSuccess) e = cudaMalloc(&out->d_depth, n * 4);
+        if (e == cudaSuccess) e = cudaMalloc(&out->d_motion_emissive, n * 8);
+        if (e == cudaSuccess) e = cudaMalloc(&out->d_coat, n * 8);
+        if (e == cudaSuccess && with_tridiff) e = cudaMalloc(&out->d_tridiff, n * 24);
+        if (e != cudaSuccess)
+        {
+            cudaGetLastError();     // the failure is reported here, not by the next launch check
+            zr_gbuffer_free(out);
+            zr::set_error("zr_gbuffer_alloc: cannot allocate the %ux%u G-buffer (%s)", width, height, cudaGetErrorString(e));
+            return e == cudaErrorMemoryAllocation ? ZR_ERR_OUT_OF_MEMORY : ZR_ERR_CUDA;
+        }
         ZR_CLEAR_BEGIN();
         ZR_CUDA(cudaMemset(out->d_core, 0, n * 16));
         ZR_CUDA(cudaMemset(out->d_depth, 0, n * 4));

@@ -10,6 +10,7 @@
 // the reference's two-dispatch sequence. The filter writes a second image instead of filtering in
 // place (the reference's in-place UAV update races with its own neighbour reads).
 #include "zr_common.cuh"
+#include "zr_planes.h"
 
 namespace zr
 {
@@ -323,7 +324,11 @@ struct zr_compositing_pass
 {
     // Compositing (Compositing/Compositing.h): owns the LIGHT_ACCUM image (RGBA32F)
     uint32_t width = 0, height = 0;
-    float4* d_composited = nullptr;     // output of compositing (fused with the firefly filter when it is on)
+    struct Sized
+    {
+        zr::Planes planes{ "zr_compositing_pass" };
+        float4* d_composited = nullptr;     // output of compositing (fused with the firefly filter when it is on); never cleared
+    } sz;
     zr_compositing_params params{ 1, 1, 1 };
     uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
     void SetRows(zr::PostParams& p, dim3& grid) const
@@ -332,18 +337,15 @@ struct zr_compositing_pass
         grid = dim3((width + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8);
     }
 
-    zr_status Init(uint32_t w, uint32_t h) { return OnWindowResized(w, h); }
+    zr_status Setup() { return ZR_OK; }
     zr_status OnWindowResized(uint32_t w, uint32_t h)
     {
-        Release();
+        Sized next;
+        ZR_TRY(next.planes.Alloc(next.d_composited, (size_t)w * h, false));
+        sz = std::move(next);
         width = w; height = h;
-        ZR_CUDA(cudaMalloc(&d_composited, (size_t)w * h * sizeof(float4)));
+        rowBegin = 0; rowEnd = 0xffffffffu;
         return ZR_OK;
-    }
-    void Release()
-    {
-        if (d_composited) cudaFree(d_composited);
-        d_composited = nullptr;
     }
     zr_status Render(const zr_frame_inputs* in, const void* d_direct, const void* d_indirect, cudaStream_t stream)
     {
@@ -353,12 +355,8 @@ struct zr_compositing_pass
             set_error("zr_compositing_pass_render: missing G-buffer");
             return ZR_ERR_INVALID_ARG;
         }
-        if (in->frame.RenderWidth != width || in->frame.RenderHeight != height)
-        {
-            set_error("zr_compositing_pass_render: frame is %ux%u but the pass was sized %ux%u",
-                in->frame.RenderWidth, in->frame.RenderHeight, width, height);
-            return ZR_ERR_INVALID_ARG;
-        }
+        const zr_status st = check_frame_size("zr_compositing_pass", in->frame, width, height);
+        if (st != ZR_OK) return st;
         PostParams p = make_params(in->frame);
         const float4* direct = params.emissive_di ? (const float4*)d_direct : nullptr;
         const float4* indirect = params.indirect ? (const float4*)d_indirect : nullptr;
@@ -369,13 +367,13 @@ struct zr_compositing_pass
             const dim3 tgrid((width + FF_TW - 1) / FF_TW, (p.rowEnd - p.rowBegin + FF_TH - 1) / FF_TH);
             ZR_PROF("k_firefly", stream);
             k_firefly_tiled<<<tgrid, FF_TW * FF_TH, 0, stream>>>((const uint4*)in->curr.d_core, (const float*)in->curr.d_depth,
-                direct, indirect, d_composited, p);
+                direct, indirect, sz.d_composited, p);
             ZR_LAUNCH_CHECK();
         }
         else
         {
             ZR_PROF("k_compositing", stream);
-            k_compositing<<<grid, 256, 0, stream>>>((const uint4*)in->curr.d_core, direct, indirect, d_composited, p);
+            k_compositing<<<grid, 256, 0, stream>>>((const uint4*)in->curr.d_core, direct, indirect, sz.d_composited, p);
             ZR_LAUNCH_CHECK();
         }
         return ZR_OK;
@@ -386,29 +384,27 @@ struct zr_taa_pass
 {
     // TAA (TAA/TAA.h): two RGBA16F images, ping-ponged every Render (TAA.cpp:99-104)
     uint32_t width = 0, height = 0;
-    uint2* d_tex[2] = { nullptr, nullptr };
+    struct Sized
+    {
+        zr::Planes planes{ "zr_taa_pass" };
+        uint2* d_tex[2] = { nullptr, nullptr };
+    } sz;
     int outIdx = 0;
     bool isTemporalTexValid = false;
     float blendWeight = 0.1f;       // DefaultParamVals::BlendWeight
     uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
 
+    zr_status Setup() { return ZR_OK; }
     zr_status OnWindowResized(uint32_t w, uint32_t h)
     {
-        Release();
+        Sized next;
+        for (int i = 0; i < 2; i++) ZR_TRY(next.planes.Alloc(next.d_tex[i], (size_t)w * h));
+        ZR_TRY(next.planes.Clear());
+        sz = std::move(next);
         width = w; height = h;
-        ZR_CLEAR_BEGIN();
-        for (int i = 0; i < 2; i++)
-        {
-            ZR_CUDA(cudaMalloc(&d_tex[i], (size_t)w * h * sizeof(uint2)));
-            ZR_CUDA(cudaMemset(d_tex[i], 0, (size_t)w * h * sizeof(uint2)));
-        }
-        ZR_CLEAR_END();
+        rowBegin = 0; rowEnd = 0xffffffffu;
         isTemporalTexValid = false;
         return ZR_OK;
-    }
-    void Release()
-    {
-        for (int i = 0; i < 2; i++) { if (d_tex[i]) cudaFree(d_tex[i]); d_tex[i] = nullptr; }
     }
     zr_status Render(const zr_frame_inputs* in, const void* d_signal, cudaStream_t stream)
     {
@@ -418,11 +414,8 @@ struct zr_taa_pass
             set_error("zr_taa_pass_render: missing input");
             return ZR_ERR_INVALID_ARG;
         }
-        if (in->frame.RenderWidth != width || in->frame.RenderHeight != height)
-        {
-            set_error("zr_taa_pass_render: frame/pass size mismatch");
-            return ZR_ERR_INVALID_ARG;
-        }
+        const zr_status st = check_frame_size("zr_taa_pass", in->frame, width, height);
+        if (st != ZR_OK) return st;
         PostParams p = make_params(in->frame);
         p.blendWeight = blendWeight;
         p.temporalIsValid = isTemporalTexValid ? 1u : 0u;
@@ -431,7 +424,7 @@ struct zr_taa_pass
         outIdx ^= 1;
         ZR_PROF("k_taa", stream);
         k_taa<<<grid, 256, 0, stream>>>((const float*)in->curr.d_depth, (const uint2*)in->curr.d_motion_emissive,
-            (const float4*)d_signal, d_tex[outIdx ^ 1], d_tex[outIdx], p);
+            (const float4*)d_signal, sz.d_tex[outIdx ^ 1], sz.d_tex[outIdx], p);
         ZR_LAUNCH_CHECK();
         isTemporalTexValid = true;
         return ZR_OK;
@@ -440,20 +433,8 @@ struct zr_taa_pass
 
 extern "C"
 {
-    zr_status zr_compositing_pass_create(uint32_t width, uint32_t height, zr_compositing_pass** out)
-    {
-        if (!out || !width || !height) { zr::set_error("zr_compositing_pass_create: bad args"); return ZR_ERR_INVALID_ARG; }
-        zr_compositing_pass* p = new zr_compositing_pass();
-        zr_status s = p->Init(width, height);
-        if (s != ZR_OK) { delete p; return s; }
-        *out = p;
-        return ZR_OK;
-    }
-    zr_status zr_compositing_pass_resize(zr_compositing_pass* p, uint32_t width, uint32_t height)
-    {
-        if (!p) return ZR_ERR_INVALID_ARG;
-        return p->OnWindowResized(width, height);
-    }
+    zr_status zr_compositing_pass_create(uint32_t width, uint32_t height, zr_compositing_pass** out) { return zr::CreatePass("zr_compositing_pass", width, height, out); }
+    zr_status zr_compositing_pass_resize(zr_compositing_pass* p, uint32_t width, uint32_t height) { return zr::ResizePass("zr_compositing_pass", p, width, height); }
     zr_status zr_compositing_pass_set_params(zr_compositing_pass* p, const zr_compositing_params* params)
     {
         if (!p || !params) return ZR_ERR_INVALID_ARG;
@@ -475,25 +456,13 @@ extern "C"
     zr_status zr_compositing_pass_get_output(zr_compositing_pass* p, zr_image2d* out)
     {
         if (!p || !out) return ZR_ERR_INVALID_ARG;
-        *out = zr_image2d{ p->d_composited, p->width, p->height, p->width * 16u, 16u };
+        *out = zr_image2d{ p->sz.d_composited, p->width, p->height, p->width * 16u, 16u };
         return ZR_OK;
     }
-    void zr_compositing_pass_destroy(zr_compositing_pass* p) { if (p) { p->Release(); delete p; } }
+    void zr_compositing_pass_destroy(zr_compositing_pass* p) { delete p; }
 
-    zr_status zr_taa_pass_create(uint32_t width, uint32_t height, zr_taa_pass** out)
-    {
-        if (!out || !width || !height) { zr::set_error("zr_taa_pass_create: bad args"); return ZR_ERR_INVALID_ARG; }
-        zr_taa_pass* p = new zr_taa_pass();
-        zr_status s = p->OnWindowResized(width, height);
-        if (s != ZR_OK) { delete p; return s; }
-        *out = p;
-        return ZR_OK;
-    }
-    zr_status zr_taa_pass_resize(zr_taa_pass* p, uint32_t width, uint32_t height)
-    {
-        if (!p) return ZR_ERR_INVALID_ARG;
-        return p->OnWindowResized(width, height);
-    }
+    zr_status zr_taa_pass_create(uint32_t width, uint32_t height, zr_taa_pass** out) { return zr::CreatePass("zr_taa_pass", width, height, out); }
+    zr_status zr_taa_pass_resize(zr_taa_pass* p, uint32_t width, uint32_t height) { return zr::ResizePass("zr_taa_pass", p, width, height); }
     zr_status zr_taa_pass_set_rows(zr_taa_pass* p, uint32_t y0, uint32_t y1)
     {
         if (!p || y0 >= y1 || y0 >= p->height) { zr::set_error("zr_taa_pass_set_rows: empty row range"); return ZR_ERR_INVALID_ARG; }
@@ -514,8 +483,8 @@ extern "C"
     zr_status zr_taa_pass_get_output(zr_taa_pass* p, zr_image2d* out)
     {
         if (!p || !out) return ZR_ERR_INVALID_ARG;
-        *out = zr_image2d{ p->d_tex[p->outIdx], p->width, p->height, p->width * 8u, 8u };
+        *out = zr_image2d{ p->sz.d_tex[p->outIdx], p->width, p->height, p->width * 8u, 8u };
         return ZR_OK;
     }
-    void zr_taa_pass_destroy(zr_taa_pass* p) { if (p) { p->Release(); delete p; } }
+    void zr_taa_pass_destroy(zr_taa_pass* p) { delete p; }
 }

@@ -9,6 +9,7 @@
 // the RGBA16F target plane is a uint2 (8 B/px). k_di_spatial keeps the reference's 8x8 group / swizzle so one
 // warp is one reference wave (the disocclusion vote is a wave op) and the group RNG is seeded by the block id.
 #include "zr_pixel.cuh"
+#include "zr_planes.h"
 #include "zr_schedule.h"
 
 #include "zr_rdi.cuh"
@@ -240,48 +241,48 @@ namespace
 struct zr_direct_pass
 {
     uint32_t width = 0, height = 0;
-    zr_rdi_reservoir* d_res[2] = { nullptr, nullptr };
-    uint2* d_target = nullptr;      // RGBA16F
-    float4* d_final = nullptr;
+    struct Sized
+    {
+        zr::Planes planes{ "zr_direct_pass" };
+        zr_rdi_reservoir* d_res[2] = { nullptr, nullptr };
+        uint2* d_target = nullptr;      // RGBA16F
+        float4* d_final = nullptr;
+    } sz;
     int currTemporalIdx = 0;
     bool isTemporalReservoirValid = false;
     bool resetTemporalTextures = true;
     bool patternLoaded = false;
-    zr_direct_params params{};
+    zr_direct_params params = Defaults();
     zr::LightingStrip strip{ "zr_direct_pass" };     // both kernels share the 8x8-group block schedule
 
-    static void Defaults(zr_direct_params* p)
+    static zr_direct_params Defaults()
     {
         // DirectLighting.cpp:99-107, DirectLighting.h:93-98
-        p->temporal_resample = 1; p->spatial_resample = 1; p->stochastic_spatial = 1; p->extra_disocclusion_sampling = 1;
-        p->M_max = 20; p->alpha_min = 0.05f * 0.05f;
+        zr_direct_params p{};
+        p.temporal_resample = 1; p.spatial_resample = 1; p.stochastic_spatial = 1; p.extra_disocclusion_sampling = 1;
+        p.M_max = 20; p.alpha_min = 0.05f * 0.05f;
+        return p;
     }
-    void Release()
-    {
-        for (int i = 0; i < 2; i++) { if (d_res[i]) cudaFree(d_res[i]); d_res[i] = nullptr; }
-        strip.Release();
-        if (d_target) cudaFree(d_target); if (d_final) cudaFree(d_final);
-        d_target = nullptr; d_final = nullptr;
-    }
+    zr_status Setup() { return ZR_OK; }
     zr_status OnWindowResized(uint32_t w, uint32_t h)
     {
-        Release();
-        width = w; height = h;
         const size_t n = (size_t)w * h;
-        for (int i = 0; i < 2; i++) ZR_CUDA(cudaMalloc(&d_res[i], n * sizeof(zr_rdi_reservoir)));
-        ZR_CUDA(cudaMalloc(&d_target, n * 8));
-        ZR_CUDA(cudaMalloc(&d_final, n * 16));
-        return ResetTemporal();
+        Sized next;
+        for (int i = 0; i < 2; i++) ZR_TRY(next.planes.Alloc(next.d_res[i], n));
+        ZR_TRY(next.planes.Alloc(next.d_target, n));
+        ZR_TRY(next.planes.Alloc(next.d_final, n));
+        ZR_TRY(next.planes.Clear());
+        sz = std::move(next);
+        width = w; height = h;
+        strip.ForgetSize();
+        ResetFlags();
+        return ZR_OK;
     }
+    void ResetFlags() { currTemporalIdx = 0; isTemporalReservoirValid = false; resetTemporalTextures = true; }
     zr_status ResetTemporal()
     {
-        const size_t n = (size_t)width * height;
-        ZR_CLEAR_BEGIN();
-        for (int i = 0; i < 2; i++) ZR_CUDA(cudaMemset(d_res[i], 0, n * sizeof(zr_rdi_reservoir)));
-        ZR_CUDA(cudaMemset(d_target, 0, n * 8));
-        ZR_CUDA(cudaMemset(d_final, 0, n * 16));
-        ZR_CLEAR_END();
-        currTemporalIdx = 0; isTemporalReservoirValid = false; resetTemporalTextures = true;
+        ZR_TRY(sz.planes.Clear());
+        ResetFlags();
         return ZR_OK;
     }
     zr_status LoadPattern()
@@ -317,14 +318,14 @@ struct zr_direct_pass
         if (st != ZR_OK) return st;
         const BlockSchedule& sched = strip.sched;
         ZR_PROF("k_di_temporal", stream);
-        k_di_temporal<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, d_res[cur], d_res[1 - cur], d_target, d_final, dispX, dispY, sched.d_order);
+        k_di_temporal<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, dispX, dispY, sched.d_order);
         ZR_LAUNCH_CHECK();
         // the temporal output is what neighbours read in the spatial pass and what the next frame reprojects into
-        strip.Exchange(d_res[cur], width, height, 32u, stream);
+        strip.Exchange(sz.d_res[cur], width, height, 32u, stream);
         if (doSpatial)
         {
             ZR_PROF("k_di_spatial", stream);
-            k_di_spatial<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, d_res[cur], d_target, d_final, dispX, dispY, sched.d_order);
+            k_di_spatial<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY, sched.d_order);
             ZR_LAUNCH_CHECK();
         }
         isTemporalReservoirValid = true;
@@ -336,28 +337,10 @@ struct zr_direct_pass
 
 extern "C"
 {
-    zr_status zr_direct_pass_create(uint32_t width, uint32_t height, zr_direct_pass** out)
-    {
-        if (!out || !width || !height) { zr::set_error("zr_direct_pass_create: bad args"); return ZR_ERR_INVALID_ARG; }
-        zr_direct_pass* p = new zr_direct_pass();
-        zr_direct_pass::Defaults(&p->params);
-        zr_status s = p->OnWindowResized(width, height);
-        if (s != ZR_OK) { p->Release(); delete p; return s; }
-        *out = p;
-        return ZR_OK;
-    }
-    zr_status zr_direct_pass_resize(zr_direct_pass* p, uint32_t width, uint32_t height)
-    {
-        if (!p || !width || !height) return ZR_ERR_INVALID_ARG;
-        return p->OnWindowResized(width, height);
-    }
-    zr_status zr_direct_pass_reset_temporal(zr_direct_pass* p) { return p ? p->ResetTemporal() : ZR_ERR_INVALID_ARG; }
-    zr_status zr_direct_pass_default_params(zr_direct_params* out)
-    {
-        if (!out) return ZR_ERR_INVALID_ARG;
-        zr_direct_pass::Defaults(out);
-        return ZR_OK;
-    }
+    zr_status zr_direct_pass_create(uint32_t width, uint32_t height, zr_direct_pass** out) { return zr::CreatePass("zr_direct_pass", width, height, out); }
+    zr_status zr_direct_pass_resize(zr_direct_pass* p, uint32_t width, uint32_t height) { return zr::ResizePass("zr_direct_pass", p, width, height); }
+    zr_status zr_direct_pass_reset_temporal(zr_direct_pass* p) { return zr::ResetPass(p); }
+    zr_status zr_direct_pass_default_params(zr_direct_params* out) { return zr::DefaultParams<zr_direct_pass>(out); }
     zr_status zr_direct_pass_set_params(zr_direct_pass* p, const zr_direct_params* params)
     {
         if (!p || !params) return ZR_ERR_INVALID_ARG;
@@ -383,9 +366,9 @@ extern "C"
         const uint32_t w = p->width, h = p->height;
         switch (id)
         {
-        case ZR_DIRECT_FINAL: *out = zr_image2d{ p->d_final, w, h, w * 16u, 16u }; break;
-        case ZR_DIRECT_RESERVOIR_CURR: *out = zr_image2d{ p->d_res[1 - p->currTemporalIdx], w, h, w * 32u, 32u }; break;
-        case ZR_DIRECT_TARGET: *out = zr_image2d{ p->d_target, w, h, w * 8u, 8u }; break;
+        case ZR_DIRECT_FINAL: *out = zr_image2d{ p->sz.d_final, w, h, w * 16u, 16u }; break;
+        case ZR_DIRECT_RESERVOIR_CURR: *out = zr_image2d{ p->sz.d_res[1 - p->currTemporalIdx], w, h, w * 32u, 32u }; break;
+        case ZR_DIRECT_TARGET: *out = zr_image2d{ p->sz.d_target, w, h, w * 8u, 8u }; break;
         default: zr::set_error("zr_direct_pass_get_output: unknown output id"); return ZR_ERR_INVALID_ARG;
         }
         return ZR_OK;
@@ -401,5 +384,5 @@ extern "C"
         *n = 5;
         return ZR_OK;
     }
-    void zr_direct_pass_destroy(zr_direct_pass* p) { if (p) { p->Release(); delete p; } }
+    void zr_direct_pass_destroy(zr_direct_pass* p) { delete p; }
 }

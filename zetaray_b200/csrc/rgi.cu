@@ -20,6 +20,7 @@
 #define ZR_NO_DEGENERATE_RAY_EARLY_OUT
 #include "zr_pixel.cuh"
 #include "zr_rpt.cuh"       // ZR_PHASE
+#include "zr_planes.h"
 #include "zr_schedule.h"
 
 #include "zr_rgi.cuh"
@@ -285,47 +286,48 @@ namespace
 struct zr_gi_pass
 {
     uint32_t width = 0, height = 0;
-    zr_rgi_reservoir* d_res[2] = { nullptr, nullptr };
-    float4* d_final = nullptr;
+    struct Sized
+    {
+        zr::Planes planes{ "zr_gi_pass" };
+        zr_rgi_reservoir* d_res[2] = { nullptr, nullptr };
+        float4* d_final = nullptr;
+    } sz;
     int currTemporalIdx = 0;
     bool isTemporalReservoirValid = false;
     bool resetTemporalTextures = true;
-    zr_gi_params params{};
+    zr_gi_params params = Defaults();
     bool plainPathTracer = false;       // INTEGRATOR::PATH_TRACING instead of ReSTIR_GI (both read cb_ReSTIR_GI in the reference)
     // the hook makes the reservoirs just written coherent across strips (they are next frame's temporal candidates, searched up to
     // 16 px around the reprojected pixel: ReSTIR_GI/Params.hlsli:45); no tile costs are ever set, so blocks run in plain order
     zr::LightingStrip strip{ "zr_gi_pass" };
 
-    static void Defaults(zr_gi_params* p)
+    static zr_gi_params Defaults()
     {
         // IndirectLighting.h:231-244, IndirectLighting.cpp:143-160
-        p->max_non_tr_bounces = 3; p->max_glossy_tr_bounces = 4; p->russian_roulette = 1; p->stochastic_multi_bounce = 1;
-        p->boiling_suppression = 1; p->M_max = 10; p->temporal_resample = 1;
+        zr_gi_params p{};
+        p.max_non_tr_bounces = 3; p.max_glossy_tr_bounces = 4; p.russian_roulette = 1; p.stochastic_multi_bounce = 1;
+        p.boiling_suppression = 1; p.M_max = 10; p.temporal_resample = 1;
+        return p;
     }
-    void Release()
-    {
-        for (int i = 0; i < 2; i++) { if (d_res[i]) cudaFree(d_res[i]); d_res[i] = nullptr; }
-        if (d_final) cudaFree(d_final);
-        d_final = nullptr;
-        strip.Release();
-    }
+    zr_status Setup() { return ZR_OK; }
     zr_status OnWindowResized(uint32_t w, uint32_t h)
     {
-        Release();
-        width = w; height = h;
         const size_t n = (size_t)w * h;
-        for (int i = 0; i < 2; i++) ZR_CUDA(cudaMalloc(&d_res[i], n * sizeof(zr_rgi_reservoir)));
-        ZR_CUDA(cudaMalloc(&d_final, n * 16));
-        return ResetTemporal();
+        Sized next;
+        for (int i = 0; i < 2; i++) ZR_TRY(next.planes.Alloc(next.d_res[i], n));
+        ZR_TRY(next.planes.Alloc(next.d_final, n));
+        ZR_TRY(next.planes.Clear());
+        sz = std::move(next);
+        width = w; height = h;
+        strip.ForgetSize();
+        ResetFlags();
+        return ZR_OK;
     }
+    void ResetFlags() { currTemporalIdx = 0; isTemporalReservoirValid = false; resetTemporalTextures = true; }
     zr_status ResetTemporal()
     {
-        const size_t n = (size_t)width * height;
-        ZR_CLEAR_BEGIN();
-        for (int i = 0; i < 2; i++) ZR_CUDA(cudaMemset(d_res[i], 0, n * sizeof(zr_rgi_reservoir)));
-        ZR_CUDA(cudaMemset(d_final, 0, n * 16));
-        ZR_CLEAR_END();
-        currTemporalIdx = 0; isTemporalReservoirValid = false; resetTemporalTextures = true;
+        ZR_TRY(sz.planes.Clear());
+        ResetFlags();
         return ZR_OK;
     }
     zr_status Render(const zr_frame_inputs* in, cudaStream_t stream)
@@ -355,14 +357,14 @@ struct zr_gi_pass
         if (plainPathTracer)
         {
             ZR_PROF("k_pathtracer", stream);
-            k_rgi<true><<<sched.count, ZR_RGI_THREADS, 0, stream>>>(in->scene->dev, f, prm, d_res[cur], d_res[1 - cur], d_final, dispX, dispY, sched.d_order);
+            k_rgi<true><<<sched.count, ZR_RGI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_final, dispX, dispY, sched.d_order);
             ZR_LAUNCH_CHECK();
             return ZR_OK;       // no reservoirs: the ReSTIR GI history is left as it is (and is dropped by SetMethod)
         }
         ZR_PROF("k_rgi", stream);
-        k_rgi<false><<<sched.count, ZR_RGI_THREADS, 0, stream>>>(in->scene->dev, f, prm, d_res[cur], d_res[1 - cur], d_final, dispX, dispY, sched.d_order);
+        k_rgi<false><<<sched.count, ZR_RGI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_final, dispX, dispY, sched.d_order);
         ZR_LAUNCH_CHECK();
-        strip.Exchange(d_res[cur], width, height, (uint32_t)sizeof(zr_rgi_reservoir), stream);
+        strip.Exchange(sz.d_res[cur], width, height, (uint32_t)sizeof(zr_rgi_reservoir), stream);
         isTemporalReservoirValid = true;
         currTemporalIdx = 1 - cur;
         resetTemporalTextures = false;
@@ -372,28 +374,10 @@ struct zr_gi_pass
 
 extern "C"
 {
-    zr_status zr_gi_pass_create(uint32_t width, uint32_t height, zr_gi_pass** out)
-    {
-        if (!out || !width || !height) { zr::set_error("zr_gi_pass_create: bad args"); return ZR_ERR_INVALID_ARG; }
-        zr_gi_pass* p = new zr_gi_pass();
-        zr_gi_pass::Defaults(&p->params);
-        zr_status s = p->OnWindowResized(width, height);
-        if (s != ZR_OK) { p->Release(); delete p; return s; }
-        *out = p;
-        return ZR_OK;
-    }
-    zr_status zr_gi_pass_resize(zr_gi_pass* p, uint32_t width, uint32_t height)
-    {
-        if (!p || !width || !height) return ZR_ERR_INVALID_ARG;
-        return p->OnWindowResized(width, height);
-    }
-    zr_status zr_gi_pass_reset_temporal(zr_gi_pass* p) { return p ? p->ResetTemporal() : ZR_ERR_INVALID_ARG; }
-    zr_status zr_gi_pass_default_params(zr_gi_params* out)
-    {
-        if (!out) return ZR_ERR_INVALID_ARG;
-        zr_gi_pass::Defaults(out);
-        return ZR_OK;
-    }
+    zr_status zr_gi_pass_create(uint32_t width, uint32_t height, zr_gi_pass** out) { return zr::CreatePass("zr_gi_pass", width, height, out); }
+    zr_status zr_gi_pass_resize(zr_gi_pass* p, uint32_t width, uint32_t height) { return zr::ResizePass("zr_gi_pass", p, width, height); }
+    zr_status zr_gi_pass_reset_temporal(zr_gi_pass* p) { return zr::ResetPass(p); }
+    zr_status zr_gi_pass_default_params(zr_gi_params* out) { return zr::DefaultParams<zr_gi_pass>(out); }
     zr_status zr_gi_pass_set_params(zr_gi_pass* p, const zr_gi_params* params)
     {
         if (!p || !params) return ZR_ERR_INVALID_ARG;
@@ -433,12 +417,12 @@ extern "C"
         const uint32_t w = p->width, h = p->height;
         switch (id)
         {
-        case ZR_GI_FINAL: *out = zr_image2d{ p->d_final, w, h, w * 16u, 16u }; break;
-        case ZR_GI_RESERVOIR_CURR: *out = zr_image2d{ p->d_res[1 - p->currTemporalIdx], w, h, w * 48u, 48u }; break;
-        case ZR_GI_RESERVOIR_PREV: *out = zr_image2d{ p->d_res[p->currTemporalIdx], w, h, w * 48u, 48u }; break;
+        case ZR_GI_FINAL: *out = zr_image2d{ p->sz.d_final, w, h, w * 16u, 16u }; break;
+        case ZR_GI_RESERVOIR_CURR: *out = zr_image2d{ p->sz.d_res[1 - p->currTemporalIdx], w, h, w * 48u, 48u }; break;
+        case ZR_GI_RESERVOIR_PREV: *out = zr_image2d{ p->sz.d_res[p->currTemporalIdx], w, h, w * 48u, 48u }; break;
         default: zr::set_error("zr_gi_pass_get_output: unknown output id"); return ZR_ERR_INVALID_ARG;
         }
         return ZR_OK;
     }
-    void zr_gi_pass_destroy(zr_gi_pass* p) { if (p) { p->Release(); delete p; } }
+    void zr_gi_pass_destroy(zr_gi_pass* p) { delete p; }
 }

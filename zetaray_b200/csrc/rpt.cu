@@ -524,56 +524,37 @@ namespace
 struct zr_indirect_pass
 {
     uint32_t width = 0, height = 0;
-    zr_rpt_reservoir* d_res[2] = { nullptr, nullptr };
-    float4* d_target = nullptr;
-    float4* d_final = nullptr;
-    uint16_t* d_neighbor = nullptr;
-    uint16_t* d_threadMap[2] = { nullptr, nullptr };   // CtN, NtC
+    struct Sized
+    {
+        zr::Planes planes{ "zr_indirect_pass" };
+        zr_rpt_reservoir* d_res[2] = { nullptr, nullptr };
+        float4* d_target = nullptr;
+        float4* d_final = nullptr;
+        uint16_t* d_neighbor = nullptr;
+        uint16_t* d_threadMap = nullptr;    // NtC
+        // temporal and spatial reuse: per-case shift queues + streaming merge (rpt_temporal.cu, rpt_spatial.cu)
+        zr::SpatialQueued queued;
+    } sz;
+    zr::ShiftStreams shiftStreams;
     int currTemporalIdx = 0;
     bool isTemporalReservoirValid = false;
     bool resetTemporalTextures = true;
     bool patternLoaded = false;
     zr::LightingStrip strip{ "zr_indirect_pass" };  // the block schedule is k_pathtrace's
-    // temporal and spatial reuse: per-case shift queues + streaming merge (rpt_temporal.cu, rpt_spatial.cu)
-    zr::SpatialQueued spatialQueued;
-    zr::TemporalQueued temporalQueued;
-    zr_indirect_params params{};
+    zr_indirect_params params = Defaults();
 
-    static void Defaults(zr_indirect_params* p)
+    static zr_indirect_params Defaults()
     {
         // IndirectLighting.h:231-244, IndirectLighting.cpp:146-165
-        p->max_non_tr_bounces = 3; p->max_glossy_tr_bounces = 4; p->russian_roulette = 1; p->temporal_resample = 1;
-        p->num_spatial_passes = 1; p->M_max_temporal = 10; p->M_max_spatial = 8; p->boiling_suppression = 1;
-        p->sort_temporal = 1; p->sort_spatial = 1; p->alpha_min = 0.175f * 0.175f;
+        zr_indirect_params p{};
+        p.max_non_tr_bounces = 3; p.max_glossy_tr_bounces = 4; p.russian_roulette = 1; p.temporal_resample = 1;
+        p.num_spatial_passes = 1; p.M_max_temporal = 10; p.M_max_spatial = 8; p.boiling_suppression = 1;
+        p.sort_temporal = 1; p.sort_spatial = 1; p.alpha_min = 0.175f * 0.175f;
+        return p;
     }
 
-    void Release()
+    zr_status Setup()
     {
-        for (int i = 0; i < 2; i++) { if (d_res[i]) cudaFree(d_res[i]); d_res[i] = nullptr; if (d_threadMap[i]) cudaFree(d_threadMap[i]); d_threadMap[i] = nullptr; }
-        strip.Release();
-        spatialQueued.Release();
-        temporalQueued.Release();
-        if (d_target) cudaFree(d_target); if (d_final) cudaFree(d_final); if (d_neighbor) cudaFree(d_neighbor);
-        d_target = d_final = nullptr; d_neighbor = nullptr;
-    }
-
-    zr_status OnWindowResized(uint32_t w, uint32_t h)
-    {
-        Release();
-        width = w; height = h;
-        const size_t n = (size_t)w * h;
-        for (int i = 0; i < 2; i++)
-        {
-            ZR_CUDA(cudaMalloc(&d_res[i], n * sizeof(zr_rpt_reservoir)));
-            ZR_CUDA(cudaMalloc(&d_threadMap[i], n * 2));
-        }
-        ZR_CUDA(cudaMalloc(&d_target, n * 16));
-        ZR_CUDA(cudaMalloc(&d_final, n * 16));
-        ZR_CUDA(cudaMalloc(&d_neighbor, n * 2));
-        zr_status st = spatialQueued.Resize(w, h, d_res[0], d_res[1]);
-        if (st != ZR_OK) return st;
-        st = temporalQueued.Resize(w, h);
-        if (st != ZR_OK) return st;
         // k_pathtrace's parked state needs more than the 48 KB of static shared memory. The carveout asks for just the shared
         // memory its resident blocks use (plus the 1 KB the system reserves per block); the rest of the 256 KB stays L1 for
         // what still spills.
@@ -588,25 +569,32 @@ struct zr_indirect_pass
         const size_t ptSmem = (size_t)ptBlocks * (zr::PT_SMEM_BYTES + 1024);
         ZR_CUDA(cudaFuncSetAttribute(zr::k_pathtrace, cudaFuncAttributePreferredSharedMemoryCarveout,
             (int)((ptSmem * 100 + 228 * 1024 - 1) / (228 * 1024))));
-        return ResetTemporal();
+        return shiftStreams.Init();
     }
 
+    zr_status OnWindowResized(uint32_t w, uint32_t h)
+    {
+        const size_t n = (size_t)w * h;
+        Sized next;
+        for (int i = 0; i < 2; i++) ZR_TRY(next.planes.Alloc(next.d_res[i], n));
+        ZR_TRY(next.planes.Alloc(next.d_threadMap, n));
+        ZR_TRY(next.planes.Alloc(next.d_target, n));
+        ZR_TRY(next.planes.Alloc(next.d_final, n));
+        ZR_TRY(next.planes.Alloc(next.d_neighbor, n));
+        ZR_TRY(next.queued.Build(w, h, next.d_res[0], next.d_res[1]));
+        ZR_TRY(next.planes.Clear());
+        sz = std::move(next);
+        width = w; height = h;
+        strip.ForgetSize();
+        ResetFlags();
+        return ZR_OK;
+    }
+
+    void ResetFlags() { currTemporalIdx = 0; isTemporalReservoirValid = false; resetTemporalTextures = true; }
     zr_status ResetTemporal()
     {
-        const size_t n = (size_t)width * height;
-        ZR_CLEAR_BEGIN();
-        for (int i = 0; i < 2; i++)
-        {
-            ZR_CUDA(cudaMemset(d_res[i], 0, n * sizeof(zr_rpt_reservoir)));
-            ZR_CUDA(cudaMemset(d_threadMap[i], 0, n * 2));
-        }
-        ZR_CUDA(cudaMemset(d_target, 0, n * 16));
-        ZR_CUDA(cudaMemset(d_final, 0, n * 16));
-        ZR_CUDA(cudaMemset(d_neighbor, 0, n * 2));
-        ZR_CLEAR_END();
-        currTemporalIdx = 0;
-        isTemporalReservoirValid = false;
-        resetTemporalTextures = true;
+        ZR_TRY(sz.planes.Clear());
+        ResetFlags();
         return ZR_OK;
     }
 
@@ -651,35 +639,35 @@ struct zr_indirect_pass
         int cur = currTemporalIdx;
         const uint32_t dispX = (width + 15) / 16, dispY = (height + 7) / 8;
         ZR_PROF("k_pathtrace", stream);
-        k_pathtrace<<<strip.sched.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, d_res[cur], d_target, d_final, dispX, dispY,
+        k_pathtrace<<<strip.sched.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY,
             strip.sched.d_order);
         ZR_LAUNCH_CHECK();
         if (doTemporal)
         {
-            st = temporalQueued.Run(spatialQueued, in->scene->dev, f, prm, d_res[cur], d_res[1 - cur], d_target, d_final, stream);
+            st = sz.queued.RunTemporal(shiftStreams, in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, stream);
             if (st != ZR_OK) return st;
         }
         // reservoirs written so far are read by neighbours (spatial pass) and by the next frame's temporal pass
-        strip.Exchange(d_res[cur], width, height, 64u, stream);
+        strip.Exchange(sz.d_res[cur], width, height, 64u, stream);
         if (doSpatial)
         {
             for (uint32_t pass = 0; pass < params.num_spatial_passes; pass++)
             {
                 ZR_PROF("k_spatial_search", stream);
-                k_spatial_search<<<dim3((width + 31) / 32, (rows + 7) / 8), 256, 0, stream>>>(f, prm, d_neighbor);
+                k_spatial_search<<<dim3((width + 31) / 32, (rows + 7) / 8), 256, 0, stream>>>(f, prm, sz.d_neighbor);
                 ZR_LAUNCH_CHECK();
-                zr_rpt_reservoir* rin = d_res[cur];
-                zr_rpt_reservoir* rout = d_res[1 - cur];
+                zr_rpt_reservoir* rin = sz.d_res[cur];
+                zr_rpt_reservoir* rout = sz.d_res[1 - cur];
                 cur = 1 - cur;
                 if (params.sort_spatial)
                 {
                     const uint32_t sx = (width + 31) / 32, sy = (height + 31) / 32;
                     ZR_PROF("k_sort", stream);
                     const uint32_t ty0 = prm.rowBegin / 32, ty1 = (prm.rowEnd + 31) / 32;
-                    k_sort<<<dim3(sx, ty1 - ty0), 256, 0, stream>>>(f, 3, 1u, rin, nullptr, d_neighbor, d_threadMap[1], sx, sy, ty0);
+                    k_sort<<<dim3(sx, ty1 - ty0), 256, 0, stream>>>(f, 3, 1u, rin, nullptr, sz.d_neighbor, sz.d_threadMap, sx, sy, ty0);
                     ZR_LAUNCH_CHECK();
                 }
-                st = spatialQueued.Run(in->scene->dev, f, prm, rin, rout, d_target, d_final, d_neighbor, d_threadMap[1], stream);
+                st = sz.queued.Run(shiftStreams, in->scene->dev, f, prm, rin, rout, sz.d_target, sz.d_final, sz.d_neighbor, sz.d_threadMap, stream);
                 if (st != ZR_OK) return st;
                 strip.Exchange(rout, width, height, 64u, stream);
             }
@@ -693,28 +681,10 @@ struct zr_indirect_pass
 
 extern "C"
 {
-    zr_status zr_indirect_pass_create(uint32_t width, uint32_t height, zr_indirect_pass** out)
-    {
-        if (!out || !width || !height) { zr::set_error("zr_indirect_pass_create: bad args"); return ZR_ERR_INVALID_ARG; }
-        zr_indirect_pass* p = new zr_indirect_pass();
-        zr_indirect_pass::Defaults(&p->params);
-        zr_status s = p->OnWindowResized(width, height);
-        if (s != ZR_OK) { p->Release(); delete p; return s; }
-        *out = p;
-        return ZR_OK;
-    }
-    zr_status zr_indirect_pass_resize(zr_indirect_pass* p, uint32_t width, uint32_t height)
-    {
-        if (!p || !width || !height) return ZR_ERR_INVALID_ARG;
-        return p->OnWindowResized(width, height);
-    }
-    zr_status zr_indirect_pass_reset_temporal(zr_indirect_pass* p) { return p ? p->ResetTemporal() : ZR_ERR_INVALID_ARG; }
-    zr_status zr_indirect_pass_default_params(zr_indirect_params* out)
-    {
-        if (!out) return ZR_ERR_INVALID_ARG;
-        zr_indirect_pass::Defaults(out);
-        return ZR_OK;
-    }
+    zr_status zr_indirect_pass_create(uint32_t width, uint32_t height, zr_indirect_pass** out) { return zr::CreatePass("zr_indirect_pass", width, height, out); }
+    zr_status zr_indirect_pass_resize(zr_indirect_pass* p, uint32_t width, uint32_t height) { return zr::ResizePass("zr_indirect_pass", p, width, height); }
+    zr_status zr_indirect_pass_reset_temporal(zr_indirect_pass* p) { return zr::ResetPass(p); }
+    zr_status zr_indirect_pass_default_params(zr_indirect_params* out) { return zr::DefaultParams<zr_indirect_pass>(out); }
     zr_status zr_indirect_pass_set_params(zr_indirect_pass* p, const zr_indirect_params* params)
     {
         if (!p || !params) return ZR_ERR_INVALID_ARG;
@@ -738,14 +708,13 @@ extern "C"
         const uint32_t w = p->width, h = p->height;
         switch (id)
         {
-        case ZR_INDIRECT_FINAL: *out = zr_image2d{ p->d_final, w, h, w * 16u, 16u }; break;
+        case ZR_INDIRECT_FINAL: *out = zr_image2d{ p->sz.d_final, w, h, w * 16u, 16u }; break;
         // after Render() the frame's output reservoirs are the ones the NEXT frame will call "previous"
-        case ZR_INDIRECT_RESERVOIR_CURR: *out = zr_image2d{ p->d_res[1 - p->currTemporalIdx], w, h, w * 64u, 64u }; break;
-        case ZR_INDIRECT_RESERVOIR_PREV: *out = zr_image2d{ p->d_res[p->currTemporalIdx], w, h, w * 64u, 64u }; break;
-        case ZR_INDIRECT_TARGET: *out = zr_image2d{ p->d_target, w, h, w * 16u, 16u }; break;
-        case ZR_INDIRECT_NEIGHBOR: *out = zr_image2d{ p->d_neighbor, w, h, w * 2u, 2u }; break;
-        case ZR_INDIRECT_THREADMAP_CTN: *out = zr_image2d{ p->d_threadMap[0], w, h, w * 2u, 2u }; break;
-        case ZR_INDIRECT_THREADMAP_NTC: *out = zr_image2d{ p->d_threadMap[1], w, h, w * 2u, 2u }; break;
+        case ZR_INDIRECT_RESERVOIR_CURR: *out = zr_image2d{ p->sz.d_res[1 - p->currTemporalIdx], w, h, w * 64u, 64u }; break;
+        case ZR_INDIRECT_RESERVOIR_PREV: *out = zr_image2d{ p->sz.d_res[p->currTemporalIdx], w, h, w * 64u, 64u }; break;
+        case ZR_INDIRECT_TARGET: *out = zr_image2d{ p->sz.d_target, w, h, w * 16u, 16u }; break;
+        case ZR_INDIRECT_NEIGHBOR: *out = zr_image2d{ p->sz.d_neighbor, w, h, w * 2u, 2u }; break;
+        case ZR_INDIRECT_THREADMAP_NTC: *out = zr_image2d{ p->sz.d_threadMap, w, h, w * 2u, 2u }; break;
         default: zr::set_error("zr_indirect_pass_get_output: unknown output id"); return ZR_ERR_INVALID_ARG;
         }
         return ZR_OK;
@@ -769,5 +738,5 @@ extern "C"
     }
     zr_status zr_indirect_pass_set_cost_map(zr_indirect_pass* p, void* d_cycles) { return p ? p->strip.SetCostMap(d_cycles) : ZR_ERR_INVALID_ARG; }
     zr_status zr_indirect_pass_set_rows(zr_indirect_pass* p, uint32_t y0, uint32_t y1) { return p ? p->strip.SetRows(y0, y1, p->height) : ZR_ERR_INVALID_ARG; }
-    void zr_indirect_pass_destroy(zr_indirect_pass* p) { if (p) { p->Release(); delete p; } }
+    void zr_indirect_pass_destroy(zr_indirect_pass* p) { delete p; }
 }

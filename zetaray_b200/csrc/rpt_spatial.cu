@@ -321,59 +321,8 @@ namespace
 // -------------------------------------------------------------------------------------------------------------------
 // host side
 // -------------------------------------------------------------------------------------------------------------------
-void SpatialQueued::Release()
+zr_status ShiftStreams::Init()
 {
-    if (d_queue) cudaFree(d_queue);
-    if (d_counters) cudaFree(d_counters);
-    if (d_shift) cudaFree(d_shift);
-    if (d_maps) cudaFree(d_maps);
-    for (int i = 0; i < 2; i++)
-    {
-        if (aux[i]) cudaStreamDestroy(aux[i]);
-        if (evJoin[i]) cudaEventDestroy(evJoin[i]);
-        aux[i] = nullptr; evJoin[i] = nullptr;
-    }
-    if (evFork) cudaEventDestroy(evFork);
-    evFork = nullptr;
-    d_queue = nullptr; d_counters = nullptr; d_shift = nullptr; d_maps = nullptr;
-    ready = false;
-}
-
-zr_status SpatialQueued::Resize(uint32_t w, uint32_t h, const zr_rpt_reservoir* res0, const zr_rpt_reservoir* res1)
-{
-    Release();
-    width = w; height = h;
-    const size_t n = (size_t)w * h;
-    capacity = 2 * n;
-    ZR_CUDA(cudaMalloc(&d_queue, NUM_CLASSES * capacity * sizeof(uint32_t)));
-    ZR_CUDA(cudaMalloc(&d_counters, 16 * sizeof(uint32_t)));
-    ZR_CUDA(cudaMalloc(&d_shift, n * sizeof(ShiftResult)));
-    ZR_CUDA(cudaMemset(d_shift, 0, n * sizeof(ShiftResult)));
-    const zr_rpt_reservoir* planes[2] = { res0, res1 };
-    swizzled = (w % 2) == 0;
-    for (int i = 0; i < 2; i++)
-    {
-        mapBase[i] = planes[i];
-        bool ok;
-        if (swizzled)
-        {
-            const uint64_t dims[3] = { 16, w / 2, h };
-            const uint64_t strides[2] = { 128, (uint64_t)w * 64 };
-            const uint32_t box[3] = { 16, 16, 32 };
-            ok = tma::EncodeWords(&mapRes[i], planes[i], 3, dims, strides, box, true);
-        }
-        else
-            ok = tma::EncodePlane2D(&mapRes[i], planes[i], w, h, 64, (uint64_t)w * 64, 32, 32);
-        if (!ok)
-        {
-            set_error("zr_indirect_pass: cuTensorMapEncodeTiled failed for the %ux%u reservoir plane", w, h);
-            return ZR_ERR_CUDA;
-        }
-    }
-    // the maps are read from global memory, one address per plane, written once here
-    ZR_CUDA(cudaMalloc(&d_maps, 2 * sizeof(CUtensorMap)));
-    ZR_CUDA(cudaMemcpy(d_maps, mapRes, 2 * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
-    ZR_CUDA(cudaDeviceSynchronize());
     int dev = 0;
     ZR_CUDA(cudaGetDevice(&dev));
     ZR_CUDA(cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev));
@@ -384,14 +333,58 @@ zr_status SpatialQueued::Resize(uint32_t w, uint32_t h, const zr_rpt_reservoir* 
         ZR_CUDA(cudaEventCreateWithFlags(&evJoin[i], cudaEventDisableTiming));
     }
     ZR_CUDA(cudaEventCreateWithFlags(&evFork, cudaEventDisableTiming));
-    ready = true;
     return ZR_OK;
 }
 
-zr_status SpatialQueued::Run(const SceneDev& sc, const FrameView& f, const RptParams& prm, const zr_rpt_reservoir* resIn,
+ShiftStreams::~ShiftStreams()
+{
+    for (int i = 0; i < 2; i++)
+    {
+        if (aux[i]) cudaStreamDestroy(aux[i]);
+        if (evJoin[i]) cudaEventDestroy(evJoin[i]);
+    }
+    if (evFork) cudaEventDestroy(evFork);
+}
+
+zr_status SpatialQueued::Build(uint32_t w, uint32_t h, const zr_rpt_reservoir* res0, const zr_rpt_reservoir* res1)
+{
+    width = w; height = h;
+    const size_t n = (size_t)w * h;
+    capacity = 2 * n;
+    ZR_TRY(planes.Alloc(d_queue, NUM_CLASSES * capacity, false));
+    ZR_TRY(planes.Alloc(d_counters, 16, false));
+    ZR_TRY(planes.Alloc(d_shift, n));
+    ZR_TRY(planes.Alloc(d_flags, n));
+    ZR_TRY(planes.Alloc(d_maps, 2, false));
+    const zr_rpt_reservoir* res[2] = { res0, res1 };
+    CUtensorMap maps[2];
+    swizzled = (w % 2) == 0;
+    for (int i = 0; i < 2; i++)
+    {
+        mapBase[i] = res[i];
+        bool ok;
+        if (swizzled)
+        {
+            const uint64_t dims[3] = { 16, w / 2, h };
+            const uint64_t strides[2] = { 128, (uint64_t)w * 64 };
+            const uint32_t box[3] = { 16, 16, 32 };
+            ok = tma::EncodeWords(&maps[i], res[i], 3, dims, strides, box, true);
+        }
+        else
+            ok = tma::EncodePlane2D(&maps[i], res[i], w, h, 64, (uint64_t)w * 64, 32, 32);
+        if (!ok)
+        {
+            set_error("zr_indirect_pass: cuTensorMapEncodeTiled failed for the %ux%u reservoir plane", w, h);
+            return ZR_ERR_CUDA;
+        }
+    }
+    ZR_CUDA(cudaMemcpy(d_maps, maps, sizeof(maps), cudaMemcpyHostToDevice));
+    return planes.Clear();
+}
+
+zr_status SpatialQueued::Run(const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm, const zr_rpt_reservoir* resIn,
     zr_rpt_reservoir* resOut, const float4* target, float4* finalImg, const uint16_t* neighbor, const uint16_t* threadMap, cudaStream_t stream)
 {
-    if (!ready) { set_error("zr_indirect_pass: queued spatial path is not initialised"); return ZR_ERR_NOT_INITIALIZED; }
     const int plane = resIn == mapBase[0] ? 0 : (resIn == mapBase[1] ? 1 : -1);
     if (plane < 0) { set_error("zr_indirect_pass: spatial input is not one of the pass's reservoir planes"); return ZR_ERR_INVALID_ARG; }
     const uint32_t rows = prm.rowEnd - prm.rowBegin;
@@ -403,7 +396,7 @@ zr_status SpatialQueued::Run(const SceneDev& sc, const FrameView& f, const RptPa
     }
     {
         ZR_PROF("k_shift", stream);
-        const zr_status ls = LaunchShifts<false>(*this, sc, f, prm, resIn, nullptr, neighbor, stream);
+        const zr_status ls = LaunchShifts<false>(*this, ss, sc, f, prm, resIn, nullptr, neighbor, stream);
         zr::prof_after();
         if (ls != ZR_OK) return ls;
         cudaError_t e = cudaGetLastError();
@@ -416,7 +409,7 @@ zr_status SpatialQueued::Run(const SceneDev& sc, const FrameView& f, const RptPa
         // A second form -- 512 threads x 2 co-resident blocks per SM, per-pixel state parked in shared memory between the phases -- was
         // bit-identical and no faster: the kernel waits for its global loads at 32 warps per
         // SM in either form. Removed again.
-        const uint32_t grid = numTiles < (uint32_t)numSMs ? numTiles : (uint32_t)numSMs;
+        const uint32_t grid = numTiles < (uint32_t)ss.numSMs ? numTiles : (uint32_t)ss.numSMs;
         ZR_PROF("k_spatial_merge", stream);
         k_spatial_merge<<<grid, 1024, sizeof(MergeSmem), stream>>>(d_maps + plane, f, prm, resIn, resOut, target, finalImg, neighbor, threadMap,
             d_shift, tilesX, tileRow0, numTiles, swizzled ? 1u : 0u);

@@ -185,35 +185,20 @@ namespace
     }
 }
 
-void TemporalQueued::Release()
-{
-    if (d_flags) cudaFree(d_flags);
-    d_flags = nullptr;
-}
-
-zr_status TemporalQueued::Resize(uint32_t w, uint32_t h)
-{
-    Release();
-    ZR_CUDA(cudaMalloc(&d_flags, (size_t)w * h));
-    ZR_CUDA(cudaMemset(d_flags, 0, (size_t)w * h));
-    return ZR_OK;
-}
-
-zr_status TemporalQueued::Run(SpatialQueued& q, const SceneDev& sc, const FrameView& f, const RptParams& prm, zr_rpt_reservoir* resCurr,
+zr_status SpatialQueued::RunTemporal(const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm, zr_rpt_reservoir* resCurr,
     const zr_rpt_reservoir* resPrev, float4* target, float4* finalImg, cudaStream_t stream)
 {
-    if (!q.ready || !d_flags) { set_error("zr_indirect_pass: queued temporal path is not initialised"); return ZR_ERR_NOT_INITIALIZED; }
     const uint32_t rows = prm.rowEnd - prm.rowBegin;
-    const dim3 grid((q.width + 31) / 32, (rows + 7) / 8);
-    ZR_CUDA(cudaMemsetAsync(q.d_counters, 0, 16 * sizeof(uint32_t), stream));
+    const dim3 grid((width + 31) / 32, (rows + 7) / 8);
+    ZR_CUDA(cudaMemsetAsync(d_counters, 0, 16 * sizeof(uint32_t), stream));
     {
         ZR_PROF("k_temporal_classify", stream);
-        k_temporal_classify<<<grid, 256, 0, stream>>>(sc, f, prm, resCurr, resPrev, d_flags, q.d_queue, q.d_counters, (uint32_t)q.capacity);
+        k_temporal_classify<<<grid, 256, 0, stream>>>(sc, f, prm, resCurr, resPrev, d_flags, d_queue, d_counters, (uint32_t)capacity);
         ZR_LAUNCH_CHECK();
     }
     {
         ZR_PROF("k_shift_temporal", stream);
-        const zr_status ls = LaunchShifts<true>(q, sc, f, prm, resCurr, resPrev, nullptr, stream);
+        const zr_status ls = LaunchShifts<true>(*this, ss, sc, f, prm, resCurr, resPrev, nullptr, stream);
         zr::prof_after();
         if (ls != ZR_OK) return ls;
         cudaError_t e = cudaGetLastError();
@@ -221,7 +206,7 @@ zr_status TemporalQueued::Run(SpatialQueued& q, const SceneDev& sc, const FrameV
     }
     {
         ZR_PROF("k_temporal_merge", stream);
-        k_temporal_merge<<<grid, 256, 0, stream>>>(sc, f, prm, resCurr, resPrev, target, finalImg, d_flags, q.d_shift);
+        k_temporal_merge<<<grid, 256, 0, stream>>>(sc, f, prm, resCurr, resPrev, target, finalImg, d_flags, d_shift);
         ZR_LAUNCH_CHECK();
     }
     return ZR_OK;

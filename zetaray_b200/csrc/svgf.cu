@@ -12,9 +12,9 @@
 // therefore reads 1.2-1.4x and writes 1.0x its algorithmic bytes from L2 / HBM at any step, with no strided global access.
 // Step 1 is the same kernel over a plain 2-D map (64 x 16 pixel tiles).
 #include "zr_common.cuh"
+#include "zr_planes.h"
 #include "zr_tma.cuh"
 #include <cstdlib>
-#include <cstring>
 
 namespace zr
 {
@@ -278,117 +278,110 @@ namespace
 struct zr_svgf_pass
 {
     static constexpr int MAX_PASSES = 5;
-    uint32_t width = 0, height = 0, pitch = 0, rows = 0;      // pitch / rows: padded plane size in pixels (OnWindowResized)
-    uint2* d_cv[2] = { nullptr, nullptr };
-    uint2* d_guide[2] = { nullptr, nullptr };
-    uint4* d_hist[2] = { nullptr, nullptr };
-    float4* d_out = nullptr;
+    uint32_t width = 0, height = 0;
+    struct Sized
+    {
+        zr::Planes planes{ "zr_svgf_pass" };
+        uint32_t pitch = 0, rows = 0;       // padded plane size in pixels
+        uint2* d_cv[2] = { nullptr, nullptr };
+        uint2* d_guide[2] = { nullptr, nullptr };
+        uint4* d_hist[2] = { nullptr, nullptr };
+        float4* d_out = nullptr;
+        CUtensorMap* d_maps = nullptr;      // [kind 0 = cv load, 1 = cv store, 2 = guide load][pass][plane]; load boxes depend on the radius
+    } sz;
     int cur = 0;
     bool historyValid = false;
-    zr_svgf_params params{};
-    // tensor maps: [pass][plane]; load boxes depend on the radius, store boxes do not
-    CUtensorMap mapCvLoad[MAX_PASSES][2], mapCvStore[MAX_PASSES][2], mapGuideLoad[MAX_PASSES][2];
-    CUtensorMap* d_maps = nullptr;      // device copy: [kind 0 = cv load, 1 = cv store, 2 = guide load][pass][plane]
-    const CUtensorMap* DevMap(int kind, int k, int plane) const { return d_maps + ((kind * MAX_PASSES + k) * 2 + plane); }
-    bool mapsReady = false;
+    zr_svgf_params params = Defaults();
+    const CUtensorMap* DevMap(int kind, int k, int plane) const { return sz.d_maps + ((kind * MAX_PASSES + k) * 2 + plane); }
 
-    static void Defaults(zr_svgf_params* p) { p->sigma_z = 0.02f; p->k_n = 16.0f; p->sigma_l = 4.0f; p->radius = 2; p->num_passes = 5; }
+    static zr_svgf_params Defaults() { zr_svgf_params p{}; p.sigma_z = 0.02f; p.k_n = 16.0f; p.sigma_l = 4.0f; p.radius = 2; p.num_passes = 5; return p; }
 
-    void Release()
-    {
-        for (int i = 0; i < 2; i++)
-        {
-            if (d_cv[i]) cudaFree(d_cv[i]); if (d_guide[i]) cudaFree(d_guide[i]); if (d_hist[i]) cudaFree(d_hist[i]);
-            d_cv[i] = nullptr; d_guide[i] = nullptr; d_hist[i] = nullptr;
-        }
-        if (d_out) cudaFree(d_out);
-        if (d_maps) cudaFree(d_maps);
-        d_out = nullptr; d_maps = nullptr; mapsReady = false;
-    }
-
-    zr_status EncodeMaps()
+    zr_status Setup()
     {
         using namespace zr;
-        const uint32_t R = params.radius;
+        cudaError_t e = cudaSuccess;
+#define ZR_SVGF_ATTR(R, P, LAST) \
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_svgf_atrous<R, P, LAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, AtrousTile<R, P>::BYTES)
+        ZR_SVGF_ATTR(1, 1, false); ZR_SVGF_ATTR(1, 1, true); ZR_SVGF_ATTR(1, 2, false); ZR_SVGF_ATTR(1, 2, true);
+        ZR_SVGF_ATTR(2, 1, false); ZR_SVGF_ATTR(2, 1, true); ZR_SVGF_ATTR(2, 2, false); ZR_SVGF_ATTR(2, 2, true);
+#undef ZR_SVGF_ATTR
+        if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(k_svgf_atrous)");
+        return ZR_OK;
+    }
+
+    // writes the maps of s's planes for radius R to s.d_maps; on failure s.d_maps is unchanged
+    static zr_status EncodeMaps(const Sized& s, uint32_t R)
+    {
+        using namespace zr;
+        CUtensorMap host[3][MAX_PASSES][2];     // [cv load, cv store, guide load][pass][plane]
         for (int k = 0; k < MAX_PASSES; k++)
         {
-            const uint64_t s = 1ull << k;
+            const uint64_t st = 1ull << k;
             for (int pl = 0; pl < 2; pl++)
             {
                 bool ok = true;
-                if (s == 1)
+                if (st == 1)
                 {
-                    const uint64_t dims[2] = { pitch, rows };
-                    const uint64_t strides[1] = { (uint64_t)pitch * 8 };
+                    const uint64_t dims[2] = { s.pitch, s.rows };
+                    const uint64_t strides[1] = { (uint64_t)s.pitch * 8 };
                     const uint32_t boxL[2] = { 64 + 2 * 2, 16 + 2 * R }, boxS[2] = { 64, 16 };       // AtrousTile<R, 1>::AX == 2
-                    ok = ok && tma::EncodeWords(&mapCvLoad[k][pl], d_cv[pl], 2, dims, strides, boxL);
-                    ok = ok && tma::EncodeWords(&mapGuideLoad[k][pl], d_guide[pl], 2, dims, strides, boxL);
-                    ok = ok && tma::EncodeWords(&mapCvStore[k][pl], d_cv[pl], 2, dims, strides, boxS);
+                    ok = ok && tma::EncodeWords(&host[0][k][pl], s.d_cv[pl], 2, dims, strides, boxL);
+                    ok = ok && tma::EncodeWords(&host[2][k][pl], s.d_guide[pl], 2, dims, strides, boxL);
+                    ok = ok && tma::EncodeWords(&host[1][k][pl], s.d_cv[pl], 2, dims, strides, boxS);
                 }
                 else
                 {
                     // {phase_x, u, phase_y, v}: pixel (u s + phase_x, v s + phase_y)
-                    const uint64_t dims[4] = { s, pitch / s, s, rows / s };
-                    const uint64_t strides[3] = { s * 8, (uint64_t)pitch * 8, s * (uint64_t)pitch * 8 };
+                    const uint64_t dims[4] = { st, s.pitch / st, st, s.rows / st };
+                    const uint64_t strides[3] = { st * 8, (uint64_t)s.pitch * 8, st * (uint64_t)s.pitch * 8 };
                     const uint32_t boxL[4] = { 2, 32 + 2 * R, 1, 16 + 2 * R }, boxS[4] = { 2, 32, 1, 16 };
-                    ok = ok && tma::EncodeWords(&mapCvLoad[k][pl], d_cv[pl], 4, dims, strides, boxL);
-                    ok = ok && tma::EncodeWords(&mapGuideLoad[k][pl], d_guide[pl], 4, dims, strides, boxL);
-                    ok = ok && tma::EncodeWords(&mapCvStore[k][pl], d_cv[pl], 4, dims, strides, boxS);
+                    ok = ok && tma::EncodeWords(&host[0][k][pl], s.d_cv[pl], 4, dims, strides, boxL);
+                    ok = ok && tma::EncodeWords(&host[2][k][pl], s.d_guide[pl], 4, dims, strides, boxL);
+                    ok = ok && tma::EncodeWords(&host[1][k][pl], s.d_cv[pl], 4, dims, strides, boxS);
                 }
                 if (!ok)
                 {
-                    set_error("zr_svgf_pass: cuTensorMapEncodeTiled failed (step %u)", (unsigned)s);
+                    set_error("zr_svgf_pass: cuTensorMapEncodeTiled failed (step %u)", (unsigned)st);
                     return ZR_ERR_CUDA;
                 }
             }
         }
         // no kernel may still be using the old maps, and the new ones are in place before the next launch
         ZR_CUDA(cudaDeviceSynchronize());
-        if (!d_maps) ZR_CUDA(cudaMalloc(&d_maps, sizeof(CUtensorMap) * 3 * MAX_PASSES * 2));
-        CUtensorMap host[3][MAX_PASSES][2];
-        memcpy(host[0], mapCvLoad, sizeof(mapCvLoad)); memcpy(host[1], mapCvStore, sizeof(mapCvStore)); memcpy(host[2], mapGuideLoad, sizeof(mapGuideLoad));
-        ZR_CUDA(cudaMemcpy(d_maps, host, sizeof(host), cudaMemcpyHostToDevice));
+        ZR_CUDA(cudaMemcpy(s.d_maps, host, sizeof(host), cudaMemcpyHostToDevice));
         ZR_CUDA(cudaDeviceSynchronize());
-        mapsReady = true;
         return ZR_OK;
     }
 
     zr_status OnWindowResized(uint32_t w, uint32_t h)
     {
-        Release();
-        width = w; height = h;
+        Sized next;
         // padded so that (a) every lattice view divides evenly (multiples of 32 >= 2 * 16) and (b) no TMA box is larger than the
         // tensor it is cut from, even for the coarsest lattice (step 16: 36 x 20 lattice points) of a small image
-        pitch = (w + 31) / 32 * 32; rows = (h + 31) / 32 * 32;
-        if (pitch < 16u * 36u) pitch = 16u * 36u;
-        if (rows < 16u * 20u) rows = 16u * 20u;
-        const size_t n = (size_t)pitch * rows;
+        next.pitch = (w + 31) / 32 * 32; next.rows = (h + 31) / 32 * 32;
+        if (next.pitch < 16u * 36u) next.pitch = 16u * 36u;
+        if (next.rows < 16u * 20u) next.rows = 16u * 20u;
+        const size_t n = (size_t)next.pitch * next.rows;
         for (int i = 0; i < 2; i++)
         {
-            ZR_CUDA(cudaMalloc(&d_cv[i], n * 8));
-            ZR_CUDA(cudaMalloc(&d_guide[i], n * 8));
-            ZR_CUDA(cudaMalloc(&d_hist[i], n * 16));
+            ZR_TRY(next.planes.Alloc(next.d_cv[i], n));
+            ZR_TRY(next.planes.Alloc(next.d_guide[i], n));
+            ZR_TRY(next.planes.Alloc(next.d_hist[i], n));
         }
-        ZR_CUDA(cudaMalloc(&d_out, (size_t)w * h * 16));
-        zr_status st = ResetTemporal();
-        if (st != ZR_OK) return st;
-        return EncodeMaps();
+        ZR_TRY(next.planes.Alloc(next.d_out, (size_t)w * h));
+        ZR_TRY(next.planes.Alloc(next.d_maps, 3 * MAX_PASSES * 2, false));
+        ZR_TRY(next.planes.Clear());
+        ZR_TRY(EncodeMaps(next, params.radius));
+        sz = std::move(next);
+        width = w; height = h;
+        historyValid = false; cur = 0;
+        return ZR_OK;
     }
 
     zr_status ResetTemporal()
     {
-        const size_t n = (size_t)pitch * rows;
-        ZR_CLEAR_BEGIN();
-        for (int i = 0; i < 2; i++)
-        {
-            ZR_CUDA(cudaMemset(d_cv[i], 0, n * 8));
-            ZR_CUDA(cudaMemset(d_guide[i], 0, n * 8));
-            ZR_CUDA(cudaMemset(d_hist[i], 0, n * 16));
-        }
-        ZR_CUDA(cudaMemset(d_out, 0, (size_t)width * height * 16));
-        ZR_CLEAR_END();
-        historyValid = false;
-        cur = 0;
+        ZR_TRY(sz.planes.Clear());
+        historyValid = false; cur = 0;
         return ZR_OK;
     }
 
@@ -406,8 +399,8 @@ struct zr_svgf_pass
         {
             using T = AtrousTile<R, 1>;
             const uint32_t tilesU = (width + T::TU - 1) / T::TU, tilesV = (height + T::TV - 1) / T::TV;
-            if (last) k_svgf_atrous<R, 1, true><<<dim3(tilesU * tilesV, 1), 512, T::BYTES, stream>>>(mIn, mG, mOut, d_out, width, height, s, tilesU, prm);
-            else k_svgf_atrous<R, 1, false><<<dim3(tilesU * tilesV, 1), 512, T::BYTES, stream>>>(mIn, mG, mOut, d_out, width, height, s, tilesU, prm);
+            if (last) k_svgf_atrous<R, 1, true><<<dim3(tilesU * tilesV, 1), 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, prm);
+            else k_svgf_atrous<R, 1, false><<<dim3(tilesU * tilesV, 1), 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, prm);
         }
         else
         {
@@ -415,8 +408,8 @@ struct zr_svgf_pass
             const uint32_t latW = (width + s - 1) / s, latH = (height + s - 1) / s;
             const uint32_t tilesU = (latW + T::TU - 1) / T::TU, tilesV = (latH + T::TV - 1) / T::TV;
             const dim3 grid(tilesU * tilesV, (s / 2) * s);
-            if (last) k_svgf_atrous<R, 2, true><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, d_out, width, height, s, tilesU, prm);
-            else k_svgf_atrous<R, 2, false><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, d_out, width, height, s, tilesU, prm);
+            if (last) k_svgf_atrous<R, 2, true><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, prm);
+            else k_svgf_atrous<R, 2, false><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, prm);
         }
         ZR_LAUNCH_CHECK();
         if (getenv("ZR_SVGF_DEBUG"))
@@ -435,18 +428,14 @@ struct zr_svgf_pass
             set_error("zr_svgf_pass_render: missing input");
             return ZR_ERR_INVALID_ARG;
         }
-        if (in->frame.RenderWidth != width || in->frame.RenderHeight != height)
-        {
-            set_error("zr_svgf_pass_render: frame/pass size mismatch");
-            return ZR_ERR_INVALID_ARG;
-        }
-        if (!mapsReady) { set_error("zr_svgf_pass_render: tensor maps are not initialised"); return ZR_ERR_NOT_INITIALIZED; }
+        const zr_status fs = check_frame_size("zr_svgf_pass", in->frame, width, height);
+        if (fs != ZR_OK) return fs;
         cur = 1 - cur;
         {
             ZR_PROF("k_svgf_temporal", stream);
             k_svgf_temporal<<<dim3((width + 31) / 32, (height + 7) / 8), 256, 0, stream>>>(in->frame, (const uint4*)in->curr.d_core,
-                (const uint2*)in->curr.d_motion_emissive, (const float4*)d_signal, d_guide[1 - cur], d_hist[1 - cur], historyValid ? 1 : 0,
-                d_hist[cur], d_cv[0], d_guide[cur], pitch);
+                (const uint2*)in->curr.d_motion_emissive, (const float4*)d_signal, sz.d_guide[1 - cur], sz.d_hist[1 - cur], historyValid ? 1 : 0,
+                sz.d_hist[cur], sz.d_cv[0], sz.d_guide[cur], sz.pitch);
             ZR_LAUNCH_CHECK();
         }
         int plane = 0;
@@ -464,36 +453,10 @@ struct zr_svgf_pass
 
 extern "C"
 {
-    zr_status zr_svgf_pass_create(uint32_t width, uint32_t height, zr_svgf_pass** out)
-    {
-        if (!out || !width || !height) { zr::set_error("zr_svgf_pass_create: bad args"); return ZR_ERR_INVALID_ARG; }
-        zr_svgf_pass* p = new zr_svgf_pass();
-        zr_svgf_pass::Defaults(&p->params);
-        using namespace zr;
-        cudaError_t e = cudaSuccess;
-#define ZR_SVGF_ATTR(R, P, LAST) \
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_svgf_atrous<R, P, LAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, AtrousTile<R, P>::BYTES)
-        ZR_SVGF_ATTR(1, 1, false); ZR_SVGF_ATTR(1, 1, true); ZR_SVGF_ATTR(1, 2, false); ZR_SVGF_ATTR(1, 2, true);
-        ZR_SVGF_ATTR(2, 1, false); ZR_SVGF_ATTR(2, 1, true); ZR_SVGF_ATTR(2, 2, false); ZR_SVGF_ATTR(2, 2, true);
-#undef ZR_SVGF_ATTR
-        if (e != cudaSuccess) { delete p; zr::cuda_fail(e, "cudaFuncSetAttribute(k_svgf_atrous)"); return ZR_ERR_CUDA; }
-        zr_status s = p->OnWindowResized(width, height);
-        if (s != ZR_OK) { p->Release(); delete p; return s; }
-        *out = p;
-        return ZR_OK;
-    }
-    zr_status zr_svgf_pass_resize(zr_svgf_pass* p, uint32_t width, uint32_t height)
-    {
-        if (!p || !width || !height) return ZR_ERR_INVALID_ARG;
-        return p->OnWindowResized(width, height);
-    }
-    zr_status zr_svgf_pass_reset_temporal(zr_svgf_pass* p) { return p ? p->ResetTemporal() : ZR_ERR_INVALID_ARG; }
-    zr_status zr_svgf_pass_default_params(zr_svgf_params* out)
-    {
-        if (!out) return ZR_ERR_INVALID_ARG;
-        zr_svgf_pass::Defaults(out);
-        return ZR_OK;
-    }
+    zr_status zr_svgf_pass_create(uint32_t width, uint32_t height, zr_svgf_pass** out) { return zr::CreatePass("zr_svgf_pass", width, height, out); }
+    zr_status zr_svgf_pass_resize(zr_svgf_pass* p, uint32_t width, uint32_t height) { return zr::ResizePass("zr_svgf_pass", p, width, height); }
+    zr_status zr_svgf_pass_reset_temporal(zr_svgf_pass* p) { return zr::ResetPass(p); }
+    zr_status zr_svgf_pass_default_params(zr_svgf_params* out) { return zr::DefaultParams<zr_svgf_pass>(out); }
     zr_status zr_svgf_pass_set_params(zr_svgf_pass* p, const zr_svgf_params* params)
     {
         if (!p || !params) return ZR_ERR_INVALID_ARG;
@@ -503,9 +466,9 @@ extern "C"
             zr::set_error("zr_svgf_pass_set_params: radius must be 1 or 2, 1..5 passes, positive sigmas");
             return ZR_ERR_INVALID_ARG;
         }
-        const bool remap = params->radius != p->params.radius;
+        if (params->radius != p->params.radius) ZR_TRY(zr_svgf_pass::EncodeMaps(p->sz, params->radius));
         p->params = *params;
-        return remap ? p->EncodeMaps() : ZR_OK;
+        return ZR_OK;
     }
     zr_status zr_svgf_pass_render(zr_svgf_pass* p, const zr_frame_inputs* in, const void* d_signal, void* stream)
     {
@@ -518,13 +481,13 @@ extern "C"
         const uint32_t w = p->width, h = p->height;
         switch (id)
         {
-        case ZR_SVGF_DENOISED: *out = zr_image2d{ p->d_out, w, h, w * 16u, 16u }; break;
-        case ZR_SVGF_ACCUMULATED: *out = zr_image2d{ p->d_cv[0], w, h, p->pitch * 8u, 8u }; break;       // only valid with num_passes == 1 .. see header
-        case ZR_SVGF_GUIDE: *out = zr_image2d{ p->d_guide[p->cur], w, h, p->pitch * 8u, 8u }; break;
-        case ZR_SVGF_HISTORY: *out = zr_image2d{ p->d_hist[p->cur], w, h, p->pitch * 16u, 16u }; break;
+        case ZR_SVGF_DENOISED: *out = zr_image2d{ p->sz.d_out, w, h, w * 16u, 16u }; break;
+        case ZR_SVGF_ACCUMULATED: *out = zr_image2d{ p->sz.d_cv[0], w, h, p->sz.pitch * 8u, 8u }; break;       // only valid with num_passes == 1 .. see header
+        case ZR_SVGF_GUIDE: *out = zr_image2d{ p->sz.d_guide[p->cur], w, h, p->sz.pitch * 8u, 8u }; break;
+        case ZR_SVGF_HISTORY: *out = zr_image2d{ p->sz.d_hist[p->cur], w, h, p->sz.pitch * 16u, 16u }; break;
         default: zr::set_error("zr_svgf_pass_get_output: unknown output id"); return ZR_ERR_INVALID_ARG;
         }
         return ZR_OK;
     }
-    void zr_svgf_pass_destroy(zr_svgf_pass* p) { if (p) { p->Release(); delete p; } }
+    void zr_svgf_pass_destroy(zr_svgf_pass* p) { delete p; }
 }

@@ -42,6 +42,8 @@ void set_error(const char* fmt, ...);
 // Reads the first `bytes` bytes of <directory of this library>/assets/<name> into dst; `who` prefixes the error message.
 zr_status read_asset(const char* who, const char* name, void* dst, size_t bytes);
 zr_status cuda_fail(cudaError_t e, const char* what);
+// ZR_ERR_INVALID_ARG with "<pass>_render: frame is WxH but the pass was sized wxh" unless the frame has the pass's size
+zr_status check_frame_size(const char* pass, const zr_frame_constants& frame, uint32_t width, uint32_t height);
 void count_launch(uint64_t n = 1);
 #define ZR_CUDA(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return zr::cuda_fail(e__, #expr); } while (0)
 // Host-side clears (reset / resize / alloc) run on the legacy default stream, which is NOT ordered against the

@@ -42,11 +42,8 @@ inline zr_status LightingFrame(const char* pass, const zr_frame_inputs* in, uint
         set_error("%s_render: missing scene or G-buffer", pass);
         return ZR_ERR_INVALID_ARG;
     }
-    if (in->frame.RenderWidth != width || in->frame.RenderHeight != height)
-    {
-        set_error("%s_render: frame is %ux%u but the pass was sized %ux%u", pass, in->frame.RenderWidth, in->frame.RenderHeight, width, height);
-        return ZR_ERR_INVALID_ARG;
-    }
+    const zr_status st = check_frame_size(pass, in->frame, width, height);
+    if (st != ZR_OK) return st;
     if (in->scene->dev.numEmissives == 0 || !in->scene->aliasBuilt)
     {
         // PathTracer.cpp:274-284: the emissive variants only run when the scene has emissive triangles

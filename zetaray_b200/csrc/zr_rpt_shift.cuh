@@ -132,14 +132,14 @@ namespace
     // queue is drained, which frees its slot for the next class's blocks. Measured on the strip-sharded frame, where every queue is a
     // fraction of the machine (DESIGN 7).
     template<bool TEMPORAL>
-    zr_status LaunchShifts(SpatialQueued& q, const SceneDev& sc, const FrameView& f, const RptParams& prm, const zr_rpt_reservoir* resIn,
-        const zr_rpt_reservoir* resPrev, const uint16_t* neighbor, cudaStream_t stream)
+    zr_status LaunchShifts(const SpatialQueued& q, const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm,
+        const zr_rpt_reservoir* resIn, const zr_rpt_reservoir* resPrev, const uint16_t* neighbor, cudaStream_t stream)
     {
-        const uint32_t grid = (uint32_t)q.numSMs * SHIFT_MINBLOCKS;
-        cudaStream_t s1 = q.aux[0], s2 = q.aux[1];
-        ZR_CUDA(cudaEventRecord(q.evFork, stream));
-        ZR_CUDA(cudaStreamWaitEvent(s1, q.evFork, 0));
-        ZR_CUDA(cudaStreamWaitEvent(s2, q.evFork, 0));
+        const uint32_t grid = (uint32_t)ss.numSMs * SHIFT_MINBLOCKS;
+        cudaStream_t s1 = ss.aux[0], s2 = ss.aux[1];
+        ZR_CUDA(cudaEventRecord(ss.evFork, stream));
+        ZR_CUDA(cudaStreamWaitEvent(s1, ss.evFork, 0));
+        ZR_CUDA(cudaStreamWaitEvent(s2, ss.evFork, 0));
 #define ZR_LAUNCH_SHIFT(CASE, REPLAY, CLS, STREAM) \
         k_shift<CASE, REPLAY, TEMPORAL><<<grid, SHIFT_THREADS, 0, STREAM>>>(sc, f, prm, resIn, resPrev, neighbor, q.d_queue + (size_t)(CLS) * q.capacity, \
             q.d_counters, CLS, q.d_shift); \
@@ -151,10 +151,10 @@ namespace
         ZR_LAUNCH_SHIFT(2, true, 3, s2);
         ZR_LAUNCH_SHIFT(3, true, 5, stream);
 #undef ZR_LAUNCH_SHIFT
-        ZR_CUDA(cudaEventRecord(q.evJoin[0], s1));
-        ZR_CUDA(cudaEventRecord(q.evJoin[1], s2));
-        ZR_CUDA(cudaStreamWaitEvent(stream, q.evJoin[0], 0));
-        ZR_CUDA(cudaStreamWaitEvent(stream, q.evJoin[1], 0));
+        ZR_CUDA(cudaEventRecord(ss.evJoin[0], s1));
+        ZR_CUDA(cudaEventRecord(ss.evJoin[1], s2));
+        ZR_CUDA(cudaStreamWaitEvent(stream, ss.evJoin[0], 0));
+        ZR_CUDA(cudaStreamWaitEvent(stream, ss.evJoin[1], 0));
         return ZR_OK;
     }
 

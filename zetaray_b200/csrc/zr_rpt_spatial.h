@@ -10,6 +10,7 @@
 // Results are bit-identical to the oracle.
 #pragma once
 #include <cuda.h>
+#include "zr_planes.h"
 #include "zr_rpt_io.cuh"
 
 namespace zr
@@ -25,39 +26,43 @@ struct ShiftResult
 };
 static_assert(sizeof(ShiftResult) == 32, "ShiftResult is two 128-bit words");
 
+// What the shift launches need whatever the frame size: created once with the pass (Init, which also sets k_spatial_merge's shared
+// memory limit), released with it. The six class launches of a shift stage are independent (own queue, own claim cursor, disjoint result
+// bytes): they are spread over the caller's stream and two forked ones, so that short queues -- small classes, strip-sharded frames --
+// run side by side.
+struct ShiftStreams
+{
+    int numSMs = 0;
+    cudaStream_t aux[2] = { nullptr, nullptr };
+    cudaEvent_t evFork = nullptr, evJoin[2] = { nullptr, nullptr };
+    ShiftStreams() = default;
+    ShiftStreams(const ShiftStreams&) = delete;
+    ShiftStreams& operator=(const ShiftStreams&) = delete;
+    ~ShiftStreams();
+    zr_status Init();
+};
+
+// The queues, shift results and tensor maps of one frame size. Temporal reuse runs through the same queues, counters and shift-result
+// plane (the two passes never overlap in a frame).
 struct SpatialQueued
 {
     static constexpr int NUM_CLASSES = 6;       // (case 1, 2, 3) x (k == 2, k > 2)
+    Planes planes{ "zr_indirect_pass" };        // Build clears the shift results and the temporal flags, nothing else
     uint32_t width = 0, height = 0;
     uint32_t* d_queue = nullptr;                // NUM_CLASSES x capacity items: x | y << 16 | direction << 31
     uint32_t* d_counters = nullptr;             // [c] = items queued, [8 + c] = claim cursor of the persistent blocks
     ShiftResult* d_shift = nullptr;
+    uint8_t* d_flags = nullptr;                 // temporal, per pixel: bit 0 = reuse valid, bit 1 = the replay's tighter plane test passed
     size_t capacity = 0;
-    CUtensorMap mapRes[2];                      // the two reservoir planes as [H][W] x 64 B, 32x32-pixel boxes
     const void* mapBase[2] = { nullptr, nullptr };
-    CUtensorMap* d_maps = nullptr;              // device copy of mapRes (the kernel reads the descriptor from global memory)
-    int numSMs = 0;
-    bool ready = false;
-    // the six class launches of a shift stage are independent (own queue, own claim cursor, disjoint result bytes): they are spread over
-    // the caller's stream and two forked ones, so that short queues -- small classes, strip-sharded frames -- run side by side
-    cudaStream_t aux[2] = { nullptr, nullptr };
-    cudaEvent_t evFork = nullptr, evJoin[2] = { nullptr, nullptr };
+    CUtensorMap* d_maps = nullptr;              // the two reservoir planes as [H][W] x 64 B, 32x32-pixel boxes (read from global memory)
     bool swizzled = false;                      // even widths: 3-D map {128-byte record pair, W / 2, H} with the 128-byte swizzle
 
-    zr_status Resize(uint32_t w, uint32_t h, const zr_rpt_reservoir* res0, const zr_rpt_reservoir* res1);
-    void Release();
-    // resIn must be one of the two planes given to Resize
-    zr_status Run(const SceneDev& sc, const FrameView& f, const RptParams& prm, const zr_rpt_reservoir* resIn, zr_rpt_reservoir* resOut,
-        const float4* target, float4* finalImg, const uint16_t* neighbor, const uint16_t* threadMap, cudaStream_t stream);
-};
-
-// Temporal reuse through the same queues, counters and shift-result plane (the two passes never overlap in a frame).
-struct TemporalQueued
-{
-    uint8_t* d_flags = nullptr;     // per pixel: bit 0 = temporal reuse valid, bit 1 = the replay's tighter plane test passed
-    zr_status Resize(uint32_t w, uint32_t h);
-    void Release();
-    zr_status Run(SpatialQueued& q, const SceneDev& sc, const FrameView& f, const RptParams& prm, zr_rpt_reservoir* resCurr,
+    zr_status Build(uint32_t w, uint32_t h, const zr_rpt_reservoir* res0, const zr_rpt_reservoir* res1);
+    // resIn must be one of the two planes given to Build
+    zr_status Run(const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm, const zr_rpt_reservoir* resIn,
+        zr_rpt_reservoir* resOut, const float4* target, float4* finalImg, const uint16_t* neighbor, const uint16_t* threadMap, cudaStream_t stream);
+    zr_status RunTemporal(const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm, zr_rpt_reservoir* resCurr,
         const zr_rpt_reservoir* resPrev, float4* target, float4* finalImg, cudaStream_t stream);
 };
 } // namespace zr

@@ -22,6 +22,10 @@ struct BlockSchedule
     // key of the inputs the table was built from
     uint32_t rowBegin = 0xffffffffu, rowEnd = 0, costVersion = 0xffffffffu;
 
+    BlockSchedule() = default;
+    BlockSchedule(const BlockSchedule&) = delete;
+    BlockSchedule& operator=(const BlockSchedule&) = delete;
+    ~BlockSchedule() { Release(); }
     void Release() { if (d_order) cudaFree(d_order); d_order = nullptr; count = 0; rowBegin = 0xffffffffu; }
     bool UpToDate(uint32_t y0, uint32_t y1, uint32_t version) const { return d_order && rowBegin == y0 && rowEnd == y1 && costVersion == version; }
     cudaError_t Upload(const std::vector<uint32_t>& order, uint32_t y0, uint32_t y1, uint32_t version)
@@ -121,7 +125,14 @@ struct LightingStrip
     BlockSchedule sched;
 
     explicit LightingStrip(const char* passName) : pass(passName) {}
-    void Release() { sched.Release(); }
+    // after a resize: the rows, cost map, tile costs and block table described the old frame; the halo hook stays
+    void ForgetSize()
+    {
+        rowBegin = 0; rowEnd = 0xffffffffu;
+        d_costMap = nullptr;
+        tileCosts = TileCosts{};
+        sched.Release();
+    }
     uint32_t ClampedRowEnd(uint32_t height) const { return rowEnd < height ? rowEnd : height; }
 
     zr_status SetRows(uint32_t y0, uint32_t y1, uint32_t height)
