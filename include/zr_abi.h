@@ -307,6 +307,12 @@ ZR_API zr_status zr_scene_create(const zr_scene_desc* desc, zr_scene** out);
 ZR_API void zr_scene_destroy(zr_scene* scene);
 /* BVH statistics for tests: {num_nodes, num_tris, max_depth, bytes}. */
 ZR_API zr_status zr_scene_bvh_stats(const zr_scene* scene, uint32_t out[4]);
+/* The optional BSDF features the scene's materials use: the OR over its material table, fixed at zr_scene_create. The
+ * lighting passes run kernels built without clear coat, specular transmission and thin-walled transmission when none is set. */
+#define ZR_MATERIAL_COAT         0x1u   /* coat weight > 0 */
+#define ZR_MATERIAL_TRANSMISSION 0x2u   /* transmissive flag (bit 26 of CoatColor_Flags) */
+#define ZR_MATERIAL_THIN_WALLED  0x4u   /* thin-walled flag (bit 29 of CoatColor_Flags) with subsurface weight > 0 */
+ZR_API zr_status zr_scene_material_features(const zr_scene* scene, uint32_t* out);
 
 /* The BVH builder alone, on host memory (no GPU needed): world-space triangles as 9 floats {v0, e1, e2} in, 80-byte
  * nodes and the leaf-order permutation out (either may be NULL to query sizes). out_info = {num_nodes, num_tris,

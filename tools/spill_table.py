@@ -3,7 +3,8 @@
     ZR_PTXAS_V=1 python zetaray_b200/build.py --force 2> ptxas.log
     python tools/spill_table.py ptxas.log [zetaray_b200/libzetaray_b200.so]
 
-For every k_pathtrace, k_di_temporal, k_di_spatial and k_shift<CASE, REPLAY, TEMPORAL> entry point it prints what ptxas
+For every k_pathtrace, k_di_temporal, k_di_spatial and k_shift<CASE, REPLAY, TEMPORAL> entry point, in its plain (no clear coat,
+no transmission) and its full material-feature build, it prints what ptxas
 reported (registers, stack frame, static spill store / load bytes, static shared memory; k_pathtrace's dynamic shared
 memory is not in the log) and, from `cuobjdump -sass` of the library,
 the number of SASS instructions and of local-memory loads (LDL) and stores (STL) in the kernel's code. The library
@@ -18,17 +19,22 @@ CUDA_BIN = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin")
 KERNELS = ("k_pathtrace", "k_di_temporal", "k_di_spatial", "k_shift")
 
 
+def variant(mf):
+    """The material-feature template argument (BSDF::ShadingDataT): 0 = the plain build, otherwise the full one."""
+    return "plain" if int(mf) == 0 else "full"
+
+
 def short_name(mangled):
-    """_ZN2zr..._GLOBAL__N__..._6_rdi_cu_...13k_di_temporalENS_... -> k_di_temporal; k_shift keeps its template arguments and
-    the pass it belongs to (spatial / temporal)."""
+    """_ZN2zr..._GLOBAL__N__..._6_rdi_cu_...13k_di_temporalILj0EEvNS_... -> k_di_temporal [plain]; k_shift keeps its template
+    arguments and the pass it belongs to (spatial / temporal). Every kernel is listed once per material-feature build."""
     for k in KERNELS:
-        m = re.search(r"\d+%s(I[^E]*E[^E]*E[^E]*E)?" % k, mangled)
-        if not m:
+        if not re.search(r"\d+%sI" % k, mangled):
             continue
         if k != "k_shift":
-            return k
-        case, replay, temporal = re.search(r"ILi(\d)ELb(\d)ELb(\d)E", mangled).groups()
-        return "k_shift<%s,%s,%s>" % (case, "replay" if replay == "1" else "-", "temporal" if temporal == "1" else "spatial")
+            return "%s [%s]" % (k, variant(re.search(r"\d+%sILj(\d+)E" % k, mangled).group(1)))
+        case, replay, temporal, mf = re.search(r"ILi(\d)ELb(\d)ELb(\d)ELj(\d+)E", mangled).groups()
+        return "k_shift<%s,%s,%s> [%s]" % (case, "replay" if replay == "1" else "-", "temporal" if temporal == "1" else "spatial",
+                                           variant(mf))
     return None
 
 

@@ -19,16 +19,19 @@ namespace zr
 namespace
 {
 // 512 threads at 128 registers: on an H100 SXM (700 W) k_di_temporal + k_di_spatial take 1.30 + 0.73 ms per bench frame, against
-// 1.55 + 1.01 at 1024 x 64 registers, 1.32 + 0.92 at 768 x 80 and 1.44 + 0.93 at 512 x 2 blocks x 64 (DESIGN 4.1).
+// 1.55 + 1.01 at 1024 x 64 registers, 1.32 + 0.92 at 768 x 80 and 1.44 + 0.93 at 512 x 2 blocks x 64 (DESIGN 4.1). Swept before the plain material build existed; both builds use this shape.
 #ifndef ZR_RDI_THREADS
 #define ZR_RDI_THREADS 512
 #endif
     // ReSTIR_DI_Temporal.hlsl main + EstimateDirectLighting. A block is ZR_RDI_THREADS/64 consecutive 8x8 groups of the
     // reference's swizzled dispatch, walking the resampling phases together (no thread leaves before the last barrier).
+    // MF: the material features the kernel is compiled for (BSDF::ShadingDataT); the scene's materials must use no others.
+    template<uint32_t MF>
     __global__ void ZR_LB(ZR_RDI_THREADS) k_di_temporal(SceneDev sc, FrameView f, DIParams prm, zr_rdi_reservoir* __restrict__ resCurr,
         const zr_rdi_reservoir* __restrict__ resPrev, uint2* __restrict__ target, float4* __restrict__ finalImg, uint32_t dispX, uint32_t dispY,
         const uint32_t* __restrict__ order)
     {
+        using SD = BSDF::ShadingDataT<MF>;
         const zr_frame_constants& fc = f.fc;
         uint2 sg = make_uint2(0, 0);
         const uint32_t groupFlat = order[blockIdx.x] * (ZR_RDI_THREADS / 64) + (threadIdx.x >> 6);
@@ -55,14 +58,14 @@ namespace
                 act = false;
             }
         }
-        Pixel p;
-        p.surface = BSDF::ShadingData::InitEmpty();
+        PixelT<SD> p;
+        p.surface = SD::InitEmpty();
         p.pos = f3(0); p.normal = f3(0); p.roughness = 0;
         RNG rng_thread; rng_thread.State = 0;
         int numBsdfSamples = 0;
         if (act)
         {
-            p = LoadPixel(f, sc, f.core, f.coat, x, y, false, x, y);
+            p = LoadPixel<SD>(f, sc, f.core, f.coat, x, y, false, x, y);
             rng_thread = RNG::Init(x, y, fc.FrameNum);
             numBsdfSamples = (!p.surface.GlossSpecular() && p.roughness < 0.3f) ? 2 : 1;
         }
@@ -73,8 +76,8 @@ namespace
         if (prm.temporal)
         {
             float2 motionVec = f2(0, 0);
-            TemporalCandidate tc; tc.valid = false; tc.px = tc.py = 0; tc.pos = tc.normal = f3(0);
-            tc.surface = BSDF::ShadingData::InitEmpty();
+            TemporalCandidateT<SD> tc; tc.valid = false; tc.px = tc.py = 0; tc.pos = tc.normal = f3(0);
+            tc.surface = SD::InitEmpty();
             ZR_PHASE();
             if (act)
             {
@@ -106,10 +109,12 @@ namespace
     }
 
     // ReSTIR_DI_Spatial.hlsl main + SpatialResample
+    template<uint32_t MF>
     __global__ void ZR_LB(ZR_RDI_THREADS) k_di_spatial(SceneDev sc, FrameView f, DIParams prm, const zr_rdi_reservoir* __restrict__ resCurr,
         const uint2* __restrict__ target, float4* __restrict__ finalImg, uint32_t dispX, uint32_t dispY,
         const uint32_t* __restrict__ order)
     {
+        using SD = BSDF::ShadingDataT<MF>;
         const zr_frame_constants& fc = f.fc;
         uint2 sg = make_uint2(0, 0);
         const uint32_t groupFlat = order[blockIdx.x] * (ZR_RDI_THREADS / 64) + (threadIdx.x >> 6);
@@ -131,14 +136,14 @@ namespace
                 active = false;
             }
         }
-        Pixel p;
-        p.surface = BSDF::ShadingData::InitEmpty();
+        PixelT<SD> p;
+        p.surface = SD::InitEmpty();
         p.pos = f3(0); p.normal = f3(0); p.roughness = 0; p.z = 0;
         Reservoir r = Reservoir::Init();
         bool disoccluded = false;
         if (active)
         {
-            p = LoadPixel(f, sc, f.core, f.coat, x, y, false, x, y);
+            p = LoadPixel<SD>(f, sc, f.core, f.coat, x, y, false, x, y);
             zr_rdi_reservoir rec;
             LoadRdi(&resCurr[idx], rec);
             r = Reservoir::Load(rec);
@@ -189,7 +194,7 @@ namespace
             float rough_i;
             const GFlags flags_i = FlagsAt(f.core, f.W, qx, qy, &rough_i);
             if (flags_i.invalid || flags_i.emissive) continue;
-            const Pixel pi = LoadPixel(f, sc, f.core, f.coat, qx, qy, false, qx, qy);
+            const PixelT<SD> pi = LoadPixel<SD>(f, sc, f.core, f.coat, qx, qy, false, qx, qy);
             bool valid = PlaneHeuristicDI(pi.pos, p.normal, p.pos, p.z);
             valid = valid && (fabsf(rough_i - p.roughness) < 0.15f);
             if (!valid) continue;
@@ -202,21 +207,21 @@ namespace
             const bool go = active && (i < k);
             if (!__syncthreads_or(go))
                 break;
-            Pixel pi;
+            PixelT<SD> pi;
             pi.normal = f3(0);
-            BSDF::ShadingData surface_i = BSDF::ShadingData::InitEmpty();
+            SD surface_i = SD::InitEmpty();
             Reservoir r_spatial = Reservoir::Init();
             float3 pos_i = f3(0);
             if (go)
             {
-                pi = LoadPixel(f, sc, f.core, f.coat, spx[i], spy[i], false, spx[i], spy[i]);
+                pi = LoadPixel<SD>(f, sc, f.core, f.coat, spx[i], spy[i], false, spx[i], spy[i]);
                 // the neighbour surface is rebuilt with transmission depth = 0 (Resampling.hlsli:507-510)
                 const uint4 c = ld128(&f.core[(size_t)spy[i] * f.W + spx[i]]);
                 const float3 bc = f3((float)(c.z & 0xff) / 255.0f, (float)((c.z >> 8) & 0xff) / 255.0f, (float)((c.z >> 16) & 0xff) / 255.0f);
                 const float bw = pi.flags.subsurface ? (float)(c.z >> 24) / 255.0f : 0.0f;
                 pos_i = samplePos[i];
                 const float3 wo_i = normalize(pi.origin - pos_i);
-                surface_i = BSDF::ShadingData::Init(pi.normal, wo_i, pi.flags.metallic, pi.roughness, bc, BSDF::ETA_AIR,
+                surface_i = SD::Init(pi.normal, wo_i, pi.flags.metallic, pi.roughness, bc, BSDF::ETA_AIR,
                     pi.eta_next, pi.flags.transmissive, 0.0f, to_half(bw), pi.surface.coat_weight, pi.surface.coat_color,
                     pi.coatRoughness, pi.coatIor, sc.rho);
                 zr_rdi_reservoir recN;
@@ -317,15 +322,16 @@ struct zr_direct_pass
         st = strip.Schedule(width, height, 8, 8, ZR_RDI_THREADS / 64);
         if (st != ZR_OK) return st;
         const BlockSchedule& sched = strip.sched;
+        const bool plain = (in->scene->materialFeatures & BSDF::MF_ALL) == 0;
         ZR_PROF("k_di_temporal", stream);
-        k_di_temporal<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, dispX, dispY, sched.d_order);
+        (plain ? k_di_temporal<BSDF::MF_NONE> : k_di_temporal<BSDF::MF_ALL>)<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, dispX, dispY, sched.d_order);
         ZR_LAUNCH_CHECK();
         // the temporal output is what neighbours read in the spatial pass and what the next frame reprojects into
         strip.Exchange(sz.d_res[cur], width, height, 32u, stream);
         if (doSpatial)
         {
             ZR_PROF("k_di_spatial", stream);
-            k_di_spatial<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY, sched.d_order);
+            (plain ? k_di_spatial<BSDF::MF_NONE> : k_di_spatial<BSDF::MF_ALL>)<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY, sched.d_order);
             ZR_LAUNCH_CHECK();
         }
         isTemporalReservoirValid = true;

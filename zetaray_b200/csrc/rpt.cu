@@ -34,7 +34,7 @@ namespace
 // 768 threads at 80 registers with the parked state below (157 KB of shared memory per block). Measured on an H100 SXM (700 W):
 // 2.61 ms per bench frame, against 2.60 ms at 640 x 96 registers and 2.68 ms at 512 x 128; 640 threads spill far less but are no
 // faster. An earlier sweep, before the traversal rewrite: 3.33 ms, against 3.65 ms at 1024 x 64, 3.52 ms at 512 x 128 and 4.40 ms
-// at 512 x 2 blocks x 64 (DESIGN 4.1).
+// at 512 x 2 blocks x 64 (DESIGN 4.1). Swept before the plain material build existed; both builds use this shape.
 #ifndef ZR_PT_THREADS
 #define ZR_PT_THREADS 768
 #endif
@@ -53,10 +53,13 @@ namespace
 
     // A block is ZR_PT_THREADS/128 consecutive 16x8 groups of the reference's swizzled dispatch; each warp is one
     // reference wave. The warps of a block walk the bounce phases together (zr_rpt.cuh "block-synchronous phases").
-    // Dynamic shared memory: PT_SMEM_BYTES (PtParked per thread).
+    // Dynamic shared memory: PT_SMEM_BYTES (PtParked per thread). MF: the material features the kernel is compiled for
+    // (BSDF::ShadingDataT); the scene's materials must use no others.
+    template<uint32_t MF>
     __global__ void ZR_LB(ZR_PT_THREADS) k_pathtrace(SceneDev sc, FrameView f, RptParams prm, zr_rpt_reservoir* __restrict__ res,
         float4* __restrict__ target, float4* __restrict__ finalImg, uint32_t dispX, uint32_t dispY, const uint32_t* __restrict__ order)
     {
+        using SD = BSDF::ShadingDataT<MF>;
         extern __shared__ PtParked s_ptParked[];
         const zr_frame_constants& fc = f.fc;
         const long long t0 = clock64();
@@ -81,7 +84,7 @@ namespace
         }
         // loop-carried state
         float3 pos = f3(0), normal = f3(0), li = f3(0), throughput = f3(0), throughput_k = f3(1), tr = f3(1);
-        BSDF::ShadingData surface;
+        SD surface;
         BSDF::BSDFSample bsdfSample = BSDF::BSDFSample::Init();
         HitEmissive nextHit;
         nextHit.hit = false;
@@ -101,7 +104,7 @@ namespace
 
         if (inBounds)
         {
-            const Pixel p = LoadPixel(f, sc, f.core, f.coat, px.x, px.y, false, px.x, px.y);
+            const PixelT<SD> p = LoadPixel<SD>(f, sc, f.core, f.coat, px.x, px.y, false, px.x, px.y);
             rngGroup = RNG::Init4(sg.x, sg.y, fc.FrameNum, 1);
             const uint3 state = RNG::PCG3d(make_uint3(px.x, px.y, fc.FrameNum));
             rngReplay = RNG::InitSeed(state.x);
@@ -148,7 +151,7 @@ namespace
                     prevBsdfSamplePdf = bsdfSample.pdf;
                     prevBsdfSampleLobe = bsdfSample.lobe;
                     tr = f3(1);
-                    if (inTranslucentMedium && (surface.trDepth > 0))
+                    if (inTranslucentMedium && surface.TrDepthGt0())
                     {
                         const float3 c = surface.baseColor_Fr0_TrCol;
                         const float3 extCoeff = f3(-zr_logf(c.x), -zr_logf(c.y), -zr_logf(c.z)) / surface.trDepth;
@@ -196,7 +199,7 @@ namespace
                 if (lightSample)
                 {
                     seed_nee = rngThread.State;
-                    BSDF::ShadingData surfNee = surface;
+                    SD surfNee = surface;
                     nee = NEE_Emissive_Begin(sc, pos, hitInfo.normal, surfNee, sampleSetIdx, rngThread);
                 }
             }
@@ -218,7 +221,7 @@ namespace
                 {
                     // the shading copy NEE_Emissive_Begin evaluated the light sample with, rebuilt by the same SetWi instead of
                     // carried through the shadow-segment traversal
-                    BSDF::ShadingData surfNee = surface;
+                    SD surfNee = surface;
                     surfNee.SetWi(nee.ret.wi, hitInfo.normal);
                     bsdfPdf = BSDF::BSDFSamplerPdf(hitInfo.normal, surfNee, nee.ret.wi, rngThread);
                     bsdfPdf *= nee.dwdA;
@@ -558,17 +561,22 @@ struct zr_indirect_pass
         // k_pathtrace's parked state needs more than the 48 KB of static shared memory. The carveout asks for just the shared
         // memory its resident blocks use (plus the 1 KB the system reserves per block); the rest of the 256 KB stays L1 for
         // what still spills.
-        ZR_CUDA(cudaFuncSetAttribute(zr::k_pathtrace, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zr::PT_SMEM_BYTES));
-        int ptBlocks = 0;
-        ZR_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ptBlocks, zr::k_pathtrace, ZR_PT_THREADS, zr::PT_SMEM_BYTES));
-        if (ptBlocks < 1)
+        // Both material-feature builds are set up, whichever scenes the pass will render.
+        decltype(&zr::k_pathtrace<zr::BSDF::MF_ALL>) const kernels[2] = { zr::k_pathtrace<zr::BSDF::MF_NONE>, zr::k_pathtrace<zr::BSDF::MF_ALL> };
+        for (const auto kernel : kernels)
         {
-            zr::set_error("zr_indirect_pass: k_pathtrace (%d threads, %zu B shared) cannot be resident", ZR_PT_THREADS, zr::PT_SMEM_BYTES);
-            return ZR_ERR_UNSUPPORTED;
+            ZR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zr::PT_SMEM_BYTES));
+            int ptBlocks = 0;
+            ZR_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ptBlocks, kernel, ZR_PT_THREADS, zr::PT_SMEM_BYTES));
+            if (ptBlocks < 1)
+            {
+                zr::set_error("zr_indirect_pass: k_pathtrace (%d threads, %zu B shared) cannot be resident", ZR_PT_THREADS, zr::PT_SMEM_BYTES);
+                return ZR_ERR_UNSUPPORTED;
+            }
+            const size_t ptSmem = (size_t)ptBlocks * (zr::PT_SMEM_BYTES + 1024);
+            ZR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                (int)((ptSmem * 100 + 228 * 1024 - 1) / (228 * 1024))));
         }
-        const size_t ptSmem = (size_t)ptBlocks * (zr::PT_SMEM_BYTES + 1024);
-        ZR_CUDA(cudaFuncSetAttribute(zr::k_pathtrace, cudaFuncAttributePreferredSharedMemoryCarveout,
-            (int)((ptSmem * 100 + 228 * 1024 - 1) / (228 * 1024))));
         return shiftStreams.Init();
     }
 
@@ -638,13 +646,14 @@ struct zr_indirect_pass
 
         int cur = currTemporalIdx;
         const uint32_t dispX = (width + 15) / 16, dispY = (height + 7) / 8;
+        const bool plain = (in->scene->materialFeatures & BSDF::MF_ALL) == 0;
         ZR_PROF("k_pathtrace", stream);
-        k_pathtrace<<<strip.sched.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY,
+        (plain ? k_pathtrace<BSDF::MF_NONE> : k_pathtrace<BSDF::MF_ALL>)<<<strip.sched.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY,
             strip.sched.d_order);
         ZR_LAUNCH_CHECK();
         if (doTemporal)
         {
-            st = sz.queued.RunTemporal(shiftStreams, in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, stream);
+            st = sz.queued.RunTemporal(shiftStreams, in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, plain, stream);
             if (st != ZR_OK) return st;
         }
         // reservoirs written so far are read by neighbours (spatial pass) and by the next frame's temporal pass
@@ -667,7 +676,7 @@ struct zr_indirect_pass
                     k_sort<<<dim3(sx, ty1 - ty0), 256, 0, stream>>>(f, 3, 1u, rin, nullptr, sz.d_neighbor, sz.d_threadMap, sx, sy, ty0);
                     ZR_LAUNCH_CHECK();
                 }
-                st = sz.queued.Run(shiftStreams, in->scene->dev, f, prm, rin, rout, sz.d_target, sz.d_final, sz.d_neighbor, sz.d_threadMap, stream);
+                st = sz.queued.Run(shiftStreams, in->scene->dev, f, prm, rin, rout, sz.d_target, sz.d_final, sz.d_neighbor, sz.d_threadMap, plain, stream);
                 if (st != ZR_OK) return st;
                 strip.Exchange(rout, width, height, 64u, stream);
             }

@@ -383,7 +383,7 @@ zr_status SpatialQueued::Build(uint32_t w, uint32_t h, const zr_rpt_reservoir* r
 }
 
 zr_status SpatialQueued::Run(const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm, const zr_rpt_reservoir* resIn,
-    zr_rpt_reservoir* resOut, const float4* target, float4* finalImg, const uint16_t* neighbor, const uint16_t* threadMap, cudaStream_t stream)
+    zr_rpt_reservoir* resOut, const float4* target, float4* finalImg, const uint16_t* neighbor, const uint16_t* threadMap, bool plain, cudaStream_t stream)
 {
     const int plane = resIn == mapBase[0] ? 0 : (resIn == mapBase[1] ? 1 : -1);
     if (plane < 0) { set_error("zr_indirect_pass: spatial input is not one of the pass's reservoir planes"); return ZR_ERR_INVALID_ARG; }
@@ -396,7 +396,7 @@ zr_status SpatialQueued::Run(const ShiftStreams& ss, const SceneDev& sc, const F
     }
     {
         ZR_PROF("k_shift", stream);
-        const zr_status ls = LaunchShifts<false>(*this, ss, sc, f, prm, resIn, nullptr, neighbor, stream);
+        const zr_status ls = LaunchShifts<false>(*this, ss, sc, f, prm, resIn, nullptr, neighbor, plain, stream);
         zr::prof_after();
         if (ls != ZR_OK) return ls;
         cudaError_t e = cudaGetLastError();

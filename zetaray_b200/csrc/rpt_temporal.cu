@@ -186,7 +186,7 @@ namespace
 }
 
 zr_status SpatialQueued::RunTemporal(const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm, zr_rpt_reservoir* resCurr,
-    const zr_rpt_reservoir* resPrev, float4* target, float4* finalImg, cudaStream_t stream)
+    const zr_rpt_reservoir* resPrev, float4* target, float4* finalImg, bool plain, cudaStream_t stream)
 {
     const uint32_t rows = prm.rowEnd - prm.rowBegin;
     const dim3 grid((width + 31) / 32, (rows + 7) / 8);
@@ -198,7 +198,7 @@ zr_status SpatialQueued::RunTemporal(const ShiftStreams& ss, const SceneDev& sc,
     }
     {
         ZR_PROF("k_shift_temporal", stream);
-        const zr_status ls = LaunchShifts<true>(*this, ss, sc, f, prm, resCurr, resPrev, nullptr, stream);
+        const zr_status ls = LaunchShifts<true>(*this, ss, sc, f, prm, resCurr, resPrev, nullptr, plain, stream);
         zr::prof_after();
         if (ls != ZR_OK) return ls;
         cudaError_t e = cudaGetLastError();

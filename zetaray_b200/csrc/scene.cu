@@ -125,6 +125,17 @@ zr_status scene_create(const zr_scene_desc* desc, zr_scene** out)
     UP(emissives, desc->h_emissives, desc->num_emissives);
     sc->dev.numInstances = desc->num_instances;
     sc->dev.numEmissives = desc->num_emissives;
+    // The per-pixel coat / transmissive / subsurface bits of the G-buffer and the surfaces built at path vertices come from these
+    // material fields alone (no textures or instance overrides in this build), read as Mat::GetCoatWeight, Mat::Transmissive and
+    // Mat::ThinWalled ? Mat::GetSubsurface : 0 do.
+    for (uint32_t i = 0; i < desc->num_materials; i++)
+    {
+        const zr_material& m = desc->h_materials[i];
+        if ((m.BaseColorTex_Subsurf_CoatWeight >> 24) & 0xff) sc->materialFeatures |= ZR_MATERIAL_COAT;
+        if (m.CoatColor_Flags & (1u << 26)) sc->materialFeatures |= ZR_MATERIAL_TRANSMISSION;
+        if ((m.CoatColor_Flags & (1u << 29)) && ((m.BaseColorTex_Subsurf_CoatWeight >> 16) & 0xff))
+            sc->materialFeatures |= ZR_MATERIAL_THIN_WALLED;
+    }
 
     // triangle -> mesh maps
     std::vector<uint32_t> triMesh, meshFirst(desc->num_instances);
@@ -244,6 +255,12 @@ extern "C"
     {
         if (!sc || !out) return ZR_ERR_INVALID_ARG;
         out[0] = sc->info.numNodes; out[1] = sc->info.numTris; out[2] = sc->info.maxDepth; out[3] = sc->info.bytes;
+        return ZR_OK;
+    }
+    zr_status zr_scene_material_features(const zr_scene* sc, uint32_t* out)
+    {
+        if (!sc || !out) return ZR_ERR_INVALID_ARG;
+        *out = sc->materialFeatures;
         return ZR_OK;
     }
     zr_status zr_scene_trace_closest(const zr_scene* sc, const float* d_rays, uint32_t n, float* d_hits, void* stream)

@@ -212,14 +212,32 @@ namespace BSDF
         return (NDF * G1) / ndotwo;
     }
 
-    struct ShadingData
+    // Material features (ZR_MATERIAL_* bits): the optional lobes a ShadingDataT<MF> compiles in. For a feature outside MF the
+    // predicates that guard its code -- Coated(), ThinWalled(), Transmissive(), specTr -- are compile-time false, so a kernel
+    // instantiated for MF_NONE carries no clear-coat, specular-transmission, thin-walled or medium code. Such a surface type may
+    // only shade materials without those features (zr_scene::materialFeatures); for them every value it computes is the one
+    // MF_ALL computes, because the predicates it drops are false at run time too.
+    constexpr uint32_t MF_NONE = 0;
+    constexpr uint32_t MF_ALL = ZR_MATERIAL_COAT | ZR_MATERIAL_TRANSMISSION | ZR_MATERIAL_THIN_WALLED;
+
+    template<bool Stored> struct SpecTrField { bool specTr; };
+    template<> struct SpecTrField<false> { static constexpr bool specTr = false; };
+
+    template<uint32_t MF>
+    struct ShadingDataT : SpecTrField<(MF & ZR_MATERIAL_TRANSMISSION) != 0>
     {
+        static constexpr bool HasCoat = (MF & ZR_MATERIAL_COAT) != 0;
+        static constexpr bool HasTransmission = (MF & ZR_MATERIAL_TRANSMISSION) != 0;
+        static constexpr bool HasThinWalled = (MF & ZR_MATERIAL_THIN_WALLED) != 0;
+        using ShadingData = ShadingDataT;
+        using SpecTrField<HasTransmission>::specTr;
+
         float alpha;
         float3 wo;
         float ndotwi, ndotwo, ndotwh, whdotwi, whdotwo, wodotwi, g_wo;
         float3 baseColor_Fr0_TrCol;
         float eta;
-        bool specTr, metallic, backfacing_wo, invalid, reflection;
+        bool metallic, backfacing_wo, invalid, reflection;
         float trDepth;      // half
         float subsurface;   // half
         float coat_weight;
@@ -242,7 +260,7 @@ namespace BSDF
             float coat_roughness = 0, float eta_coat = DEFAULT_ETA_COAT, const uint16_t* rhoTable = nullptr)
         {
             float2 roughness4 = f2(roughness, coat_roughness);
-            if (coat_weight > 0 && coat_roughness > 0)
+            if (HasCoat && coat_weight > 0 && coat_roughness > 0)
             {
                 roughness4 = roughness4 * roughness4;
                 roughness4 = roughness4 * roughness4;
@@ -259,7 +277,8 @@ namespace BSDF
             si.metallic = metallic;
             si.alpha = roughness * roughness;
             si.baseColor_Fr0_TrCol = baseColor;
-            si.specTr = specTr;
+            if constexpr (HasTransmission)
+                si.specTr = specTr;
             si.trDepth = to_half(transmissionDepth);
             si.subsurface = to_half(subsurface);
             float eta_base = eta_curr == ETA_AIR ? eta_next : eta_curr;
@@ -275,9 +294,11 @@ namespace BSDF
             return si;
         }
 
-        ZR_D bool ThinWalled() const { return subsurface > 0; }
+        ZR_D bool ThinWalled() const { return HasThinWalled && subsurface > 0; }
         ZR_D bool Transmissive() const { return specTr || ThinWalled(); }
-        ZR_D bool Coated() const { return coat_weight != 0; }
+        ZR_D bool Coated() const { return HasCoat && coat_weight != 0; }
+        // the transmission depth of a medium the path travels through (only transmissive materials have one)
+        ZR_D bool TrDepthGt0() const { return HasTransmission && trDepth > 0; }
         ZR_D bool GlossSpecular() const { return alpha <= MAX_ALPHA_SPECULAR; }
         ZR_D bool CoatSpecular() const { return coat_alpha <= MAX_ALPHA_SPECULAR; }
         ZR_D float3 TransmissionTint() const { return trDepth > 0 ? f3(1) : baseColor_Fr0_TrCol; }
@@ -371,8 +392,10 @@ namespace BSDF
             return FresnelSchlick_Dielectric(Fr0, cosTheta);
         }
     };
+    using ShadingData = ShadingDataT<MF_ALL>;
 
-    ZR_D bool IsLobeValid(const ShadingData& surface, LOBE lt)
+    template<class SD>
+    ZR_D bool IsLobeValid(const SD& surface, LOBE lt)
     {
         if (lt == ALL) return true;
         if (surface.metallic && (lt != GLOSSY_R) && (lt != COAT)) return false;
@@ -382,14 +405,16 @@ namespace BSDF
         if (!surface.Coated() && (lt == COAT)) return false;
         return true;
     }
-    ZR_D float LobeAlpha(const ShadingData& surface, LOBE lt)
+    template<class SD>
+    ZR_D float LobeAlpha(const SD& surface, LOBE lt)
     {
         if (lt == GLOSSY_R || lt == GLOSSY_T) return surface.alpha;
         if (lt == COAT) return surface.coat_alpha;
         return 1.0f;
     }
 
-    ZR_D float3 EvalDiffuse(bool EON, const ShadingData& surface)
+    template<class SD>
+    ZR_D float3 EvalDiffuse(bool EON, const SD& surface)
     {
         float s = surface.subsurface == 0 ? 1 : surface.subsurface * 0.5f;
         float diffuseRoughness = sqrtf(surface.alpha);
@@ -403,49 +428,58 @@ namespace BSDF
         Math::CoordinateSystem onb = Math::CoordinateSystem::Build(normal);
         return mad(wiLocal.x, onb.b1, mad(wiLocal.y, onb.b2, wiLocal.z * normal));
     }
-    ZR_D float DiffusePdf(const ShadingData& surface) { return surface.ndotwi * ONE_OVER_PI; }
-    ZR_D float3 EvalGloss(const ShadingData& surface, float3 fr)
+    template<class SD>
+    ZR_D float DiffusePdf(const SD& surface) { return surface.ndotwi * ONE_OVER_PI; }
+    template<class SD>
+    ZR_D float3 EvalGloss(const SD& surface, float3 fr)
     {
         return GGXMicrofacetBRDF(surface.alpha, surface.ndotwh, surface.ndotwo, surface.ndotwi, fr, surface.GlossSpecular());
     }
-    ZR_D float3 SampleGloss(const ShadingData& surface, float3 shadingNormal, float2 u)
+    template<class SD>
+    ZR_D float3 SampleGloss(const SD& surface, float3 shadingNormal, float2 u)
     {
         if (surface.GlossSpecular())
             return reflect(-surface.wo, shadingNormal);
         float3 wh = SampleGGXMicrofacet(surface.wo, surface.alpha, shadingNormal, u);
         return reflect(-surface.wo, wh);
     }
-    ZR_D float GlossPdf(const ShadingData& surface)
+    template<class SD>
+    ZR_D float GlossPdf(const SD& surface)
     {
         if (surface.GlossSpecular())
             return surface.ndotwh >= MIN_N_DOT_H_SPECULAR ? 1.0f : 0.0f;
         float pdf = GGXMicrofacetPdf(surface.alpha, surface.ndotwh, surface.ndotwo);
         return pdf / 4.0f;
     }
-    ZR_D float EvalTranslucentTr(const ShadingData& surface, float fr)
+    template<class SD>
+    ZR_D float EvalTranslucentTr(const SD& surface, float fr)
     {
         return GGXMicrofacetBTDF(surface.alpha, surface.ndotwh, surface.ndotwo, surface.ndotwi, surface.whdotwo,
             surface.whdotwi, surface.eta, fr, surface.GlossSpecular());
     }
-    ZR_D float EvalCoat(const ShadingData& surface, float Fr)
+    template<class SD>
+    ZR_D float EvalCoat(const SD& surface, float Fr)
     {
         return surface.coat_weight * GGXMicrofacetBRDF(surface.coat_alpha, surface.ndotwh, surface.ndotwo, surface.ndotwi,
             f3(Fr), surface.CoatSpecular()).x;
     }
-    ZR_D float3 SampleCoat(const ShadingData& surface, float3 shadingNormal, float2 u)
+    template<class SD>
+    ZR_D float3 SampleCoat(const SD& surface, float3 shadingNormal, float2 u)
     {
         float3 wh = surface.CoatSpecular() ? shadingNormal :
             SampleGGXMicrofacet(surface.wo, surface.coat_alpha, shadingNormal, u);
         return reflect(-surface.wo, wh);
     }
-    ZR_D float CoatPdf(const ShadingData& surface)
+    template<class SD>
+    ZR_D float CoatPdf(const SD& surface)
     {
         if (surface.CoatSpecular())
             return surface.ndotwh >= MIN_N_DOT_H_SPECULAR ? 1.0f : 0.0f;
         float pdf = GGXMicrofacetPdf(surface.coat_alpha, surface.ndotwh, surface.ndotwo);
         return pdf / 4.0f;
     }
-    ZR_D float3 TranslucentTrOverPdf(const ShadingData& surface, float fr)
+    template<class SD>
+    ZR_D float3 TranslucentTrOverPdf(const SD& surface, float fr)
     {
         if (surface.GlossSpecular())
             return (1 - fr) * surface.TransmissionTint();
@@ -457,7 +491,8 @@ namespace BSDF
         // exp(c * log(coat_color))
         return f3(zr_expf(c * zr_logf(coat_color.x)), zr_expf(c * zr_logf(coat_color.y)), zr_expf(c * zr_logf(coat_color.z)));
     }
-    ZR_D float3 BaseWeight(const ShadingData& surface)
+    template<class SD>
+    ZR_D float3 BaseWeight(const SD& surface)
     {
         float3 base_weight = f3(1);
         if (surface.Coated())
@@ -475,14 +510,16 @@ namespace BSDF
         }
         return base_weight;
     }
-    ZR_D float3 TransmittanceToDielectricBaseTr(const ShadingData& surface)
+    template<class SD>
+    ZR_D float3 TransmittanceToDielectricBaseTr(const SD& surface)
     {
         float3 base_weight = BaseWeight(surface);
         float reflectance_g = surface.GlossSpecular() ? 0 :
             GGXReflectance_Dielectric(surface.rho, surface.alpha, surface.ndotwo, surface.eta);
         return (1 - reflectance_g) * base_weight;
     }
-    ZR_D float3 DielectricBaseSpecularTr(const ShadingData& surface, float Fr_g)
+    template<class SD>
+    ZR_D float3 DielectricBaseSpecularTr(const SD& surface, float Fr_g)
     {
         if (surface.invalid || !surface.specTr)
             return f3(0);
@@ -490,7 +527,8 @@ namespace BSDF
         float glossyTr = EvalTranslucentTr(surface, Fr_g);
         return glossyTr * surface.TransmissionTint() * transmittance;
     }
-    ZR_D float3 DielectricBaseDiffuseTr(const ShadingData& surface, float Fr_g)
+    template<class SD>
+    ZR_D float3 DielectricBaseDiffuseTr(const SD& surface, float Fr_g)
     {
         if (surface.invalid)
             return f3(0);
@@ -502,7 +540,8 @@ namespace BSDF
 
     struct BSDFEval { float3 f; float3 Fr_g; bool tir; };
 
-    ZR_D BSDFEval Unified(const ShadingData& surface)
+    template<class SD>
+    ZR_D BSDFEval Unified(const SD& surface)
     {
         BSDFEval ret;
         ret.f = f3(0); ret.Fr_g = f3(0); ret.tir = false;
@@ -565,7 +604,8 @@ namespace BSDF
     };
     struct BSDFSamplerEval { float pdf; float3 bsdfOverPdf; float3 f; };
 
-    ZR_D BSDFSample SampleBSDF_NoDiffuse(float3 normal, ShadingData surface, float2 u_c, float2 u_g,
+    template<class SD>
+    ZR_D BSDFSample SampleBSDF_NoDiffuse(float3 normal, SD surface, float2 u_c, float2 u_g,
         float u_wrs_0, float u_wrs_1)
     {
         BSDFSample ret = BSDFSample::Init();
@@ -627,7 +667,8 @@ namespace BSDF
         return ret;
     }
 
-    ZR_D BSDFSample SampleBSDF_NoDiffuse(float3 normal, const ShadingData& surface, RNG& rng)
+    template<class SD>
+    ZR_D BSDFSample SampleBSDF_NoDiffuse(float3 normal, const SD& surface, RNG& rng)
     {
         float2 u_c = rng.Uniform2D();
         float2 u_g = rng.Uniform2D();
@@ -636,7 +677,8 @@ namespace BSDF
         return SampleBSDF_NoDiffuse(normal, surface, u_c, u_g, u_wrs_0, u_wrs_1);
     }
 
-    ZR_D BSDFSample SampleBSDF_NoSpecTr(float3 normal, ShadingData surface, float2 u_coat, float2 u_g, float2 u_d,
+    template<class SD>
+    ZR_D BSDFSample SampleBSDF_NoSpecTr(float3 normal, SD surface, float2 u_coat, float2 u_g, float2 u_d,
         float u_wrs_g, float u_wrs_dr, float u_wrs_dt)
     {
         BSDFSample ret = BSDFSample::Init();
@@ -719,7 +761,8 @@ namespace BSDF
     }
 
     // Always consumes exactly 9 uniforms (BSDFSampling.hlsli:318-327)
-    ZR_D BSDFSample SampleBSDF(float3 normal, const ShadingData& surface, RNG& rng)
+    template<class SD>
+    ZR_D BSDFSample SampleBSDF(float3 normal, const SD& surface, RNG& rng)
     {
         float2 u_c = rng.Uniform2D();
         float2 u_g = rng.Uniform2D();
@@ -732,7 +775,8 @@ namespace BSDF
         return SampleBSDF_NoDiffuse(normal, surface, u_c, u_g, u_wrs_0, u_wrs_1);
     }
 
-    ZR_D BSDFSamplerEval EvalBSDFSampler_NoSpecTr(float3 normal, ShadingData surface, float3 wi, LOBE lobe,
+    template<class SD>
+    ZR_D BSDFSamplerEval EvalBSDFSampler_NoSpecTr(float3 normal, SD surface, float3 wi, LOBE lobe,
         float2 u_c, float2 u_g, float2 u_d)
     {
         BSDFSamplerEval ret;
@@ -798,7 +842,8 @@ namespace BSDF
         return ret;
     }
 
-    ZR_D BSDFSamplerEval EvalBSDFSampler_NoDiffuse(float3 normal, ShadingData surface, float3 wi, LOBE lobe)
+    template<class SD>
+    ZR_D BSDFSamplerEval EvalBSDFSampler_NoDiffuse(float3 normal, SD surface, float3 wi, LOBE lobe)
     {
         float3 wh = surface.SetWi(wi, normal);
         BSDFEval eval = Unified(surface);
@@ -850,7 +895,8 @@ namespace BSDF
         return ret;
     }
 
-    ZR_D BSDFSamplerEval EvalBSDFSampler(float3 normal, const ShadingData& surface, float3 wi, LOBE lobe, RNG& rng)
+    template<class SD>
+    ZR_D BSDFSamplerEval EvalBSDFSampler(float3 normal, const SD& surface, float3 wi, LOBE lobe, RNG& rng)
     {
         float2 u_c = rng.Uniform2D();
         float2 u_g = rng.Uniform2D();
@@ -861,7 +907,8 @@ namespace BSDF
         return EvalBSDFSampler_NoDiffuse(normal, surface, wi, lobe);
     }
 
-    ZR_D float BSDFSamplerPdf_NoDiffuse(float3 normal, ShadingData surface, float3 wi)
+    template<class SD>
+    ZR_D float BSDFSamplerPdf_NoDiffuse(float3 normal, SD surface, float3 wi)
     {
         float3 wh = surface.SetWi(wi, normal);
         float pdf_base = 1;
@@ -904,7 +951,8 @@ namespace BSDF
         return pdf_g;
     }
 
-    ZR_D float BSDFSamplerPdf(float3 normal, ShadingData surface, float3 wi_z, RNG& rng)
+    template<class SD>
+    ZR_D float BSDFSamplerPdf(float3 normal, SD surface, float3 wi_z, RNG& rng)
     {
         if (surface.specTr)
             return BSDFSamplerPdf_NoDiffuse(normal, surface, wi_z);

@@ -70,12 +70,14 @@ ZR_D void AccountCost(unsigned long long* costMap, uint32_t W, uint32_t H, uint3
         atomicAdd(&costMap[(size_t)(y >> 5) * ((W + 31) >> 5) + (x >> 5)], (unsigned long long)(clock64() - t0));
 }
 
-struct Pixel
+template<class SD>
+struct PixelT
 {
     GFlags flags; float roughness; float z; float3 pos, normal, origin; float2 lensSample;
-    BSDF::ShadingData surface; float eta_next;
+    SD surface; float eta_next;
     float coatRoughness, coatIor;   // raw coat parameters (ShadingData keeps alpha / relative eta)
 };
+using Pixel = PixelT<BSDF::ShadingData>;
 
 ZR_D float3 row3(const float m[3][4], int r) { return f3(m[r][0], m[r][1], m[r][2]); }
 
@@ -86,12 +88,14 @@ ZR_D GFlags FlagsAt(const uint4* __restrict__ core, uint32_t W, int x, int y, fl
     return DecodeFlags(w & 0xff);
 }
 
-// prev == false: current camera / jitter / frame number; true: previous frame's
-ZR_D Pixel LoadPixel(const FrameView& f, const SceneDev& sc, const uint4* __restrict__ core, const uint2* __restrict__ coat,
+// prev == false: current camera / jitter / frame number; true: previous frame's. SD: the surface type of the calling kernel
+// (BSDF::ShadingDataT<scene material features>)
+template<class SD = BSDF::ShadingData>
+ZR_D PixelT<SD> LoadPixel(const FrameView& f, const SceneDev& sc, const uint4* __restrict__ core, const uint2* __restrict__ coat,
     int px, int py, bool prev, int coatX, int coatY)
 {
     const zr_frame_constants& fc = f.fc;
-    Pixel p;
+    PixelT<SD> p;
     const uint4 c = ld128(&core[(size_t)py * f.W + px]);
     p.flags = DecodeFlags(c.w & 0xff);
     p.roughness = (float)((c.w >> 8) & 0xff) / 255.0f;
@@ -130,7 +134,7 @@ ZR_D Pixel LoadPixel(const FrameView& f, const SceneDev& sc, const uint4* __rest
     }
     p.coatRoughness = coat_roughness; p.coatIor = coat_ior;
     const float3 wo = normalize(p.origin - p.pos);
-    p.surface = BSDF::ShadingData::Init(p.normal, wo, p.flags.metallic, p.roughness, baseColor, BSDF::ETA_AIR, p.eta_next,
+    p.surface = SD::Init(p.normal, wo, p.flags.metallic, p.roughness, baseColor, BSDF::ETA_AIR, p.eta_next,
         p.flags.transmissive, p.flags.trDepthGt0 ? 1.0f : 0.0f, to_half(baseW), coat_weight, coat_color, coat_roughness,
         coat_ior, sc.rho);
     return p;

@@ -148,7 +148,8 @@ struct EmissiveData
 // RIS over BSDF and light samples (Resampling.hlsli:116-331) as block-synchronous phases (zr_rpt.cuh): every
 // thread of the block walks the same 2 + 3 sample slots, `act` / the per-pixel sample counts predicate the work.
 #define ZR_PHASE() __syncthreads()
-ZR_D Reservoir RIS_InitialCandidates_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, float roughness, BSDF::ShadingData surface,
+template<class SD>
+ZR_D Reservoir RIS_InitialCandidates_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, float roughness, SD surface,
     uint32_t sampleSetIdx, int numBsdfSamples, RNG& rng)
 {
     Reservoir r = Reservoir::Init();
@@ -261,11 +262,14 @@ ZR_D bool PlaneHeuristicDI(float3 samplePos, float3 currNormal, float3 currPos, 
     return fabsf(planeDist) <= tolerance * linearDepth;
 }
 
-struct TemporalCandidate { BSDF::ShadingData surface; float3 pos, normal; int px, py; bool valid; };
+template<class SD>
+struct TemporalCandidateT { SD surface; float3 pos, normal; int px, py; bool valid; };
+using TemporalCandidate = TemporalCandidateT<BSDF::ShadingData>;
 
-ZR_D TemporalCandidate FindTemporalCandidate(const FrameView& f, const SceneDev& sc, float3 pos, float3 normal, float roughness, const BSDF::ShadingData& surface, float2 prevUV)
+template<class SD>
+ZR_D TemporalCandidateT<SD> FindTemporalCandidate(const FrameView& f, const SceneDev& sc, float3 pos, float3 normal, float roughness, const SD& surface, float2 prevUV)
 {
-    TemporalCandidate c; c.valid = false; c.px = c.py = 0; c.pos = c.normal = f3(0);
+    TemporalCandidateT<SD> c; c.valid = false; c.px = c.py = 0; c.pos = c.normal = f3(0);
     if (prevUV.x < 0.0f || prevUV.y < 0.0f || prevUV.x > 1.0f || prevUV.y > 1.0f) return c;
     const float2 renderDim = f2((float)f.W, (float)f.H);
     float2 pp = prevUV * renderDim;
@@ -275,7 +279,7 @@ ZR_D TemporalCandidate FindTemporalCandidate(const FrameView& f, const SceneDev&
     if (prevFlags.invalid || prevFlags.emissive || (fabsf(prevRoughness - roughness) > 0.15f) ||
         (prevFlags.metallic != surface.metallic) || (prevFlags.transmissive != surface.specTr))
         return c;
-    Pixel p = LoadPixel(f, sc, f.pcore, f.pcoat, ppx, ppy, true, ppx, ppy);
+    const PixelT<SD> p = LoadPixel<SD>(f, sc, f.pcore, f.pcoat, ppx, ppy, true, ppx, ppy);
     // note: the depth passed to the plane test is the PREVIOUS pixel's (Resampling.hlsli:77)
     if (!PlaneHeuristicDI(p.pos, normal, pos, p.z))
         return c;
@@ -285,7 +289,8 @@ ZR_D TemporalCandidate FindTemporalCandidate(const FrameView& f, const SceneDev&
 
 // Resampling.hlsli temporal resample (OffsetPathTarget_CtT / _TtC + TemporalResample1) as phases:
 // BSDF value at the temporal pixel | its shadow segment | BSDF value at the current pixel | its shadow segment
-ZR_D void TemporalResample1_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, const BSDF::ShadingData& surface, TemporalCandidate candidate,
+template<class SD>
+ZR_D void TemporalResample1_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, const SD& surface, TemporalCandidateT<SD> candidate,
     const zr_rdi_reservoir* prevRes, uint32_t W, Reservoir& r_curr, RNG& rng)
 {
     Reservoir r_prev = Reservoir::Init();
@@ -331,7 +336,7 @@ ZR_D void TemporalResample1_Sync(bool act, const SceneDev& sc, float3 pos, float
     // ---- temporal sample in the current domain ----
     const bool doTtC = act && (r_prev.lightIdx != UINT32_MAX_);
     EmissiveData prevEmissive;
-    BSDF::ShadingData surfaceWi = surface;
+    SD surfaceWi = surface;
     float3 target_curr = f3(0);
     if (doTtC)
     {
@@ -396,8 +401,9 @@ struct PairwiseMIS
         m_c += 1 - (numerator / denom);
     }
     // phases: shadow segment c<-i | BSDF value c<-i | shadow segment i<-c | BSDF value i<-c
-    ZR_D void Stream_Sync(bool act, const SceneDev& sc, const Reservoir& r_c, float3 pos_c, float3 normal_c, BSDF::ShadingData surface_c, const Reservoir& r_i,
-        float3 pos_i, float3 normal_i, BSDF::ShadingData surface_i, RNG& rng)
+    template<class SD>
+    ZR_D void Stream_Sync(bool act, const SceneDev& sc, const Reservoir& r_c, float3 pos_c, float3 normal_c, SD surface_c, const Reservoir& r_i,
+        float3 pos_i, float3 normal_i, SD surface_i, RNG& rng)
     {
         float3 target_c_y_i = f3(0), target_i_y_c = f3(0.0f);
         float m_i = 0;

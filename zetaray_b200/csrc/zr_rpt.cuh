@@ -268,7 +268,8 @@ namespace RPT
         }
     };
 
-    ZR_D bool IsSpecularSurface(const ShadingData& surface)
+    template<class SD>
+    ZR_D bool IsSpecularSurface(const SD& surface)
     {
         return surface.GlossSpecular() && (surface.metallic || surface.specTr) && (!surface.Coated() || surface.CoatSpecular());
     }
@@ -376,7 +377,8 @@ namespace RPT
     }
 
     // ReSTIR_PT_NEE.hlsli:145-222 -- everything after the closest-hit query of the BSDF-sampled direction
-    ZR_D DirectLightingEstimate NEE_Bsdf_Finish(const SceneDev& sc, float3 pos, const ShadingData& surface, int nextBounce,
+    template<class SD>
+    ZR_D DirectLightingEstimate NEE_Bsdf_Finish(const SceneDev& sc, float3 pos, const SD& surface, int nextBounce,
         int maxNumBounces, BSDF::BSDFSample& bsdfSample, const HitEmissive& hitInfo)
     {
         DirectLightingEstimate ret = DirectLightingEstimate::Init();
@@ -420,7 +422,8 @@ namespace RPT
     // sampler pdf + MIS. `surface` is the caller's copy with wi set (the reference passes it by value).
     struct NeeLightState { DirectLightingEstimate ret; float3 ld; float t, lightPdf, dwdA; bool facing; };
 
-    ZR_D NeeLightState NEE_Emissive_Begin(const SceneDev& sc, float3 pos, float3 normal, ShadingData& surface, uint32_t sampleSetIdx, RNG& rng)
+    template<class SD>
+    ZR_D NeeLightState NEE_Emissive_Begin(const SceneDev& sc, float3 pos, float3 normal, SD& surface, uint32_t sampleSetIdx, RNG& rng)
     {
         NeeLightState st;
         st.ret = DirectLightingEstimate::Init();
@@ -459,24 +462,25 @@ namespace RPT
     // Path context carried from replay to the reconnection step. The reference round-trips it
     // through the r-buffers (RGBA16F + 2 x RGBA32UI + R16UI, Shift.hlsli:191-358); Quantize() applies
     // that storage precision so keeping the context on chip gives the same numbers.
-    struct OffsetPathContext
+    template<class SD>
+    struct OffsetPathContextT
     {
         float3 throughput, pos, normal;
-        ShadingData surface;
+        SD surface;
         float eta_curr, eta_next;
         RNG rngReplay;
 
-        static ZR_D OffsetPathContext Init()
+        static ZR_D OffsetPathContextT Init()
         {
-            OffsetPathContext c;
+            OffsetPathContextT c;
             c.throughput = f3(0); c.pos = f3(0); c.normal = f3(0);
-            c.surface = ShadingData::InitEmpty();
+            c.surface = SD::InitEmpty();
             c.eta_curr = BSDF::ETA_AIR; c.eta_next = BSDF::DEFAULT_ETA_MAT; c.rngReplay.State = 0;
             return c;
         }
-        ZR_D OffsetPathContext Quantize() const
+        ZR_D OffsetPathContextT Quantize() const
         {
-            OffsetPathContext ctx = Init();
+            OffsetPathContextT ctx = Init();
             ctx.throughput = f3(to_half(throughput.x), to_half(throughput.y), to_half(throughput.z));
             if (dot(ctx.throughput, ctx.throughput) == 0)
                 return ctx;
@@ -502,18 +506,20 @@ namespace RPT
                 float coat_eta = surface.coat_eta >= 1.0f ? surface.coat_eta : 1.0f / surface.coat_eta;
                 coat_ior = mad(Math::UNorm8ToFloat(Math::FloatToUNorm8((coat_eta - 1.0f) / 1.5f)), 1.5f, 1.0f);
             }
-            ctx.surface = ShadingData::Init(ctx.normal, wo, metallic, roughness, baseColor, ctx.eta_curr, eta_next_, specTr,
+            ctx.surface = SD::Init(ctx.normal, wo, metallic, roughness, baseColor, ctx.eta_curr, eta_next_, specTr,
                 trDepth, to_half(subsurface), coat_weight, coat_color, coat_roughness, coat_ior, surface.rho);
             return ctx;
         }
     };
+    using OffsetPathContext = OffsetPathContextT<ShadingData>;
 
     // Shift.hlsli:377-474 (Replay) + :818-859 (Replay_kGt2) as one phase loop: random replay of the first k-2
     // bounces from a new primary vertex. Returns the unquantised context; throughput == 0 means the replay failed.
-    ZR_D OffsetPathContext Replay_kGt2_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, float ior, const ShadingData& surface,
+    template<class SD>
+    ZR_D OffsetPathContextT<SD> Replay_kGt2_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, float ior, const SD& surface,
         const Reconnection& rc, float alpha_min)
     {
-        OffsetPathContext ctx = OffsetPathContext::Init();
+        OffsetPathContextT<SD> ctx = OffsetPathContextT<SD>::Init();
         BSDF::BSDFSample bsdfSample = BSDF::BSDFSample::Init();
         const int numBounces = (int)rc.k - 2;
         int bounce = 0;
@@ -558,7 +564,7 @@ namespace RPT
                     ctx.pos = mad(hitInfo.t, bsdfSample.wi, ctx.pos);
                     ctx.normal = hitInfo.normal;
                     bounce++;
-                    if (inTranslucentMedium && (ctx.surface.trDepth > 0))
+                    if (inTranslucentMedium && ctx.surface.TrDepthGt0())
                     {
                         float3 c = ctx.surface.baseColor_Fr0_TrCol;
                         float3 extCoeff = f3(-zr_logf(c.x), -zr_logf(c.y), -zr_logf(c.z)) / ctx.surface.trDepth;
@@ -599,12 +605,12 @@ namespace RPT
     // `replayed` = context from Replay_kGt2_Sync (already quantised) when k > 2.
     // CASE: 0 = the reconnection case is read from `rc` (fused kernels); 1 / 2 / 3 = every thread of the block holds that case
     // (the queued kernels draw their work from per-case queues), so the phases of the other cases compile away.
-    template<int CASE = 0>
-    ZR_D OffsetPath Shift2_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, float ior, const ShadingData& surface,
-        const Reconnection& rc, const OffsetPathContext* replayed, float alpha_min)
+    template<int CASE = 0, class SD>
+    ZR_D OffsetPath Shift2_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, float ior, const SD& surface,
+        const Reconnection& rc, const OffsetPathContextT<SD>* replayed, float alpha_min)
     {
         OffsetPath ret; ret.target = f3(0); ret.partialJacobian = 0; ret.surfKMin1Tramsmissive = false;
-        OffsetPathContext ctx = OffsetPathContext::Init();
+        OffsetPathContextT<SD> ctx = OffsetPathContextT<SD>::Init();
         const bool case1 = CASE == 0 ? rc.IsCase1() : CASE == 1, case2 = CASE == 0 ? rc.IsCase2() : CASE == 2,
             case3 = CASE == 0 ? rc.IsCase3() : CASE == 3;
         bool go = act;
@@ -688,7 +694,7 @@ namespace RPT
                 if (!GetMaterialData(sc, -w_k_min_1, ctx.eta_curr, hitInfo, ctx.surface, ctx.eta_next)) { step = false; go = false; }
                 else
                 {
-                    if (inTranslucentMedium && (ctx.surface.trDepth > 0))
+                    if (inTranslucentMedium && ctx.surface.TrDepthGt0())
                     {
                         float3 c = ctx.surface.baseColor_Fr0_TrCol;
                         float3 extCoeff = f3(-zr_logf(c.x), -zr_logf(c.y), -zr_logf(c.z)) / ctx.surface.trDepth;
@@ -707,7 +713,7 @@ namespace RPT
         }
         // ---- the reconnection vertex: case 1 re-evaluates the sampler towards x_{k+1}; cases 2/3 re-evaluate NEE ----
         const bool nee = go && !case1;
-        ShadingData surfWi = ctx.surface;          // EvalDirect_* take the surface by value and set wi on the copy
+        SD surfWi = ctx.surface;          // EvalDirect_* take the surface by value and set wi on the copy
         float3 wiE = rc.w_k_lightNormal_w_sky;      // case 1 / 2: w_k
         float3 nrmE = ctx.normal;
         LOBE lobeE = rc.lobe_k;

@@ -147,8 +147,9 @@ namespace
     // ---- path generation helpers (k_pathtrace, rpt.cu) ----
     struct PrevHit { float alpha_lobe; float3 wi; float pdf; BSDF::LOBE lobe; };
 
+    template<class SD>
     ZR_D void MaybeSetCase2OrCase3(int pathVertex, float3 pos, float3 normal, float t, uint32_t ID, uint32_t meshIdx,
-        const BSDF::ShadingData& surface, const PrevHit& prevHit, const DirectLightingEstimate& ls, uint32_t seed_nee,
+        const SD& surface, const PrevHit& prevHit, const DirectLightingEstimate& ls, uint32_t seed_nee,
         Reconnection& rc, float alpha_min)
     {
         const float alpha_lobe_direct = BSDF::LobeAlpha(surface, ls.lobe);

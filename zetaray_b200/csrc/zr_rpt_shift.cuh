@@ -6,6 +6,7 @@
 // Block size: 512 threads x 1 block per SM (128 registers). At 64 registers the replay classes spill ~1 KB per thread, more
 // than L1 holds at a full SM. Measured on an H100 SXM (700 W), spatial + temporal shift per bench frame: 0.88 + 0.78 ms at
 // 512 x 1, 0.87 + 0.85 at 768 x 1 (80 registers), 0.96 + 0.83 at 512 x 2 (64 registers), 0.99 + 0.87 at 1024 x 1 (DESIGN 4.1).
+// Swept before the plain material build existed; both builds use this shape.
 #pragma once
 #include "zr_rpt_spatial.h"
 
@@ -34,12 +35,13 @@ namespace
 
 
     // item = x | y << 16 | flag << 30 | direction << 31 (x < 65536, y < 16384); flag: temporal pass only, "the tighter plane test
-    // of the replay passed" (ReSTIR_PT_Replay.hlsl:404)
-    template<int CASE, bool REPLAY, bool TEMPORAL>
+    // of the replay passed" (ReSTIR_PT_Replay.hlsl:404). MF: the material features the kernel is compiled for (BSDF::ShadingDataT).
+    template<int CASE, bool REPLAY, bool TEMPORAL, uint32_t MF>
     __global__ void __launch_bounds__(SHIFT_THREADS, SHIFT_MINBLOCKS) k_shift(SceneDev sc, FrameView f, RptParams prm,
         const zr_rpt_reservoir* __restrict__ resIn, const zr_rpt_reservoir* __restrict__ resPrev, const uint16_t* __restrict__ neighbor,
         const uint32_t* __restrict__ queue, uint32_t* __restrict__ counters, uint32_t cls, ShiftResult* __restrict__ out)
     {
+        using SD = BSDF::ShadingDataT<MF>;
         __shared__ uint32_t s_base;
         const uint32_t total = counters[cls];
         for (;;)
@@ -54,7 +56,7 @@ namespace
             uint32_t dir = 0;
             bool replayOk = act;
             Reservoir r = Reservoir::Init();
-            Pixel p, pr;
+            PixelT<SD> p, pr;
             if (act)
             {
                 const uint32_t item = __ldg(&queue[base + threadIdx.x]);
@@ -70,11 +72,11 @@ namespace
                     r = Reservoir::Load_NonReconnection(rec);
                     r.rc.x_k_in_motion = false;
                     r.Load_Reconnection(rec);
-                    if (dir == 0) p = LoadPixel(f, sc, f.core, f.coat, nx, ny, false, x, y);
-                    else p = LoadPixel(f, sc, f.core, f.coat, x, y, false, x, y);
+                    if (dir == 0) p = LoadPixel<SD>(f, sc, f.core, f.coat, nx, ny, false, x, y);
+                    else p = LoadPixel<SD>(f, sc, f.core, f.coat, x, y, false, x, y);
                     if (REPLAY)
                     {
-                        if (dir == 0) pr = LoadPixel(f, sc, f.core, f.coat, nx, ny, false, nx, ny);
+                        if (dir == 0) pr = LoadPixel<SD>(f, sc, f.core, f.coat, nx, ny, false, nx, ny);
                         else pr = p;
                     }
                 }
@@ -93,12 +95,12 @@ namespace
                         if (dir == 0) XkToPrev(sc, r.rc);
                         else XkToCurr(sc, r.rc);
                     }
-                    if (dir == 0) p = LoadPixel(f, sc, f.pcore, f.pcoat, ppx, ppy, true, x, y);
-                    else p = LoadPixel(f, sc, f.core, f.coat, x, y, false, x, y);
+                    if (dir == 0) p = LoadPixel<SD>(f, sc, f.pcore, f.pcoat, ppx, ppy, true, x, y);
+                    else p = LoadPixel<SD>(f, sc, f.core, f.coat, x, y, false, x, y);
                     if (REPLAY) pr = p;
                 }
             }
-            OffsetPathContext ctx = OffsetPathContext::Init();
+            OffsetPathContextT<SD> ctx = OffsetPathContextT<SD>::Init();
             if (REPLAY)
             {
                 ZR_PHASE();
@@ -130,10 +132,10 @@ namespace
     // share nothing but read-only inputs -- each has its own queue and claim cursor, and the two items of a pixel write disjoint bytes of
     // its ShiftResult -- so they go to three streams (fork / join by events around the stage): a persistent block leaves as soon as its
     // queue is drained, which frees its slot for the next class's blocks. Measured on the strip-sharded frame, where every queue is a
-    // fraction of the machine (DESIGN 7).
+    // fraction of the machine (DESIGN 7). plain: the scene's materials have none of the features of BSDF::MF_ALL.
     template<bool TEMPORAL>
     zr_status LaunchShifts(const SpatialQueued& q, const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm,
-        const zr_rpt_reservoir* resIn, const zr_rpt_reservoir* resPrev, const uint16_t* neighbor, cudaStream_t stream)
+        const zr_rpt_reservoir* resIn, const zr_rpt_reservoir* resPrev, const uint16_t* neighbor, bool plain, cudaStream_t stream)
     {
         const uint32_t grid = (uint32_t)ss.numSMs * SHIFT_MINBLOCKS;
         cudaStream_t s1 = ss.aux[0], s2 = ss.aux[1];
@@ -141,7 +143,7 @@ namespace
         ZR_CUDA(cudaStreamWaitEvent(s1, ss.evFork, 0));
         ZR_CUDA(cudaStreamWaitEvent(s2, ss.evFork, 0));
 #define ZR_LAUNCH_SHIFT(CASE, REPLAY, CLS, STREAM) \
-        k_shift<CASE, REPLAY, TEMPORAL><<<grid, SHIFT_THREADS, 0, STREAM>>>(sc, f, prm, resIn, resPrev, neighbor, q.d_queue + (size_t)(CLS) * q.capacity, \
+        (plain ? k_shift<CASE, REPLAY, TEMPORAL, BSDF::MF_NONE> : k_shift<CASE, REPLAY, TEMPORAL, BSDF::MF_ALL>)<<<grid, SHIFT_THREADS, 0, STREAM>>>(sc, f, prm, resIn, resPrev, neighbor, q.d_queue + (size_t)(CLS) * q.capacity, \
             q.d_counters, CLS, q.d_shift); \
         zr::count_launch()
         ZR_LAUNCH_SHIFT(1, false, 0, stream);

@@ -59,10 +59,12 @@ struct SpatialQueued
     bool swizzled = false;                      // even widths: 3-D map {128-byte record pair, W / 2, H} with the 128-byte swizzle
 
     zr_status Build(uint32_t w, uint32_t h, const zr_rpt_reservoir* res0, const zr_rpt_reservoir* res1);
-    // resIn must be one of the two planes given to Build
+    // resIn must be one of the two planes given to Build. plain: the scene's materials use none of the features of BSDF::MF_ALL, so
+    // the shifts run the kernels compiled without them.
     zr_status Run(const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm, const zr_rpt_reservoir* resIn,
-        zr_rpt_reservoir* resOut, const float4* target, float4* finalImg, const uint16_t* neighbor, const uint16_t* threadMap, cudaStream_t stream);
+        zr_rpt_reservoir* resOut, const float4* target, float4* finalImg, const uint16_t* neighbor, const uint16_t* threadMap, bool plain,
+        cudaStream_t stream);
     zr_status RunTemporal(const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm, zr_rpt_reservoir* resCurr,
-        const zr_rpt_reservoir* resPrev, float4* target, float4* finalImg, cudaStream_t stream);
+        const zr_rpt_reservoir* resPrev, float4* target, float4* finalImg, bool plain, cudaStream_t stream);
 };
 } // namespace zr

@@ -178,7 +178,8 @@ ZR_D bool Visibility_Segment_Precise(const SceneDev& sc, float3 origin, float3 w
 }
 
 // GetMaterialData (RayQuery.hlsli:452-510), textures unsupported (factors only)
-ZR_D bool GetMaterialData(const SceneDev& sc, float3 wo, float eta_curr, Hit& hitInfo, BSDF::ShadingData& surface, float& eta)
+template<class SD>
+ZR_D bool GetMaterialData(const SceneDev& sc, float3 wo, float eta_curr, Hit& hitInfo, SD& surface, float& eta)
 {
     const zr_material mat = LoadMaterial(sc, hitInfo.matIdx);
     const bool hitBackface = dot(wo, hitInfo.normal) < 0;
@@ -199,7 +200,7 @@ ZR_D bool GetMaterialData(const SceneDev& sc, float3 wo, float eta_curr, Hit& hi
     float3 coat_color = Mat::GetCoatColor(mat);
     float coat_roughness = Mat::GetCoatRoughness(mat);
     float coat_ior = Mat::GetCoatIOR(mat);
-    surface = BSDF::ShadingData::Init(hitInfo.normal, wo, metallic >= 0.9f, roughness, baseColor, eta_curr, eta_next, tr,
+    surface = SD::Init(hitInfo.normal, wo, metallic >= 0.9f, roughness, baseColor, eta_curr, eta_next, tr,
         trDepth, subsurface, coat_weight, coat_color, coat_roughness, coat_ior, sc.rho);
     return true;
 }

@@ -315,4 +315,5 @@ struct zr_scene
     bool samplesValid = false;      // zr_presample_emissives ran since the sets were (re)configured
     zr_voxel_sample* d_lvg = nullptr;
     bool lvgValid = false;          // zr_build_light_voxel_grid ran since the grid was (re)configured
+    uint32_t materialFeatures = 0;  // ZR_MATERIAL_* over the material table (zr_scene_create); materials never change afterwards
 };
