@@ -2,7 +2,7 @@
 
 
 def run():
-    from tests.test_rdi_gpu import _frame_loop
-    problems, _ = _frame_loop("glossy", 160, 90, 3, full=True)
+    from tests.parity import WHOLE_FRAME, frame_parity
+    problems, _ = frame_parity("glossy", 160, 90, 3, WHOLE_FRAME)
     assert not problems, "\n".join(problems)
     print("smoke frames ok (G-buffer -> ReSTIR DI -> ReSTIR PT -> compositing/firefly -> TAA, 160x90 x 3 frames, bit-exact vs oracle)")

@@ -5,7 +5,7 @@ that lobe, so the frames would differ from the oracle."""
 import ctypes as C
 import pytest
 
-from tests.test_rdi_gpu import _frame_loop
+from tests.parity import WHOLE_FRAME, frame_parity
 
 COAT, TRANSMISSION, THIN_WALLED = 0x1, 0x2, 0x4     # ZR_MATERIAL_* (include/zr_abi.h)
 
@@ -66,9 +66,7 @@ def test_one_material_sets_its_feature(name):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(CHANGED))
-def test_one_material_frames_match_the_oracle(name, monkeypatch):
+def test_one_material_frames_match_the_oracle(name):
     # ReSTIR DI, ReSTIR PT (path generation, temporal and spatial reuse), compositing and TAA, bit-exact, 3 frames
-    from tests import scene_util
-    monkeypatch.setitem(scene_util.SCENES, name, CHANGED[name][1])
-    problems, _ = _frame_loop(name, 256, 144, 3, full=True)
+    problems, _ = frame_parity(CHANGED[name][1](), 256, 144, 3, WHOLE_FRAME)
     assert not problems, "\n".join(problems)

@@ -19,37 +19,23 @@ DI_MODES = {"no_reuse": dict(temporal_resample=0, spatial_resample=0), "temporal
 
 
 def _device_replicas(T, di_params, presample):
-    from zetaray_b200 import _lib
     from zetaray_b200.camera import FrameSequence
-    from zetaray_b200.passes import Scene, GBuffers, GBufferRT, DirectLighting, download_image
-    sc = Scene(T.flat)
-    sc.prelighting()
-    if presample:
-        sc.set_presampling(*presample)
-    gb, gpass, di = GBuffers(T.w, T.h), GBufferRT(), DirectLighting(T.w, T.h)
-    if di_params:
-        di.SetParams(**di_params)
+    from zetaray_b200.passes import download_image
+    from tests.parity import DeviceFrame
+    dev = DeviceFrame(T.flat, T.w, T.h, ("rdi",), di_params=di_params, presample=presample)
     out = []
     try:
         for r in range(REPLICAS):
-            di.ResetTemporal()
+            dev.di.ResetTemporal()
             seq = FrameSequence(T.w, T.h, jitter=False, first_frame=1 + 1000 * r)
             acc = np.zeros((T.w * T.h, 3))
             for f in range(FRAMES):
-                fc = seq.next()
-                gb.flip()
-                fi = _lib.FrameInputs()
-                fi.frame = fc
-                gb.fill_inputs(fi)
-                fi.scene = sc.handle
-                gpass.Render(fi)
-                sc.presample(fc.FrameNum)
-                di.Render(fi)
+                dev.render(seq.next())
                 if f >= WARMUP:
-                    acc += download_image(di.GetOutput(0), np.float32, 4)[:, :3]
+                    acc += download_image(dev.di.GetOutput(0), np.float32, 4)[:, :3]
             out.append(acc / (FRAMES - WARMUP))
     finally:
-        gb.close()
+        dev.close()
     return np.array(out)
 
 

@@ -1,70 +1,12 @@
 """ReSTIR DI (emissive) and the whole reference-shaped frame on the device vs the CPU oracle (bit-exact)."""
 import ctypes as C
-import numpy as np
 import pytest
 
-from tests.test_rpt_gpu import _diff_report
+from tests.parity import WHOLE_FRAME, frame_parity
 
 
-def _frame_loop(which, w, h, nframes, full=False, di_params=None, cam_path=None, accumulate=False, presample=None):
-    from zetaray_b200 import lib, check, _lib
-    from zetaray_b200.passes import Scene, GBuffers, GBufferRT, DirectLighting, IndirectLighting, Compositing, TAA, download_image
-    from tests import scene_util, rpt_util
-    flat = scene_util.SCENES[which]()
-    R = rpt_util.OracleRenderer(flat, w, h)
-    sc = Scene(flat)
-    sc.prelighting()
-    if presample:
-        R.osc.set_presampling(*presample)
-        sc.set_presampling(*presample)
-    gb = GBuffers(w, h)
-    gpass, di = GBufferRT(), DirectLighting(w, h)
-    if di_params:
-        for k, v in di_params.items():
-            setattr(R.di_params, k, v)
-        di.SetParams(**di_params)
-    ind = IndirectLighting(w, h) if full else None
-    comp = Compositing(w, h) if full else None
-    taa = TAA(w, h) if full else None
-    seq = rpt_util.FrameSequence(w, h, cam_path=cam_path, accumulate=accumulate)
-    taa_prev = np.zeros((w * h, 2), dtype=np.uint32)
-    problems = []
-    for fr in range(nframes):
-        fc = seq.next()
-        R.gbuffer(fc)
-        R.rdi(fc)
-        gb.flip()
-        fi = _lib.FrameInputs()
-        fi.frame = fc
-        gb.fill_inputs(fi)
-        fi.scene = sc.handle
-        gpass.Render(fi)
-        sc.presample(fc.FrameNum)
-        di.Render(fi)
-        check(lib.zr_stream_synchronize(None))
-        checks = [("di_reservoir", download_image(di.GetOutput(1), np.uint8, 32).view(rpt_util.RDI).reshape(-1), R.di_curr_reservoirs()),
-                  ("di_final", download_image(di.GetOutput(0), np.float32, 4).view(np.uint32), R.di_final.view(np.uint32))]
-        if fr >= 1 and R.di_params.temporal_resample and R.di_params.spatial_resample:
-            checks.append(("di_target", download_image(di.GetOutput(2), np.uint32, 2), R.di_target))
-        if full:
-            R.rpt(fc)
-            ind.Render(fi)
-            comp.Render(fi, di.GetOutput(0).d_ptr, ind.GetOutput(0).d_ptr)
-            taa.Render(fi, comp.GetOutput().d_ptr)
-            check(lib.zr_stream_synchronize(None))
-            ref_comp, ref_taa = R.post(fc, taa_prev, fr > 0)
-            taa_prev = ref_taa
-            checks.append(("indirect_final", download_image(ind.GetOutput(0), np.float32, 4).view(np.uint32), R.final.view(np.uint32)))
-            checks.append(("composited", download_image(comp.GetOutput(), np.float32, 4).view(np.uint32), ref_comp.view(np.uint32)))
-            checks.append(("taa", download_image(taa.GetOutput(), np.uint32, 2), ref_taa))
-        for name, a, b in checks:
-            msg = _diff_report(name, a, b)
-            if msg:
-                problems.append("frame %d: %s" % (fc.FrameNum, msg))
-        if problems:
-            break
-    gb.close()
-    return problems, R
+def _frame_loop(which, w, h, nframes, full=False, **kw):
+    return frame_parity(which, w, h, nframes, WHOLE_FRAME if full else ("rdi",), **kw)
 
 
 @pytest.mark.gpu

@@ -1,7 +1,5 @@
 """zr_renderer (the native frame driver) produces byte-identical frames to the passes driven one by one -- which the
 other GPU tests compare with the oracle -- including the frame-1 pre-lighting protocol, presampling and the second stream."""
-import ctypes as C
-import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
@@ -9,39 +7,27 @@ pytestmark = pytest.mark.gpu
 
 @pytest.mark.parametrize("which,presample,two_streams", [("glossy", None, True), ("glass", (16, 64), True), ("cornell", None, False)])
 def test_renderer_matches_manual_sequence(which, presample, two_streams):
-    from zetaray_b200 import lib, check, _lib
-    from zetaray_b200.passes import (Scene, GBuffers, GBufferRT, DirectLighting, IndirectLighting, Compositing, TAA, Renderer,
-                                     download_image)
+    from zetaray_b200 import lib, check
+    from zetaray_b200.passes import Scene, Renderer
     from tests import scene_util, rpt_util
+    from tests.parity import WHOLE_FRAME, DeviceFrame, pt_reservoirs, uint32x2
     w, h = 320, 180
     flat = scene_util.SCENES[which]()
-    # manual sequence
-    sc = Scene(flat)
-    sc.prelighting()
-    if presample:
-        sc.set_presampling(*presample)
-    gb, g, di, ind, comp, taa = GBuffers(w, h), GBufferRT(), DirectLighting(w, h), IndirectLighting(w, h), Compositing(w, h), TAA(w, h)
+    manual = DeviceFrame(flat, w, h, WHOLE_FRAME, rpt_params=dict(M_max_temporal=9), presample=presample)
     # renderer on its own scene object (it runs pre-lighting itself in its first frame)
     sc2 = Scene(flat)
     if presample:
         sc2.set_presampling(*presample)
     R = Renderer(sc2, w, h, two_streams=two_streams)
     R.indirect.SetParams(M_max_temporal=9)
-    ind.SetParams(M_max_temporal=9)
     seq = rpt_util.FrameSequence(w, h, cam_path=lambda f: (0.02 * f, 1.2, -4.043))
-    fi = _lib.FrameInputs()
-    fi.scene = sc.handle
     for fr in range(4):
         fc = seq.next()
-        gb.flip(); fi.frame = fc; gb.fill_inputs(fi)
-        g.Render(fi); sc.presample(fc.FrameNum); di.Render(fi); ind.Render(fi)
-        comp.Render(fi, di.GetOutput(0).d_ptr, ind.GetOutput(0).d_ptr)
-        taa.Render(fi, comp.GetOutput().d_ptr)
+        manual.render(fc)
         R.Render(fc)
         check(lib.zr_stream_synchronize(None))
-        a = download_image(taa.GetOutput(), np.uint16, 4)
-        b = download_image(R.GetOutput(), np.uint16, 4)
-        assert np.array_equal(a, b), "frame %d: renderer output differs from the manual pass sequence" % fr
-        assert np.array_equal(download_image(ind.GetOutput(1), np.uint32, 16), download_image(R.indirect.GetOutput(1), np.uint32, 16))
+        assert uint32x2(manual.taa.GetOutput()).tobytes() == uint32x2(R.GetOutput()).tobytes(), \
+            "frame %d: renderer output differs from the manual pass sequence" % fr
+        assert pt_reservoirs(manual.rpt.GetOutput(1)).tobytes() == pt_reservoirs(R.indirect.GetOutput(1)).tobytes()
     assert lib.zr_renderer_render(R.handle, None, None) != 0
-    gb.close()
+    manual.close()

@@ -2,65 +2,15 @@
 48-byte reservoirs and the final image byte for byte. Covers the path-traced initial candidate (MIS NEE at the first
 indirect vertex, light-sampled NEE after it), temporal reuse with one and two candidates, the reconnection Jacobian,
 outlier suppression, the wave-wide Russian roulette (5+ bounces), presampled sets, a translating camera and DoF."""
-import numpy as np
 import pytest
 
-from tests.test_rpt_gpu import _diff_report
+from tests.parity import frame_parity
 
 pytestmark = pytest.mark.gpu
 
 
-def _run(which, w, h, nframes, params=None, cam_path=None, presample=None, dof=False, accumulate=False, lvg=None):
-    from zetaray_b200 import lib, check, _lib
-    from zetaray_b200.passes import Scene, GBuffers, GBufferRT, IndirectLightingGI, download_image
-    from tests import scene_util, rpt_util
-    flat = scene_util.SCENES[which]()
-    R = rpt_util.OracleRenderer(flat, w, h)
-    sc = Scene(flat)
-    sc.prelighting()
-    if presample:
-        R.osc.set_presampling(*presample)
-        sc.set_presampling(*presample)
-    if lvg:
-        R.osc.set_light_voxel_grid(*lvg)
-        sc.set_light_voxel_grid(*lvg)
-    gb, gpass, gi = GBuffers(w, h), GBufferRT(), IndirectLightingGI(w, h)
-    if params:
-        R.gi_params.update(params)
-        gi.SetParams(**params)
-    seq = rpt_util.FrameSequence(w, h, cam_path=cam_path, accumulate=accumulate)
-    problems = []
-    for fr in range(nframes):
-        fc = seq.next()
-        if dof:
-            fc.DoF, fc.FocusDepth, fc.LensRadius = 1, 4.0, 0.02
-        R.gbuffer(fc)
-        R.rgi(fc)
-        gb.flip()
-        fi = _lib.FrameInputs()
-        fi.frame = fc
-        gb.fill_inputs(fi)
-        fi.scene = sc.handle
-        gpass.Render(fi)
-        sc.presample(fc.FrameNum)
-        sc.build_light_voxel_grid(fc)
-        gi.Render(fi)
-        check(lib.zr_stream_synchronize(None))
-        if lvg and fr == 0:
-            n = lvg[0][0] * lvg[0][1] * lvg[0][2] * 64 * 8
-            msg = _diff_report("light voxel grid", sc.light_voxel_grid().reshape(-1, 8), R.osc.lvg[:n].reshape(-1, 8))
-            if msg:
-                problems.append(msg)
-        got_res = download_image(gi.GetOutput(1), np.uint8, 48).view(rpt_util.RGI).reshape(-1)
-        got_final = download_image(gi.GetOutput(0), np.float32, 4)
-        for name, a, b in (("gi reservoir", got_res, R.gi_curr_reservoirs()), ("gi final", got_final.view(np.uint32), R.gi_final.view(np.uint32))):
-            msg = _diff_report(name, a, b)
-            if msg:
-                problems.append("frame %d: %s" % (fc.FrameNum, msg))
-        if problems:
-            break
-    gb.close()
-    return problems, R
+def _run(which, w, h, nframes, **kw):
+    return frame_parity(which, w, h, nframes, ("rgi",), **kw)
 
 
 @pytest.mark.parametrize("which", ["cornell", "glossy", "glass"])
@@ -76,10 +26,10 @@ def test_rgi_moving_camera_and_variants():
     problems, _ = _run("glossy", 320, 180, 5, cam_path=path)
     assert not problems, "\n".join(problems)
     # deterministic bounce count, 6 bounces so the wave-wide Russian roulette runs, no outlier suppression
-    problems, _ = _run("glass", 256, 144, 4, params=dict(stochastic_multi_bounce=0, max_non_tr_bounces=6, max_glossy_tr_bounces=6,
-                                                          boiling_suppression=0), cam_path=path)
+    problems, _ = _run("glass", 256, 144, 4, gi_params=dict(stochastic_multi_bounce=0, max_non_tr_bounces=6, max_glossy_tr_bounces=6,
+                                                             boiling_suppression=0), cam_path=path)
     assert not problems, "\n".join(problems)
-    problems, _ = _run("cornell", 256, 144, 3, params=dict(temporal_resample=0, M_max=4))
+    problems, _ = _run("cornell", 256, 144, 3, gi_params=dict(temporal_resample=0, M_max=4))
     assert not problems, "\n".join(problems)
 
 
@@ -97,7 +47,7 @@ def test_rgi_light_voxel_grid():
     # presampled set as fallback outside it. A small grid so that both branches run; then the reference's own dimensions.
     path = lambda f: (0.03 * f, 1.2, -4.043 + 0.04 * f)
     problems, _ = _run("glossy", 320, 180, 4, presample=(32, 128), lvg=((8, 4, 8), (0.6, 0.45, 0.6), 0.1), cam_path=path,
-                       params=dict(stochastic_multi_bounce=0))
+                       gi_params=dict(stochastic_multi_bounce=0))
     assert not problems, "\n".join(problems)
     problems, _ = _run("glass", 256, 144, 3, presample=(128, 512), lvg=((32, 8, 40), (0.6, 0.45, 0.6), 0.0))
     assert not problems, "\n".join(problems)

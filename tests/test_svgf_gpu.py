@@ -9,16 +9,14 @@ pytestmark = pytest.mark.gpu
 
 def _run(which, w, h, nframes, radius=2, num_passes=5, cam_path=None, synthetic=False):
     import torch
-    from zetaray_b200 import lib, check, _lib
-    from zetaray_b200.passes import Scene, GBuffers, GBufferRT, SVGF, download_image, download_image_pitched
+    from zetaray_b200 import lib, check
+    from zetaray_b200.passes import SVGF, download_image, download_image_pitched
     from tests import scene_util, rpt_util
+    from tests.parity import DeviceFrame
     from tests.svgf_util import OracleSVGF
     flat = scene_util.SCENES[which]()
     R = rpt_util.OracleRenderer(flat, w, h)
-    sc = Scene(flat)
-    sc.prelighting()
-    gb = GBuffers(w, h)
-    gpass = GBufferRT()
+    dev = DeviceFrame(flat, w, h, ())
     svgf = SVGF(w, h)
     svgf.SetParams(radius=radius, num_passes=num_passes)
     osv = OracleSVGF(w, h, radius=radius, num_passes=num_passes)
@@ -38,12 +36,7 @@ def _run(which, w, h, nframes, radius=2, num_passes=5, cam_path=None, synthetic=
             signal = np.ascontiguousarray(signal, dtype=np.float32)
         core, _, me, _ = R.gb[R.cur][:4]
         want, want_acc = osv.render(fc, core, me, signal)
-        gb.flip()
-        fi = _lib.FrameInputs()
-        fi.frame = fc
-        gb.fill_inputs(fi)
-        fi.scene = sc.handle
-        gpass.Render(fi)
+        fi = dev.render(fc)
         d_signal = torch.from_numpy(signal).cuda()
         torch.cuda.synchronize()
         svgf.Render(fi, d_signal.data_ptr())
@@ -61,7 +54,7 @@ def _run(which, w, h, nframes, radius=2, num_passes=5, cam_path=None, synthetic=
                                 (fc.FrameNum, name, len(d), len(a), d[0], d[0] % w, d[0] // w, a[d[0]], b[d[0]]))
         if problems:
             break
-    gb.close()
+    dev.close()
     return problems
 
 

@@ -4,49 +4,13 @@ oracle, frame by frame, byte for byte -- stand-alone through zr_gi_pass_set_meth
 import numpy as np
 import pytest
 
-from tests.test_rpt_gpu import _diff_report
+from tests.parity import diff_report, frame_parity, rgba32f_bits, uint32x2
 
 pytestmark = pytest.mark.gpu
 
 
-def _run(which, w, h, nframes, params=None, cam_path=None, accumulate=False, presample=None):
-    from zetaray_b200 import lib, check, _lib
-    from zetaray_b200.passes import Scene, GBuffers, GBufferRT, IndirectLightingGI, download_image
-    from tests import scene_util, rpt_util
-    flat = scene_util.SCENES[which]()
-    R = rpt_util.OracleRenderer(flat, w, h)
-    sc = Scene(flat)
-    sc.prelighting()
-    if presample:
-        R.osc.set_presampling(*presample)
-        sc.set_presampling(*presample)
-    gb, gpass, pt = GBuffers(w, h), GBufferRT(), IndirectLightingGI(w, h)
-    pt.SetMethod(IndirectLightingGI.PATH_TRACING)
-    if params:
-        R.gi_params.update(params)
-        pt.SetParams(**params)
-    cam = scene_util.CAMERAS.get(which)
-    seq = rpt_util.FrameSequence(w, h, cam_path=cam_path or ((lambda f: cam) if cam else None), accumulate=accumulate)
-    problems = []
-    for fr in range(nframes):
-        fc = seq.next()
-        R.gbuffer(fc)
-        R.pt(fc)
-        gb.flip()
-        fi = _lib.FrameInputs()
-        fi.frame = fc
-        gb.fill_inputs(fi)
-        fi.scene = sc.handle
-        gpass.Render(fi)
-        sc.presample(fc.FrameNum)
-        pt.Render(fi)
-        check(lib.zr_stream_synchronize(None))
-        msg = _diff_report("path tracer final", download_image(pt.GetOutput(0), np.float32, 4).view(np.uint32), R.gi_final.view(np.uint32))
-        if msg:
-            problems.append("frame %d: %s" % (fc.FrameNum, msg))
-            break
-    gb.close()
-    return problems, R
+def _run(which, w, h, nframes, **kw):
+    return frame_parity(which, w, h, nframes, ("pt",), **kw)
 
 
 @pytest.mark.parametrize("which", ["cornell", "glossy", "glass"])
@@ -60,7 +24,7 @@ def test_path_tracer_variants():
     # translating camera, 6 bounces (the wave-wide Russian roulette runs), transmissive scene (Beer's law, exact shadow rays
     # through glass), accumulation mode, presampled sets
     path = lambda f: (0.03 * f, 1.2 + 0.01 * f, -4.043 + 0.04 * f)
-    problems, _ = _run("glass", 256, 144, 3, params=dict(max_non_tr_bounces=6, max_glossy_tr_bounces=6), cam_path=path)
+    problems, _ = _run("glass", 256, 144, 3, gi_params=dict(max_non_tr_bounces=6, max_glossy_tr_bounces=6), cam_path=path)
     assert not problems, "\n".join(problems)
     problems, _ = _run("glossy", 256, 144, 3, accumulate=True, presample=(16, 64))
     assert not problems, "\n".join(problems)
@@ -70,7 +34,7 @@ def test_path_tracer_variants():
 
 def test_path_tracer_through_the_renderer_and_method_switch():
     from zetaray_b200 import lib, check
-    from zetaray_b200.passes import Scene, Renderer, download_image
+    from zetaray_b200.passes import Scene, Renderer
     from tests import scene_util, rpt_util
     w, h = 192, 108
     flat = scene_util.glossy_cornell()
@@ -87,9 +51,9 @@ def test_path_tracer_through_the_renderer_and_method_switch():
         _, taa_prev = R.post(fc, taa_prev, fr > 0)
         rd.Render(fc)
         check(lib.zr_stream_synchronize(None))
-        msg = _diff_report("pt final", download_image(rd.gi.GetOutput(0), np.float32, 4).view(np.uint32), R.gi_final.view(np.uint32))
+        msg = diff_report("pt final", rgba32f_bits(rd.gi.GetOutput(0)), R.gi_final.view(np.uint32))
         assert not msg, "frame %d: %s" % (fr + 1, msg)
-        msg = _diff_report("taa", download_image(rd.GetOutput(), np.uint32, 2), taa_prev)
+        msg = diff_report("taa", uint32x2(rd.GetOutput()), taa_prev)
         assert not msg, "frame %d: %s" % (fr + 1, msg)
     # switching to ReSTIR GI drops the history: its first frame equals the oracle's first GI frame on this G-buffer sequence
     rd.SetMethod(Renderer.RESTIR_GI)
@@ -97,6 +61,6 @@ def test_path_tracer_through_the_renderer_and_method_switch():
     R.gbuffer(fc); R.rdi(fc); R.rgi(fc)
     rd.Render(fc)
     check(lib.zr_stream_synchronize(None))
-    msg = _diff_report("gi final after the switch", download_image(rd.gi.GetOutput(0), np.float32, 4).view(np.uint32), R.gi_final.view(np.uint32))
+    msg = diff_report("gi final after the switch", rgba32f_bits(rd.gi.GetOutput(0)), R.gi_final.view(np.uint32))
     assert not msg, msg
     assert lib.zr_gi_pass_set_method(rd.gi.handle, 2) != 0      # ReSTIR PT is a different pass object

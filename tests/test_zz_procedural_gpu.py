@@ -11,7 +11,7 @@ import os
 import numpy as np
 import pytest
 
-from tests.test_rpt_gpu import _diff_report
+from tests.parity import GBUFFER_CHECKS, WHOLE_FRAME, diff_report, frame_parity, gi_reservoirs, rgba32f_bits, uint32x2
 
 pytestmark = pytest.mark.gpu
 NTHREADS = min(os.cpu_count() or 8, 64)
@@ -27,57 +27,10 @@ def _setup(which, w, h):
     return flat, R, sc, cam
 
 
-def _frames(which, w, h, nframes, rpt_params=None, cam_path=None, with_di=True):
+def _frames(which, w, h, nframes, **kw):
     """Whole frame, pass by pass: G-buffer, ReSTIR DI, ReSTIR PT, compositing + firefly, TAA."""
-    from zetaray_b200 import lib, check, _lib
-    from zetaray_b200.passes import GBuffers, GBufferRT, DirectLighting, IndirectLighting, Compositing, TAA, download_image
-    from tests import rpt_util
-    flat, R, sc, cam = _setup(which, w, h)
-    sc.prelighting()
-    gb, gpass, di, ind, comp, taa = GBuffers(w, h), GBufferRT(), DirectLighting(w, h), IndirectLighting(w, h), Compositing(w, h), TAA(w, h)
-    if rpt_params:
-        for k, v in rpt_params.items():
-            setattr(R.params, k, v)
-        ind.SetParams(**rpt_params)
-    seq = rpt_util.FrameSequence(w, h, cam_path=cam_path or (lambda f: cam))
-    taa_prev = np.zeros((w * h, 2), dtype=np.uint32)
-    problems = []
-    for fr in range(nframes):
-        fc = seq.next()
-        core, depth, me, coat, _ = R.gbuffer(fc)
-        R.rdi(fc)
-        R.rpt(fc)
-        gb.flip()
-        fi = _lib.FrameInputs()
-        fi.frame = fc
-        gb.fill_inputs(fi)
-        fi.scene = sc.handle
-        gpass.Render(fi)
-        di.Render(fi)
-        ind.Render(fi)
-        comp.Render(fi, di.GetOutput(0).d_ptr, ind.GetOutput(0).d_ptr)
-        taa.Render(fi, comp.GetOutput().d_ptr)
-        check(lib.zr_stream_synchronize(None))
-        ref_comp, ref_taa = R.post(fc, taa_prev, fr > 0)
-        taa_prev = ref_taa
-        g_core, g_depth, g_me, g_coat, _ = gb.download("curr")
-        checks = [("gbuffer core", g_core, core), ("gbuffer depth", g_depth.view(np.uint32), depth.view(np.uint32)),
-                  ("gbuffer motion/emissive", g_me, me), ("gbuffer coat", g_coat, coat),
-                  ("di_reservoir", download_image(di.GetOutput(1), np.uint8, 32).view(rpt_util.RDI).reshape(-1), R.di_curr_reservoirs()),
-                  ("di_final", download_image(di.GetOutput(0), np.float32, 4).view(np.uint32), R.di_final.view(np.uint32)),
-                  ("pt_reservoir", download_image(ind.GetOutput(1), np.uint8, 64).view(rpt_util.RES).reshape(-1), R.curr_reservoirs()),
-                  ("pt_final", download_image(ind.GetOutput(0), np.float32, 4).view(np.uint32), R.final.view(np.uint32)),
-                  ("composited", download_image(comp.GetOutput(), np.float32, 4).view(np.uint32), ref_comp.view(np.uint32)),
-                  ("taa", download_image(taa.GetOutput(), np.uint32, 2), ref_taa)]
-        for name, a, b in checks:
-            msg = _diff_report(name, np.ascontiguousarray(a).reshape(len(b), -1) if a.dtype.fields is None else a,
-                               np.ascontiguousarray(b).reshape(len(b), -1) if b.dtype.fields is None else b)
-            if msg:
-                problems.append("frame %d: %s" % (fc.FrameNum, msg))
-        if problems:
-            break
-    gb.close()
-    return problems, R
+    checks = GBUFFER_CHECKS + ("di_reservoir", "di_final", "pt_reservoir", "pt_final", "composited", "taa")
+    return frame_parity(which, w, h, nframes, WHOLE_FRAME, checks, nthreads=NTHREADS, **kw)
 
 
 def test_atrium_whole_frame():
@@ -105,7 +58,7 @@ def test_atrium_many_lights_gi_lvg_through_the_renderer():
     integrator is ReSTIR GI (LVG NEE variant), DirectLighting reads the presampled sets. Compared with the oracle running
     the same configuration pass by pass."""
     from zetaray_b200 import lib, check
-    from zetaray_b200.passes import Renderer, download_image
+    from zetaray_b200.passes import Renderer
     from tests import rpt_util
     w, h = 128, 72
     flat, R, sc, cam = _setup("atrium_lights", w, h)
@@ -131,14 +84,14 @@ def test_atrium_many_lights_gi_lvg_through_the_renderer():
         if fr == 0:
             assert sc.sample_sets().tobytes() == R.osc.sample_sets[:128 * 512 * 10].tobytes(), "presampled sets differ"
             n = 32 * 8 * 40 * 64 * 8
-            msg = _diff_report("light voxel grid", sc.light_voxel_grid().reshape(-1, 8), R.osc.lvg[:n].reshape(-1, 8))
+            msg = diff_report("light voxel grid", sc.light_voxel_grid().reshape(-1, 8), R.osc.lvg[:n].reshape(-1, 8))
             assert not msg, msg
-        checks = [("gi reservoir", download_image(rd.gi.GetOutput(1), np.uint8, 48).view(rpt_util.RGI).reshape(-1), R.gi_curr_reservoirs()),
-                  ("gi final", download_image(rd.gi.GetOutput(0), np.float32, 4).view(np.uint32), R.gi_final.view(np.uint32)),
-                  ("di_final", download_image(rd.direct.GetOutput(0), np.float32, 4).view(np.uint32), R.di_final.view(np.uint32)),
-                  ("taa", download_image(rd.GetOutput(), np.uint32, 2), ref_taa)]
+        checks = [("gi reservoir", gi_reservoirs(rd.gi.GetOutput(1)), R.gi_curr_reservoirs()),
+                  ("gi final", rgba32f_bits(rd.gi.GetOutput(0)), R.gi_final.view(np.uint32)),
+                  ("di_final", rgba32f_bits(rd.direct.GetOutput(0)), R.di_final.view(np.uint32)),
+                  ("taa", uint32x2(rd.GetOutput()), ref_taa)]
         for name, a, b in checks:
-            msg = _diff_report(name, a, b)
+            msg = diff_report(name, a, b)
             if msg:
                 problems.append("frame %d: %s" % (fc.FrameNum, msg))
         if problems:
