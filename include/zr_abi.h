@@ -50,7 +50,8 @@ ZR_API const char* zr_last_error(void);
  * zr_renderer_get_gi_pass, zr_renderer_apply_scene_settings and zr_gi_pass_set_method; 1.2 the SVGF pass, zr_comm, the strip-sharded
  * renderer (zr_renderer_set_shard) and zr_gi_pass_set_rows / set_halo_exchange. 1.3 removed two
  * measurement and test hooks: the ReSTIR PT execution-model switch and the two-dispatch compositing entry point. 1.4 removed
- * the stage-limited ReSTIR PT render and its stage enum, which nothing called. */
+ * the stage-limited ReSTIR PT render and its stage enum, which nothing called. 1.6 added the AutoExposure and Display passes,
+ * zr_renderer_set_display / get_display_output and zr_comm_allreduce_u32. */
 ZR_API uint32_t zr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -595,6 +596,65 @@ ZR_API zr_status zr_taa_pass_render(zr_taa_pass* p, const zr_frame_inputs* in, c
 ZR_API zr_status zr_taa_pass_get_output(zr_taa_pass* p, zr_image2d* out);
 ZR_API void zr_taa_pass_destroy(zr_taa_pass* p);
 
+/* ---- AutoExposure (AutoExposure/AutoExposure.h, AutoExposure.cpp:100-140) ----
+ * A 256-bin luminance histogram of the signal TAA reads (k_lum_histogram, rows set by set_rows), then one block turns it into
+ * a temporally adapted exposure (k_exposure): output {exposure, adapted luminance} as one float2, {0, 0} after create / resize /
+ * reset (the reference's INIT_TO_ZERO texture). Adaptation reads the frame's dt in seconds: render rejects a non-finite or
+ * negative dt, and dt == 0 on the first frame after create / resize / reset (the exposure would be infinite); later frames with
+ * dt == 0 keep the adapted luminance. */
+typedef struct zr_auto_exposure_pass zr_auto_exposure_pass;
+typedef struct zr_auto_exposure_params
+{
+    float min_lum;          /* 5e-3, AutoExposure.h:73-80; >= 0 */
+    float max_lum;          /* 4; > min_lum */
+    float lum_map_exp;      /* 0.5; > 0 */
+    float adaptation_rate;  /* 1 */
+} zr_auto_exposure_params;
+/* Called between the histogram and the exposure kernel on the 256 device bins: it must leave there the sum of every rank's bins
+ * (strip-sharded frames: every rank then derives the same exposure). The renderer's hook is zr_comm_allreduce_u32. */
+typedef void (*zr_reduce_u32_fn)(void* user, uint32_t* d_values, uint32_t n, void* stream);
+ZR_API zr_status zr_auto_exposure_pass_create(uint32_t width, uint32_t height, zr_auto_exposure_pass** out);
+ZR_API zr_status zr_auto_exposure_pass_resize(zr_auto_exposure_pass* p, uint32_t width, uint32_t height);
+ZR_API zr_status zr_auto_exposure_pass_reset_temporal(zr_auto_exposure_pass* p);
+ZR_API zr_status zr_auto_exposure_pass_default_params(zr_auto_exposure_params* out);
+ZR_API zr_status zr_auto_exposure_pass_set_params(zr_auto_exposure_pass* p, const zr_auto_exposure_params* params);
+/* d_signal: float4[w*h], the image TAA reads (Compositing or SVGF output) */
+ZR_API zr_status zr_auto_exposure_pass_render(zr_auto_exposure_pass* p, const zr_frame_inputs* in, const void* d_signal, void* stream);
+ZR_API zr_status zr_auto_exposure_pass_set_rows(zr_auto_exposure_pass* p, uint32_t y0, uint32_t y1);
+ZR_API zr_status zr_auto_exposure_pass_set_reduce(zr_auto_exposure_pass* p, zr_reduce_u32_fn fn, void* user);   /* fn NULL: none */
+ZR_API zr_status zr_auto_exposure_pass_get_output(zr_auto_exposure_pass* p, zr_image2d* out);     /* 1 x 1 float2 */
+ZR_API void zr_auto_exposure_pass_destroy(zr_auto_exposure_pass* p);
+
+/* ---- Display (Display/Display.h, Display.hlsl default view, Tonemap.hlsli) ----
+ * TAA output x exposure -> tone mapper -> saturate -> sRGB OETF -> RGBA8 (alpha 255), the reference's R8G8B8A8_UNORM_SRGB back
+ * buffer. Render size must equal display size. NEUTRAL is Tony McMapface: the caller supplies its 48^3 LUT in the packed
+ * R9G9B9E5_SHAREDEXP form (x fastest, as tony_mc_mapface.dds stores it) with set_lut; rendering NEUTRAL without it is
+ * ZR_ERR_INVALID_ARG. */
+typedef enum zr_tonemapper
+{
+    ZR_TONEMAPPER_NONE = 0, ZR_TONEMAPPER_NEUTRAL = 1, ZR_TONEMAPPER_AGX_DEFAULT = 2, ZR_TONEMAPPER_AGX_GOLDEN = 3,
+    ZR_TONEMAPPER_AGX_PUNCHY = 4, ZR_TONEMAPPER_AGX_CUSTOM = 5
+} zr_tonemapper;
+typedef struct zr_display_params
+{
+    uint32_t tonemapper;    /* zr_tonemapper, default NEUTRAL (Display.cpp:70-74) */
+    uint32_t auto_exposure; /* 1: multiply by the exposure first */
+    float saturation;       /* 1: NEUTRAL's desaturation lerp and AGX_CUSTOM */
+    float agx_exp;          /* 1: AGX_CUSTOM's exponent */
+} zr_display_params;
+typedef struct zr_display_pass zr_display_pass;
+ZR_API zr_status zr_display_pass_create(uint32_t width, uint32_t height, zr_display_pass** out);
+ZR_API zr_status zr_display_pass_resize(zr_display_pass* p, uint32_t width, uint32_t height);
+ZR_API zr_status zr_display_pass_default_params(zr_display_params* out);
+ZR_API zr_status zr_display_pass_set_params(zr_display_pass* p, const zr_display_params* params);
+ZR_API zr_status zr_display_pass_set_lut(zr_display_pass* p, const uint32_t* h_rgb9e5, uint32_t dim);     /* dim must be 48 */
+/* d_signal: the TAA output (half4[w*h]); d_exposure: the auto-exposure output (float2), may be NULL with auto_exposure off */
+ZR_API zr_status zr_display_pass_render(zr_display_pass* p, const zr_frame_inputs* in, const void* d_signal, const void* d_exposure,
+    void* stream);
+ZR_API zr_status zr_display_pass_set_rows(zr_display_pass* p, uint32_t y0, uint32_t y1);
+ZR_API zr_status zr_display_pass_get_output(zr_display_pass* p, zr_image2d* out);      /* RGBA8, 4 B/px */
+ZR_API void zr_display_pass_destroy(zr_display_pass* p);
+
 /* ---- host <-> device helpers so callers need no CUDA runtime of their own ---- */
 ZR_API zr_status zr_device_malloc(void** d_ptr, size_t bytes);
 ZR_API void zr_device_free(void* d_ptr);
@@ -625,6 +685,8 @@ ZR_API zr_status zr_comm_stats(zr_comm* c, uint64_t* bytes_sent, uint64_t* calls
 ZR_API zr_status zr_comm_exchange_halos(zr_comm* c, int which_comm, const uint32_t* bounds, uint32_t halo_rows, const zr_image2d* planes,
     int n_planes, void* stream);
 ZR_API zr_status zr_comm_gather_rows(zr_comm* c, const uint32_t* bounds, const zr_image2d* plane, int root, void* stream);
+/* In-place sum of n uint32 values over every rank (one ncclAllReduce on which_comm) */
+ZR_API zr_status zr_comm_allreduce_u32(zr_comm* c, int which_comm, uint32_t* d_values, uint32_t n, void* stream);
 
 /* ---- The frame (ZetaRenderer/Default: DefaultRenderer.cpp:304-520, PathTracer.cpp:149-563) ----
  * Owns the double-buffered G-buffers and one object of every pass and runs a frame in the reference's order:
@@ -644,6 +706,12 @@ ZR_API zr_status zr_renderer_set_denoiser(zr_renderer* r, int enable, zr_svgf_pa
  * warm-up frames unsharded on every rank. */
 ZR_API zr_status zr_renderer_set_shard(zr_renderer* r, zr_comm* comm, const uint32_t* bounds, int gather_output);
 ZR_API zr_status zr_renderer_get_output(zr_renderer* r, zr_image2d* out);      /* TAA output, RGBA16F */
+/* Optional post-processing (ZetaRenderer/Default/PostProcessor.cpp): enable != 0 creates an AutoExposure pass that reads the TAA
+ * input and a Display pass on the TAA output (their defaults; NEUTRAL needs zr_display_pass_set_lut on *out_display before the
+ * next frame); 0 removes both. Sharded frames histogram each strip and all-reduce the bins on the main communicator, and
+ * gather the display image on rank 0 along with the TAA image. out_ae / out_display may be NULL. */
+ZR_API zr_status zr_renderer_set_display(zr_renderer* r, int enable, zr_auto_exposure_pass** out_ae, zr_display_pass** out_display);
+ZR_API zr_status zr_renderer_get_display_output(zr_renderer* r, zr_image2d* out);      /* RGBA8; ZR_ERR_NOT_INITIALIZED when disabled */
 ZR_API zr_status zr_renderer_get_passes(zr_renderer* r, zr_gbuffer_pass** gbuffer, zr_direct_pass** direct,
     zr_indirect_pass** indirect, zr_compositing_pass** compositing, zr_taa_pass** taa);
 ZR_API zr_status zr_renderer_get_gbuffer(zr_renderer* r, int previous, zr_gbuffer* out);

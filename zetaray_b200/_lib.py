@@ -103,6 +103,14 @@ class CompositingParams(C.Structure):
     _fields_ = [("emissive_di", u32), ("indirect", u32), ("firefly_filter", u32)]
 
 
+class AutoExposureParams(C.Structure):
+    _fields_ = [("min_lum", f32), ("max_lum", f32), ("lum_map_exp", f32), ("adaptation_rate", f32)]
+
+
+class DisplayParams(C.Structure):
+    _fields_ = [("tonemapper", u32), ("auto_exposure", u32), ("saturation", f32), ("agx_exp", f32)]
+
+
 lib.zr_last_error.restype = C.c_char_p
 lib.zr_abi_version.restype = u32
 lib.zr_kernel_launch_count.restype = u64
@@ -118,6 +126,8 @@ class RendererDesc(C.Structure):
 
 # zr_halo_exchange_fn (include/zr_abi.h "Strip-sharded frames")
 HALO_EXCHANGE_FN = C.CFUNCTYPE(None, C.c_void_p, C.POINTER(Image2D), C.c_int, C.c_void_p)
+# zr_reduce_u32_fn (include/zr_abi.h "AutoExposure")
+REDUCE_U32_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p)
 
 # every other entry point returns zr_status (int32)
 EXPORTS = [

@@ -12,7 +12,8 @@ namespace
 {
     struct NcclUniqueId { char internal[128]; };
     typedef void* NcclComm;
-    enum { NCCL_UINT8 = 1 };       // ncclUint8 (nccl.h: ncclInt8 = 0, ncclUint8 = 1)
+    enum { NCCL_UINT8 = 1, NCCL_UINT32 = 3 };      // nccl.h: ncclInt8 = 0, ncclUint8 = 1, ncclInt32 = 2, ncclUint32 = 3
+    enum { NCCL_SUM = 0 };
 
     struct NcclApi
     {
@@ -23,6 +24,7 @@ namespace
         int (*Recv)(void*, size_t, int, int, NcclComm, cudaStream_t) = nullptr;
         int (*GroupStart)() = nullptr;
         int (*GroupEnd)() = nullptr;
+        int (*AllReduce)(const void*, void*, size_t, int, int, NcclComm, cudaStream_t) = nullptr;
         const char* (*GetErrorString)(int) = nullptr;
         bool ok = false;
     };
@@ -39,9 +41,10 @@ namespace
 #define ZR_SYM(field, name) api.field = (decltype(api.field))dlsym(h, name)
         ZR_SYM(GetUniqueId, "ncclGetUniqueId"); ZR_SYM(CommInitRank, "ncclCommInitRank"); ZR_SYM(CommDestroy, "ncclCommDestroy");
         ZR_SYM(Send, "ncclSend"); ZR_SYM(Recv, "ncclRecv"); ZR_SYM(GroupStart, "ncclGroupStart"); ZR_SYM(GroupEnd, "ncclGroupEnd");
+        ZR_SYM(AllReduce, "ncclAllReduce");
         ZR_SYM(GetErrorString, "ncclGetErrorString");
 #undef ZR_SYM
-        api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.Send && api.Recv && api.GroupStart && api.GroupEnd;
+        api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.Send && api.Recv && api.GroupStart && api.GroupEnd && api.AllReduce;
         return api;
     }
 
@@ -183,6 +186,14 @@ extern "C"
             c->bytesSent += (size_t)(bounds[c->rank + 1] - bounds[c->rank]) * pitch;
         }
         ZR_NCCL(a.GroupEnd());
+        return ZR_OK;
+    }
+
+    zr_status zr_comm_allreduce_u32(zr_comm* c, int which_comm, uint32_t* d_values, uint32_t n, void* stream)
+    {
+        if (!c || !d_values || which_comm < 0 || which_comm > 1) return ZR_ERR_INVALID_ARG;
+        if (c->world == 1) return ZR_OK;
+        ZR_NCCL(Api().AllReduce(d_values, d_values, n, NCCL_UINT32, NCCL_SUM, c->comm[which_comm], (cudaStream_t)stream));
         return ZR_OK;
     }
 }

@@ -10,6 +10,7 @@
 //                     GBufferRT
 //                     DirectLighting  ||  IndirectLighting      second stream, joined before Compositing
 //                     Compositing (+ firefly filter) -> [SVGF denoise, zr_renderer_set_denoiser] -> TAA
+//                     with zr_renderer_set_display: AutoExposure on the TAA input before TAA, Display on its output after it
 //
 // The renderer owns the double-buffered G-buffers (DefaultRendererImpl.h:111-121) and the pass objects; callers reach
 // the passes through zr_renderer_get_*_pass to set parameters, exactly like the reference's UI callbacks do.
@@ -33,6 +34,8 @@ struct zr_renderer
     zr_compositing_pass* compositing = nullptr;
     zr_taa_pass* taa = nullptr;
     zr_svgf_pass* svgf = nullptr;                   // optional denoise stage between Compositing and TAA (BASELINE config 3)
+    zr_auto_exposure_pass* ae = nullptr;            // optional post-processing (PostProcessor.cpp): both or neither
+    zr_display_pass* display = nullptr;
     cudaStream_t side = nullptr;            // DirectLighting runs here when twoStreams
     cudaEvent_t evGBuffer = nullptr, evDirect = nullptr;
     bool twoStreams = true;
@@ -53,6 +56,13 @@ struct zr_renderer
         const zr_status s = zr_comm_exchange_halos(r->comm, which, r->bounds.data(), HALO, planes, n, stream);
         if (s != ZR_OK) r->hookStatus = s;
     }
+    // AutoExposure's bins: every rank's strip histogram summed in place, so every rank derives the same exposure
+    static void ReduceHook(void* user, uint32_t* d_values, uint32_t n, void* stream)
+    {
+        zr_renderer* r = (zr_renderer*)user;
+        const zr_status s = zr_comm_allreduce_u32(r->comm, 0, d_values, n, stream);
+        if (s != ZR_OK) r->hookStatus = s;
+    }
 
     // the GI pass object is created lazily (first SetMethod): it follows the renderer's current strip
     zr_status ApplyShardToGI()
@@ -62,6 +72,23 @@ struct zr_renderer
         zr_status s = sharded ? zr_gi_pass_set_rows(gi, bounds[rank], bounds[rank + 1]) : zr_gi_pass_set_rows(gi, 0, height);
         if (s == ZR_OK) s = zr_gi_pass_set_halo_exchange(gi, sharded ? HaloHook : nullptr, &hookMain);
         return s;
+    }
+
+    zr_status ApplyShardToDisplay()
+    {
+        if (!ae) return ZR_OK;
+        const bool sharded = comm && world > 1;
+        const uint32_t y0 = sharded ? bounds[rank] : 0, y1 = sharded ? bounds[rank + 1] : height;
+        zr_status s = zr_auto_exposure_pass_set_rows(ae, y0, y1);
+        if (s == ZR_OK) s = zr_auto_exposure_pass_set_reduce(ae, sharded ? ReduceHook : nullptr, this);
+        if (s == ZR_OK) s = zr_display_pass_set_rows(display, y0, y1);
+        return s;
+    }
+    void ReleaseDisplay()
+    {
+        if (ae) zr_auto_exposure_pass_destroy(ae);
+        if (display) zr_display_pass_destroy(display);
+        ae = nullptr; display = nullptr;
     }
 
     void Release()
@@ -75,6 +102,7 @@ struct zr_renderer
         if (taa) zr_taa_pass_destroy(taa);
         if (svgf) zr_svgf_pass_destroy(svgf);
         svgf = nullptr;
+        ReleaseDisplay();
         gbufferPass = nullptr; direct = nullptr; indirect = nullptr; compositing = nullptr; taa = nullptr;
         for (int i = 0; i < 2; i++) zr_gbuffer_free(&gbuffer[i]);
         if (side) cudaStreamDestroy(side);
@@ -191,14 +219,33 @@ extern "C"
             s = zr_svgf_pass_get_output(r->svgf, ZR_SVGF_DENOISED, &comp);
             if (s != ZR_OK) return s;
         }
+        zr_image2d exposure{};
+        if (r->ae)
+        {
+            s = zr_auto_exposure_pass_render(r->ae, &in, comp.d_ptr, stream);
+            if (s != ZR_OK) return s;
+            if (r->hookStatus != ZR_OK) { s = r->hookStatus; r->hookStatus = ZR_OK; return s; }
+            s = zr_auto_exposure_pass_get_output(r->ae, &exposure);
+            if (s != ZR_OK) return s;
+        }
         s = zr_taa_pass_render(r->taa, &in, comp.d_ptr, stream);
         if (s != ZR_OK) return s;
+        zr_image2d img;
+        s = zr_taa_pass_get_output(r->taa, &img);
+        if (s != ZR_OK) return s;
+        zr_image2d shown{};
+        if (r->display)
+        {
+            s = zr_display_pass_render(r->display, &in, img.d_ptr, exposure.d_ptr, stream);
+            if (s != ZR_OK) return s;
+            s = zr_display_pass_get_output(r->display, &shown);
+            if (s != ZR_OK) return s;
+        }
         if (r->comm && r->world > 1 && r->gatherOutput)
         {
-            zr_image2d img;
-            s = zr_taa_pass_get_output(r->taa, &img);
-            if (s != ZR_OK) return s;
             s = zr_comm_gather_rows(r->comm, r->bounds.data(), &img, 0, stream);
+            if (s != ZR_OK) return s;
+            if (r->display) s = zr_comm_gather_rows(r->comm, r->bounds.data(), &shown, 0, stream);
             if (s != ZR_OK) return s;
         }
         r->framesRendered++;
@@ -241,6 +288,29 @@ extern "C"
         if (out_pass) *out_pass = r->svgf;
         return s;
     }
+    // AutoExposure + Display after TAA (enable != 0 creates both with their defaults; 0 removes both and the exposure history)
+    zr_status zr_renderer_set_display(zr_renderer* r, int enable, zr_auto_exposure_pass** out_ae, zr_display_pass** out_display)
+    {
+        if (!r) return ZR_ERR_INVALID_ARG;
+        zr_status s = ZR_OK;
+        if (enable && !r->ae)
+        {
+            s = zr_auto_exposure_pass_create(r->width, r->height, &r->ae);
+            if (s == ZR_OK) s = zr_display_pass_create(r->width, r->height, &r->display);
+            if (s == ZR_OK) s = r->ApplyShardToDisplay();
+            if (s != ZR_OK) r->ReleaseDisplay();
+        }
+        if (!enable) r->ReleaseDisplay();
+        if (out_ae) *out_ae = r->ae;
+        if (out_display) *out_display = r->display;
+        return s;
+    }
+    zr_status zr_renderer_get_display_output(zr_renderer* r, zr_image2d* out)
+    {
+        if (!r || !out) return ZR_ERR_INVALID_ARG;
+        if (!r->display) { zr::set_error("zr_renderer_get_display_output: the display stage is off (zr_renderer_set_display)"); return ZR_ERR_NOT_INITIALIZED; }
+        return zr_display_pass_get_output(r->display, out);
+    }
     zr_status zr_renderer_set_shard(zr_renderer* r, zr_comm* comm, const uint32_t* bounds, int gather_output)
     {
         if (!r) return ZR_ERR_INVALID_ARG;
@@ -256,6 +326,7 @@ extern "C"
             if (s == ZR_OK) s = zr_direct_pass_set_halo_exchange(r->direct, nullptr, nullptr);
             if (s == ZR_OK) s = zr_indirect_pass_set_halo_exchange(r->indirect, nullptr, nullptr);
             if (s == ZR_OK) s = r->ApplyShardToGI();
+            if (s == ZR_OK) s = r->ApplyShardToDisplay();
             return s;
         }
         if (!bounds) { zr::set_error("zr_renderer_set_shard: bounds missing"); return ZR_ERR_INVALID_ARG; }
@@ -287,6 +358,7 @@ extern "C"
         if (s == ZR_OK) s = zr_direct_pass_set_halo_exchange(r->direct, world > 1 ? zr_renderer::HaloHook : nullptr, &r->hookSide);
         if (s == ZR_OK) s = zr_indirect_pass_set_halo_exchange(r->indirect, world > 1 ? zr_renderer::HaloHook : nullptr, &r->hookMain);
         if (s == ZR_OK) s = r->ApplyShardToGI();
+        if (s == ZR_OK) s = r->ApplyShardToDisplay();
         return s;
     }
     zr_status zr_renderer_get_gi_pass(zr_renderer* r, zr_gi_pass** gi)

@@ -1,7 +1,7 @@
 """Host-side mirrors of the reference's pass objects over the C-ABI (thin; no compute here).
 
 Names follow ZetaRenderPass: GBufferRT, PreLighting, DirectLighting, IndirectLighting, Compositing,
-TAA -- each with the reference's verbs (Init in the constructor, OnWindowResized, Render, GetOutput)."""
+TAA, AutoExposure, Display -- each with the reference's verbs (Init in the constructor, OnWindowResized, Render, GetOutput)."""
 import ctypes as C
 import numpy as np
 
@@ -380,6 +380,85 @@ class SVGF(_Pass):
         return img
 
 
+class AutoExposure(_Pass):
+    """AutoExposure (zr_auto_exposure_pass, csrc/display.cu): luminance histogram of the TAA input -> adapted exposure.
+    GetOutput() is the 1 x 1 float2 {exposure, adapted luminance}; Render reads the frame's dt (seconds)."""
+    prefix = "zr_auto_exposure_pass"
+
+    def __init__(self, w, h):
+        self.handle = C.c_void_p()
+        check(lib.zr_auto_exposure_pass_create(w, h, C.byref(self.handle)))
+        self.params = _lib.AutoExposureParams()
+        check(lib.zr_auto_exposure_pass_default_params(C.byref(self.params)))
+
+    def SetParams(self, **kw):
+        p = _lib.AutoExposureParams.from_buffer_copy(self.params)
+        for k, v in kw.items():
+            setattr(p, k, v)
+        check(lib.zr_auto_exposure_pass_set_params(self.handle, C.byref(p)))
+        self.params = p
+
+    def OnWindowResized(self, w, h):
+        check(lib.zr_auto_exposure_pass_resize(self.handle, w, h))
+
+    def ResetTemporal(self):
+        check(lib.zr_auto_exposure_pass_reset_temporal(self.handle))
+
+    def SetRows(self, y0, y1):
+        check(lib.zr_auto_exposure_pass_set_rows(self.handle, y0, y1))
+
+    def SetReduce(self, fn):
+        """fn: a _lib.REDUCE_U32_FN instance (kept alive here) or None."""
+        self._reduce_fn = fn
+        check(lib.zr_auto_exposure_pass_set_reduce(self.handle, fn if fn is not None else _lib.REDUCE_U32_FN(), None))
+
+    def Render(self, fi, d_signal, stream=None):
+        check(lib.zr_auto_exposure_pass_render(self.handle, C.byref(fi), C.c_void_p(d_signal), stream))
+
+    def GetOutput(self):
+        img = _lib.Image2D()
+        check(lib.zr_auto_exposure_pass_get_output(self.handle, C.byref(img)))
+        return img
+
+
+class Display(_Pass):
+    """Display (zr_display_pass, csrc/display.cu): TAA output x exposure -> tone mapper -> sRGB RGBA8."""
+    prefix = "zr_display_pass"
+    NONE, NEUTRAL, AGX_DEFAULT, AGX_GOLDEN, AGX_PUNCHY, AGX_CUSTOM = range(6)
+
+    def __init__(self, w, h):
+        self.handle = C.c_void_p()
+        check(lib.zr_display_pass_create(w, h, C.byref(self.handle)))
+        self.params = _lib.DisplayParams()
+        check(lib.zr_display_pass_default_params(C.byref(self.params)))
+
+    def SetParams(self, **kw):
+        p = _lib.DisplayParams.from_buffer_copy(self.params)
+        for k, v in kw.items():
+            setattr(p, k, v)
+        check(lib.zr_display_pass_set_params(self.handle, C.byref(p)))
+        self.params = p
+
+    def SetLUT(self, lut):
+        """lut: the Tony McMapface LUT as packed R9G9B9E5 texels, uint32[48][48][48] (x fastest)."""
+        a = np.ascontiguousarray(lut, dtype=np.uint32)
+        check(lib.zr_display_pass_set_lut(self.handle, _vp(a), C.c_uint32(a.shape[0] if a.ndim == 3 else 0)))
+
+    def OnWindowResized(self, w, h):
+        check(lib.zr_display_pass_resize(self.handle, w, h))
+
+    def SetRows(self, y0, y1):
+        check(lib.zr_display_pass_set_rows(self.handle, y0, y1))
+
+    def Render(self, fi, d_signal, d_exposure, stream=None):
+        check(lib.zr_display_pass_render(self.handle, C.byref(fi), C.c_void_p(d_signal), C.c_void_p(d_exposure), stream))
+
+    def GetOutput(self):
+        img = _lib.Image2D()
+        check(lib.zr_display_pass_get_output(self.handle, C.byref(img)))
+        return img
+
+
 class _Borrowed:
     """A pass handle owned by a Renderer: same verbs as the owning classes, never destroyed from here."""
 
@@ -395,6 +474,12 @@ class _Borrowed:
         if cls is SVGF:
             self.params = _lib.SvgfParams()
             check(lib.zr_svgf_pass_default_params(C.byref(self.params)))
+        if cls is AutoExposure:
+            self.params = _lib.AutoExposureParams()
+            check(lib.zr_auto_exposure_pass_default_params(C.byref(self.params)))
+        if cls is Display:
+            self.params = _lib.DisplayParams()
+            check(lib.zr_display_pass_default_params(C.byref(self.params)))
 
 
 class Comm:
@@ -425,6 +510,10 @@ class Comm:
         t = t.to(dev)
         dist.broadcast(t, 0, group=group)
         return cls(bytes(t.cpu().numpy().tobytes()), rank, world)
+
+    def allreduce_u32(self, d_values, n, stream=None, which_comm=0):
+        """In-place sum of n uint32 values (device pointer) over every rank."""
+        check(lib.zr_comm_allreduce_u32(self.handle, int(which_comm), C.c_void_p(d_values), C.c_uint32(n), stream))
 
     def stats(self):
         b, c = C.c_uint64(), C.c_uint64()
@@ -477,6 +566,21 @@ class Renderer:
         h = C.c_void_p()
         check(lib.zr_renderer_set_denoiser(self.handle, int(enable), C.byref(h)))
         self.svgf = _Borrowed(SVGF, h) if enable else None
+
+    def SetDisplay(self, enable=True, lut=None):
+        """AutoExposure on the TAA input and Display on the TAA output (PostProcessor.cpp). lut: the Tony McMapface LUT the
+        default NEUTRAL tone mapper needs (Display.SetLUT)."""
+        ae, disp = C.c_void_p(), C.c_void_p()
+        check(lib.zr_renderer_set_display(self.handle, int(enable), C.byref(ae), C.byref(disp)))
+        self.auto_exposure = _Borrowed(AutoExposure, ae) if enable else None
+        self.display = _Borrowed(Display, disp) if enable else None
+        if enable and lut is not None:
+            self.display.SetLUT(lut)
+
+    def GetDisplayOutput(self):
+        img = _lib.Image2D()
+        check(lib.zr_renderer_get_display_output(self.handle, C.byref(img)))
+        return img
 
     def ApplySceneSettings(self, use_lvg=False):
         """The reference's host decision: presampled sets iff >= 13107 emissive triangles, LVG only with them."""
