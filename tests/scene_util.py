@@ -4,12 +4,12 @@ import os
 import numpy as np
 
 from zetaray_b200 import scene as zscene
+from zetaray_b200._lib import ALIAS_ENTRY
 from tests import orc
 from tests.orc import ptr
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-ALIAS = np.dtype([("CachedP_Orig", "<f4"), ("CachedP_Alias", "<f4"), ("P_Curr", "<f4"), ("Alias", "<u4")])
 
 
 def cornell():
@@ -152,7 +152,7 @@ class OracleScene:
         self.flat = flat
         self.lut = rho_lut()
         self.o.orc_set_rho_lut(ptr(self.lut))
-        self.alias = np.zeros(max(len(flat.emissives), 1), dtype=ALIAS)
+        self.alias = np.zeros(max(len(flat.emissives), 1), dtype=ALIAS_ENTRY)
         self.o.orc_scene_create.restype = C.c_void_p
         self.h = C.c_void_p(self.o.orc_scene_create(ptr(flat.vertices), ptr(flat.indices), ptr(flat.instances),
                                                     len(flat.instances), ptr(flat.instance_num_tris), ptr(flat.materials),

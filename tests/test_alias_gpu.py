@@ -4,8 +4,7 @@ import numpy as np
 import pytest
 
 from tests.orc import ptr
-
-E16 = np.dtype([("CachedP_Orig", "<f4"), ("CachedP_Alias", "<f4"), ("P_Curr", "<f4"), ("Alias", "<u4")])
+from zetaray_b200._lib import ALIAS_ENTRY
 
 
 def make_weights(n, seed):
@@ -23,7 +22,7 @@ def test_alias_build_bit_exact(oracle, n):
     from zetaray_b200 import lib, check
     from tests.gpu_util import dev, dptr, host, stream
     w = np.array([1, 22, 4, 8, 3.5, 10], dtype=np.float32) if n == 6 else make_weights(n, n)
-    ref = np.zeros(n, dtype=E16)
+    ref = np.zeros(n, dtype=ALIAS_ENTRY)
     w_ref = w.copy()
     oracle.orc_alias_build_emissive(ptr(w_ref), C.c_int64(n), 0, ptr(ref))
 
@@ -32,7 +31,7 @@ def test_alias_build_bit_exact(oracle, n):
     d_s = torch.zeros((2 * n + 16) * 4, dtype=torch.uint8, device="cuda")       # 2n stack entries + 16 words of sums / counts
     check(lib.zr_alias_table_build(dptr(d_w), C.c_uint32(n), dptr(d_t), dptr(d_s), stream()))
     torch.cuda.synchronize()
-    got = host(d_t, E16)
+    got = host(d_t, ALIAS_ENTRY)
     assert (got["Alias"] == ref["Alias"]).all()
     for f in ("P_Curr", "CachedP_Orig", "CachedP_Alias"):
         assert got[f].tobytes() == ref[f].tobytes(), f

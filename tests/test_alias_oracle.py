@@ -9,6 +9,7 @@ import os
 import numpy as np
 import pytest
 from tests.orc import ptr
+from zetaray_b200._lib import ALIAS_ENTRY
 
 GOLDEN_REF = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_alias.npz")
 REF_SIZES = [1, 2, 6, 17, 50, 999, 13107, 100000]
@@ -184,7 +185,7 @@ def test_emissive_table_consistent_with_twin(oracle):
     rng = np.random.default_rng(5)
     w = (rng.random(n, dtype=np.float32) * 50).astype(np.float32)
     t, _ = orc_build(oracle, w)
-    e = np.zeros(n, dtype=np.dtype([("CachedP_Orig", "<f4"), ("CachedP_Alias", "<f4"), ("P_Curr", "<f4"), ("Alias", "<u4")]))
+    e = np.zeros(n, dtype=ALIAS_ENTRY)
     ww = w.copy()
     oracle.orc_alias_build_emissive(ptr(ww), C.c_int64(n), 0, ptr(e))
     assert (e["Alias"] == t["Alias"]).all()

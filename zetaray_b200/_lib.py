@@ -1,8 +1,15 @@
-"""ctypes binding of include/zr_abi.h. No compute happens here."""
+"""ctypes binding of include/zr_abi.h. No compute happens here.
+
+Every ZR_API function gets its argtypes and restype from its prototype in the header (prototypes()), so a call with a
+wrongly typed or missing argument raises in Python instead of reaching the library."""
 import ctypes as C
 import os
+import re
+
+import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+HEADER = os.path.join(os.path.dirname(HERE), "include", "zr_abi.h")
 SO_PATH = os.environ.get("ZETARAY_B200_LIB") or os.path.join(HERE, "libzetaray_b200.so")
 
 
@@ -26,14 +33,63 @@ class _NoLibrary:
     shared library is NOT mapped into the process; any call through `lib` fails loudly."""
 
     def __getattr__(self, name):
-        if name in ("zr_last_error", "zr_abi_version", "zr_kernel_launch_count"):
-            return type("_Stub", (), {"restype": None, "argtypes": None})()
         raise ZRError("zetaray_b200 was imported with ZETARAY_B200_STRUCTS_ONLY=1: %s is not available in this process" % name)
 
 
-lib = _NoLibrary() if os.environ.get("ZETARAY_B200_STRUCTS_ONLY") == "1" else _load()
-
 u32, u64, f32, vp, i32 = C.c_uint32, C.c_uint64, C.c_float, C.c_void_p, C.c_int32
+
+# Parameter and return types of the ZR_API prototypes. Besides these, every pointer parameter (T*, T**, T[N]) and every
+# function-pointer typedef is a c_void_p, which takes byref(), pointer(), arrays, None, ints and CFUNCTYPE instances;
+# every enum typedef is a c_int.
+ARG_TYPES = {"uint32_t": u32, "uint64_t": u64, "size_t": C.c_size_t, "float": f32, "int": C.c_int}
+RET_TYPES = {"zr_status": i32, "void": None, "uint32_t": u32, "uint64_t": u64, "const char*": C.c_char_p}
+
+
+def prototypes(text=None):
+    """{name: (restype, [argtypes])} for every ZR_API function of include/zr_abi.h (or of the header text `text`).
+    A declaration that does not parse or uses a type outside the maps above raises ZRError naming it."""
+    if text is None:
+        with open(HEADER) as f:
+            text = f.read()
+    text = re.sub(r"/\*.*?\*/", " ", text, flags=re.S)
+    text = re.sub(r"^\s*#.*$", "", text, flags=re.M)          # the ZR_API definition itself
+    args = dict(ARG_TYPES)
+    args.update((e, C.c_int) for e in re.findall(r"typedef\s+enum\b[^{;]*\{[^}]*\}\s*(\w+)\s*;", text))
+    args.update((fn, vp) for fn in re.findall(r"typedef\s+[\w\s*]+\(\s*\*\s*(\w+)\s*\)", text))
+    out = {}
+    for decl in re.findall(r"\bZR_API\b([^;]*);", text):
+        decl = " ".join(decl.split())
+        m = re.fullmatch(r"(.+?) ?\b(zr_\w+) ?\((.*)\)", decl)
+        if m is None:
+            raise ZRError("zr_abi.h: cannot parse the declaration %r" % decl)
+        ret, name, params = m.groups()
+        ret = ret.replace(" *", "*")
+        if ret not in RET_TYPES:
+            raise ZRError("zr_abi.h: %s returns %r, which has no ctypes type" % (decl, ret))
+        argtypes = []
+        for p in ([] if params == "void" else params.split(",")):
+            p = p.strip()
+            t = vp if "*" in p or "[" in p else args.get(p.rsplit(" ", 1)[0])
+            if t is None:
+                raise ZRError("zr_abi.h: %s takes %r, which has no ctypes type" % (decl, p))
+            argtypes.append(t)
+        out[name] = (RET_TYPES[ret], argtypes)
+    return out
+
+
+def declared_symbols():
+    """All ZR_API functions declared in include/zr_abi.h."""
+    return sorted(prototypes())
+
+
+def _declare(dll):
+    for name, (restype, argtypes) in prototypes().items():
+        f = getattr(dll, name)
+        f.restype, f.argtypes = restype, argtypes
+    return dll
+
+
+lib = _NoLibrary() if os.environ.get("ZETARAY_B200_STRUCTS_ONLY") == "1" else _declare(_load())
 
 
 class FrameConstants(C.Structure):
@@ -111,10 +167,6 @@ class DisplayParams(C.Structure):
     _fields_ = [("tonemapper", u32), ("auto_exposure", u32), ("saturation", f32), ("agx_exp", f32)]
 
 
-lib.zr_last_error.restype = C.c_char_p
-lib.zr_abi_version.restype = u32
-lib.zr_kernel_launch_count.restype = u64
-
 class GIParams(C.Structure):
     _fields_ = [("max_non_tr_bounces", u32), ("max_glossy_tr_bounces", u32), ("russian_roulette", u32), ("stochastic_multi_bounce", u32),
                 ("boiling_suppression", u32), ("M_max", u32), ("temporal_resample", u32)]
@@ -129,22 +181,10 @@ HALO_EXCHANGE_FN = C.CFUNCTYPE(None, C.c_void_p, C.POINTER(Image2D), C.c_int, C.
 # zr_reduce_u32_fn (include/zr_abi.h "AutoExposure")
 REDUCE_U32_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p)
 
-# every other entry point returns zr_status (int32)
-EXPORTS = [
-    "zr_last_error", "zr_abi_version", "zr_kernel_launch_count",
-    "zr_device_malloc", "zr_device_free", "zr_memcpy_h2d", "zr_memcpy_d2h", "zr_memset_d", "zr_stream_synchronize",
-    "zr_alias_table_build", "zr_alias_table_sample",
-]
+# zr_alias_entry (RT::EmissiveLumenAliasTableEntry) as a numpy record
+ALIAS_ENTRY = np.dtype([("CachedP_Orig", "<f4"), ("CachedP_Alias", "<f4"), ("P_Curr", "<f4"), ("Alias", "<u4")])
 
 
 def check(status):
     if status != 0:
         raise ZRError("zr_status %d: %s" % (status, lib.zr_last_error().decode()))
-
-
-def declared_symbols():
-    """All ZR_API functions declared in include/zr_abi.h (parsed from the header)."""
-    import re
-    hdr = os.path.join(os.path.dirname(HERE), "include", "zr_abi.h")
-    txt = open(hdr).read()
-    return sorted(set(re.findall(r"ZR_API\s+[\w\s\*]+?\b(zr_\w+)\s*\(", txt)))
