@@ -51,7 +51,7 @@ ZR_API const char* zr_last_error(void);
  * renderer (zr_renderer_set_shard) and zr_gi_pass_set_rows / set_halo_exchange. 1.3 removed two
  * measurement and test hooks: the ReSTIR PT execution-model switch and the two-dispatch compositing entry point. 1.4 removed
  * the stage-limited ReSTIR PT render and its stage enum, which nothing called. 1.6 added the AutoExposure and Display passes,
- * zr_renderer_set_display / get_display_output and zr_comm_allreduce_u32. */
+ * zr_renderer_set_display / get_display_output and zr_comm_allreduce_u32. 1.7 added zr_comm_create_transport (zr_comm_transport). */
 ZR_API uint32_t zr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -673,11 +673,23 @@ ZR_API uint64_t zr_kernel_launch_count(void);
  * Strip-sharded frames across GPUs (SURVEY 8e; the reference is single-GPU). One process per GPU; zr_comm carries the halo bands
  * between neighbouring strips with grouped NCCL send / recv issued from C++ on the producing stream (csrc/comm.cu).
  * Rank 0 calls zr_comm_unique_id and distributes the 256 bytes (any out-of-band channel: torch.distributed broadcast, MPI, a file);
- * every rank then calls zr_comm_create with the same bytes.
+ * every rank then calls zr_comm_create with the same bytes. A host without NCCL creates its zr_comm from its own transport instead
+ * (zr_comm_create_transport); either kind drives zr_renderer_set_shard.
  * ------------------------------------------------------------------------------------------ */
 typedef struct zr_comm zr_comm;
 ZR_API zr_status zr_comm_unique_id(void* out256);
 ZR_API zr_status zr_comm_create(const void* id256, int rank, int world, zr_comm** out);
+/* A caller-supplied transport: each callback has the contract of the zr_comm_* entry point of the same name (arguments already
+ * checked, world > 1) and returns ZR_OK or an error, which zr_renderer_render then returns. The callbacks run on the calling thread,
+ * inside zr_renderer_render or a pass's render, and must leave the bands in place in stream order. The struct is copied; dlopen is
+ * never involved. */
+typedef struct zr_comm_transport {
+    zr_status (*exchange_halos)(void* user, int which_comm, const uint32_t* bounds, uint32_t halo_rows,
+                                const zr_image2d* planes, int n_planes, void* stream);
+    zr_status (*gather_rows)(void* user, const uint32_t* bounds, const zr_image2d* plane, int root, void* stream);
+    zr_status (*allreduce_u32)(void* user, int which_comm, uint32_t* d_values, uint32_t n, void* stream);
+} zr_comm_transport;
+ZR_API zr_status zr_comm_create_transport(const zr_comm_transport* t, void* user, int rank, int world, zr_comm** out);
 ZR_API void zr_comm_destroy(zr_comm* c);
 ZR_API zr_status zr_comm_rank(zr_comm* c, int* rank, int* world);
 ZR_API zr_status zr_comm_stats(zr_comm* c, uint64_t* bytes_sent, uint64_t* calls);

@@ -17,6 +17,7 @@ MIRRORS = {
     "zr_direct_params": _lib.DirectParams, "zr_indirect_params": _lib.IndirectParams, "zr_gi_params": _lib.GIParams,
     "zr_compositing_params": _lib.CompositingParams, "zr_svgf_params": _lib.SvgfParams,
     "zr_auto_exposure_params": _lib.AutoExposureParams, "zr_display_params": _lib.DisplayParams,
+    "zr_comm_transport": _lib.CommTransport,
 }
 
 
@@ -89,6 +90,36 @@ def test_struct_mirrors_match_the_c_layout(tmp_path):
     for f in _lib.ALIAS_ENTRY.names:
         dt, off = _lib.ALIAS_ENTRY.fields[f][:2]
         assert (off, dt.itemsize) == c["zr_alias_entry", f], f
+
+
+def test_comm_transport_refuses_missing_callbacks_and_bad_rank():
+    """zr_comm_create_transport checks its arguments on the host: all three callbacks, 0 <= rank < world. A comm it makes
+    needs neither NCCL nor a GPU, and at world 1 every exchange returns before reaching the transport."""
+    from zetaray_b200.passes import Comm
+    lib = _lib.lib
+    called = []
+    fns = [lambda *a: called.append(a) or 0 for _ in range(3)]
+    fields = [ftype(fn) for (_, ftype), fn in zip(_lib.CommTransport._fields_, fns)]
+    h = C.c_void_p()
+    for i in range(3):
+        t = _lib.CommTransport(*fields)
+        setattr(t, _lib.CommTransport._fields_[i][0], _lib.CommTransport._fields_[i][1]())      # a NULL callback
+        assert lib.zr_comm_create_transport(C.byref(t), None, 0, 2, C.byref(h)) == 1
+        assert b"zr_comm_create_transport" in lib.zr_last_error()
+    t = _lib.CommTransport(*fields)
+    for rank, world in ((-1, 2), (2, 2), (3, 2), (0, 0)):
+        assert lib.zr_comm_create_transport(C.byref(t), None, rank, world, C.byref(h)) == 1, (rank, world)
+    assert lib.zr_comm_create_transport(None, None, 0, 1, C.byref(h)) == 1
+    assert lib.zr_comm_create_transport(C.byref(t), None, 0, 1, None) == 1
+    comm = Comm.from_transport(*fns, 0, 1)
+    bounds = (C.c_uint32 * 2)(0, 64)
+    img = _lib.Image2D(None, 8, 64, 32, 4)
+    assert lib.zr_comm_exchange_halos(comm.handle, 0, bounds, 32, C.byref(img), 1, None) == 0
+    assert lib.zr_comm_gather_rows(comm.handle, bounds, C.byref(img), 0, None) == 0
+    assert lib.zr_comm_allreduce_u32(comm.handle, 0, C.byref(C.c_uint32()), 1, None) == 0
+    assert lib.zr_comm_exchange_halos(comm.handle, 2, bounds, 32, C.byref(img), 1, None) == 1      # which_comm out of range
+    assert comm.stats() == (0, 0) and not called
+    comm.close()
 
 
 def test_structs_only_import_does_not_map_the_library(tmp_path):

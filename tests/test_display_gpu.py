@@ -276,17 +276,20 @@ class ThreadSum:
         self.fn = _lib.REDUCE_U32_FN(self._hook)
         self.calls = 0
 
+    def reduce(self, d_values, n, stream):
+        from zetaray_b200 import lib, check
+        st = C.c_void_p(stream)
+        self.shared[self.rank] = _download(d_values, np.zeros(n, dtype=np.uint32), st)
+        self.barrier.wait()
+        total = np.sum([self.shared[q] for q in sorted(self.shared)], axis=0, dtype=np.uint32)
+        self.barrier.wait()
+        check(lib.zr_memcpy_h2d(C.c_void_p(d_values), ptr(total), C.c_size_t(total.nbytes), st))
+        check(lib.zr_stream_synchronize(st))
+        self.calls += 1
+
     def _hook(self, user, d_values, n, stream):
-        from zetaray_b200 import lib
         try:
-            st = C.c_void_p(stream)
-            self.shared[self.rank] = _download(d_values, np.zeros(n, dtype=np.uint32), st)
-            self.barrier.wait()
-            total = np.sum([self.shared[q] for q in sorted(self.shared)], axis=0, dtype=np.uint32)
-            self.barrier.wait()
-            lib.zr_memcpy_h2d(C.c_void_p(d_values), ptr(total), C.c_size_t(total.nbytes), st)
-            lib.zr_stream_synchronize(st)
-            self.calls += 1
+            self.reduce(d_values, n, stream)
         except BaseException as e:      # noqa: BLE001  (nothing propagates out of a ctypes callback)
             self.errors.append(e)
             self.barrier.abort()

@@ -1,57 +1,91 @@
-"""Strip-sharded frames exercised on ONE GPU: two ranks run as two host threads with their own streams and full-size
-buffers on cuda:0, and the halo "transport" is a device-to-device copy between the two ranks' planes at the points where
-the passes call the exchange hook. Everything above the transport is the production code path (row ranges in every pass,
-the hook inside zr_direct_pass_render / zr_indirect_pass_render, ShardedFrame), so this checks on a single-GPU box what
-tests/test_sharded_gpu.py checks with NCCL on several: every rank's strip is byte-identical to the unsharded frame."""
+"""Strip-sharded frames of the native renderer exercised on ONE GPU: every rank is a host thread with its own scene, renderer and
+stream on cuda:0, and its zr_comm is built from a caller-supplied transport (zr_comm_create_transport) that copies the halo
+bands between the ranks' planes on the device. Everything above the transport is the product path (zr_renderer_set_shard, the
+row ranges in every pass, the exchange hooks inside the lighting passes, the exchange before Compositing, the gather on rank 0),
+so this checks on a single-GPU box what tests/test_sharded_gpu.py checks with NCCL on several: every rank's strip is
+byte-identical to the unsharded frame."""
 import ctypes as C
 import threading
+import types
 
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
+ZR_ERR_CUDA = 2
 
-class ThreadHalo:
-    """Drop-in for sharding.HaloExchanger between host threads of one process."""
 
-    def __init__(self, plan, rank, shared, barrier):
-        self.plan, self.rank, self.world = plan, rank, plan.world
-        self.shared, self.barrier = shared, barrier
-        self.calls = 0
+def _device_rows(img):
+    """uint8 [H, pitch] torch view of a zr_image2d on cuda:0, without a copy."""
+    import torch
+    cai = {"shape": (img.height * img.pitch_bytes,), "typestr": "|u1", "data": (int(img.d_ptr), False), "version": 2}
+    return torch.as_tensor(types.SimpleNamespace(__cuda_array_interface__=cai), device="cuda").view(img.height, img.pitch_bytes)
 
-    def _bands(self, r):
-        y0, y1 = self.plan.rows(r)
-        return (y0, min(y0 + 32, y1)), (max(y1 - 32, y0), y1)
 
-    def exchange(self, planes):
+class ThreadTransport:
+    """zr_comm_transport between ranks that are host threads of one process on one GPU. Each call synchronises the device (the
+    rank's rows of this stage are complete), meets the other ranks at a barrier, copies what it needs out of their planes,
+    synchronises again and meets them once more (nobody overwrites rows a peer is still reading). An exception is recorded,
+    aborts the barrier so no peer waits forever, and becomes an error status the renderer returns."""
+
+    def __init__(self, rank, world, shared, sums, barrier, errors):
+        from tests.test_display_gpu import ThreadSum
+        self.rank, self.world, self.shared, self.barrier, self.errors = rank, world, shared, barrier, errors
+        self.sum = ThreadSum(rank, sums, barrier, errors)
+        self.exchanges = [0, 0]         # per which_comm
+
+    def comm(self):
+        from zetaray_b200.passes import Comm
+        return Comm.from_transport(*(self._guarded(fn) for fn in (self._exchange_halos, self._gather_rows, self._allreduce_u32)),
+                                   self.rank, self.world)
+
+    def _guarded(self, fn):
+        def call(*args):
+            try:
+                fn(*args)
+                return 0
+            except BaseException as e:      # noqa: BLE001  (nothing propagates out of a ctypes callback)
+                self.errors.append(e)
+                self.barrier.abort()
+                return ZR_ERR_CUDA
+        return call
+
+    def _publish(self, planes):
         import torch
         torch.cuda.synchronize()                    # my rows of this stage are complete
         self.shared[self.rank] = planes
         self.barrier.wait()
-        r = self.rank
-        for i, p in enumerate(planes):
-            if r > 0:
-                (_, _), (b0, b1) = self._bands(r - 1)
-                p[b0:b1].copy_(self.shared[r - 1][i][b0:b1])
-            if r < self.world - 1:
-                (t0, t1), (_, _) = self._bands(r + 1)
-                p[t0:t1].copy_(self.shared[r + 1][i][t0:t1])
-        torch.cuda.synchronize()
-        self.barrier.wait()                         # nobody overwrites rows a peer is still reading
-        self.calls += 1
 
-    def gather_rows(self, plane):
+    def _release(self):
         import torch
         torch.cuda.synchronize()
-        self.shared[self.rank] = [plane]
-        self.barrier.wait()
-        for q in range(self.world):
-            if q != self.rank:
-                a, b = self.plan.rows(q)
-                plane[a:b].copy_(self.shared[q][0][a:b])
-        torch.cuda.synchronize()
-        self.barrier.wait()
+        self.barrier.wait()                         # nobody overwrites rows a peer is still reading
+
+    def _exchange_halos(self, user, which_comm, bounds, halo, planes, n, stream):
+        b, r = [bounds[q] for q in range(self.world + 1)], self.rank
+        mine = [_device_rows(planes[i]) for i in range(n)]
+        self._publish(mine)
+        for i, p in enumerate(mine):
+            if r > 0:                               # the upper neighbour's bottom band
+                y0 = max(b[r] - halo, b[r - 1])
+                p[y0:b[r]].copy_(self.shared[r - 1][i][y0:b[r]])
+            if r < self.world - 1:                  # the lower neighbour's top band
+                y1 = min(b[r + 1] + halo, b[r + 2])
+                p[b[r + 1]:y1].copy_(self.shared[r + 1][i][b[r + 1]:y1])
+        self._release()
+        self.exchanges[which_comm] += 1
+
+    def _gather_rows(self, user, bounds, plane, root, stream):
+        mine = _device_rows(plane[0])
+        self._publish(mine)
+        for q in range(self.world) if self.rank == root else ():
+            if q != root:
+                mine[bounds[q]:bounds[q + 1]].copy_(self.shared[q][bounds[q]:bounds[q + 1]])
+        self._release()
+
+    def _allreduce_u32(self, user, which_comm, d_values, n, stream):
+        self.sum.reduce(d_values, n, stream)
 
 
 @pytest.mark.parametrize("pass_cls,has_schedule_costs", [("DirectLighting", True), ("IndirectLighting", True), ("IndirectLightingGI", False)])
@@ -77,77 +111,120 @@ def test_lighting_pass_strip_setters_refuse_bad_input(pass_cls, has_schedule_cos
     assert set_costs(p.handle, None, 0, 0) == 0
 
 
-@pytest.mark.parametrize("which,bounds", [("glossy", [0, 96, 200]), ("glass", [0, 64, 128, 200])])
-def test_sharded_threads_equal_unsharded(which, bounds):
+def _planes(R, integrator, display):
+    """(name, image, texel bytes) of every output the sharded frame must reproduce in its strip."""
+    ind = R.gi if integrator == "gi" else R.indirect
+    out = [("direct final", R.direct.GetOutput(0)), ("direct reservoirs", R.direct.GetOutput(1)),
+           ("indirect final", ind.GetOutput(0)), ("indirect reservoirs", ind.GetOutput(1)),
+           ("composited", R.compositing.GetOutput()), ("taa", R.GetOutput())]
+    if display:
+        out.append(("display", R.GetDisplayOutput()))
+    return out
+
+
+def _download(img):
+    from zetaray_b200.passes import download_image
+    return download_image(img, np.uint8, img.texel_bytes).reshape(img.height, -1)
+
+
+@pytest.mark.parametrize("which,integrator,bounds,two_streams,cost,display", [
+    ("glossy", "pt", [0, 96, 200], True, False, False),        # the DirectLighting hook runs on the second comm
+    ("glass", "pt", [0, 64, 128, 200], False, True, False),     # measured cost map -> block schedule
+    ("glossy", "gi", [0, 32, 128, 200], False, False, False),   # ReSTIR GI; a one-band strip: its top and bottom bands coincide
+    ("cornell", "pt", [0, 96, 200], False, False, True),        # AutoExposure's all-reduce, the display image gathered
+], ids=["pt-two-streams", "pt-cost-schedule", "gi-one-band-strip", "pt-display"])
+def test_sharded_threads_equal_unsharded(which, integrator, bounds, two_streams, cost, display):
     import torch
-    from zetaray_b200 import _lib
-    from zetaray_b200.passes import (Scene, GBuffers, GBufferRT, DirectLighting, IndirectLighting, Compositing, TAA, download_image)
-    from zetaray_b200.sharding import ShardedFrame, StripPlan
+    from zetaray_b200.passes import Scene, Renderer
+    from zetaray_b200.sharding import StripPlan
     from zetaray_b200.camera import FrameSequence
     from tests import scene_util
+    from tests.test_display_oracle import load_lut
     W, H = 288, 200
+    warm, frames = 2, 4
     world = len(bounds) - 1
     plan = StripPlan(H, bounds)
-    scene = Scene(scene_util.SCENES[which]())
-    scene.prelighting()
-    torch.cuda.synchronize()
-    frames = [FrameSequence(W, H, cam_path=lambda f: (0.02 * f, 1.2, -4.043)) for _ in range(world + 1)]
-    fcs = [[seq.next() for _ in range(6)] for seq in frames]
+    flat = scene_util.SCENES[which]()
+    lut = load_lut() if display else None
+    tiles_x, tiles_y = (W + 31) // 32, StripPlan.num_units(H)
 
-    def pipeline(rank):
-        passes = dict(gbuffer=GBufferRT(), direct=DirectLighting(W, H), indirect=IndirectLighting(W, H),
-                      compositing=Compositing(W, H), taa=TAA(W, H))
-        fi = _lib.FrameInputs()
-        fi.scene = scene.handle
-        return ShardedFrame(passes, GBuffers(W, H), W, H, rank, world), fi
+    def renderer(streams):
+        # every renderer has its own scene: the first frame of each runs prelighting on it
+        R = Renderer(Scene(flat), W, H, two_streams=streams)
+        if integrator == "gi":
+            R.SetMethod(Renderer.RESTIR_GI)
+        if display:
+            R.SetDisplay(True, lut=lut)
+        return R
 
-    # unsharded reference
-    ref, fi_ref = pipeline(0)
-    ref.world = 1
+    def frame_constants():
+        seq = FrameSequence(W, H, cam_path=lambda f: (0.02 * f, 1.2, -4.043))
+        fcs = [seq.next() for _ in range(warm + frames)]
+        for fc in fcs:
+            fc.dt = 1 / 60
+        return fcs
+
+    # unsharded reference, rendered first on this thread
+    ref = renderer(False)
     s0 = torch.cuda.Stream()
-    ref_out = []
-    for fc in fcs[world]:
-        ref.render(fi_ref, fc, s0)
+    want = []
+    for fc in frame_constants():
+        ref.Render(fc, C.c_void_p(s0.cuda_stream))
         torch.cuda.synchronize()
-        ref_out.append({k: download_image(img, np.uint8, img.texel_bytes).reshape(H, -1) for k, img in (
-            ("direct", ref.p["direct"].GetOutput(0)), ("indirect", ref.p["indirect"].GetOutput(0)),
-            ("di_res", ref.p["direct"].GetOutput(1)), ("pt_res", ref.p["indirect"].GetOutput(1)), ("taa", ref.p["taa"].GetOutput()))})
+        got = {k: _download(img) for k, img in _planes(ref, integrator, display)}
+        if display:
+            got["exposure"] = _download(ref.auto_exposure.GetOutput())
+        want.append(got)
 
-    shared, barrier = {}, threading.Barrier(world)
-    errors = []
+    ranks = [renderer(two_streams) for _ in range(world)]
+    shared, sums, barrier, errors = {}, {}, threading.Barrier(world), []
+    transports = [ThreadTransport(r, world, shared, sums, barrier, errors) for r in range(world)]
+    comms = [t.comm() for t in transports]
 
     def rank_main(rank):
+        R = ranks[rank]
         try:
             torch.cuda.set_device(0)
-            stream = torch.cuda.Stream()
-            sf, fi = pipeline(rank)
-            for f, fc in enumerate(fcs[rank]):
-                if f == 2:          # two unsharded warm-up frames (every rank has the full history), then cut
-                    sf.shard(plan)
-                    sf.halo = ThreadHalo(plan, rank, shared, barrier)
-                sf.render(fi, fc, stream)
+            st = torch.cuda.Stream()
+            d_cost = torch.zeros(tiles_x * tiles_y, dtype=torch.int64, device="cuda")
+            if cost:
+                R.direct.SetCostMap(d_cost.data_ptr()); R.indirect.SetCostMap(d_cost.data_ptr())
+            y0, y1 = plan.rows(rank)
+            for f, fc in enumerate(frame_constants()):
+                if f == warm:       # unsharded warm-up frames (every rank has the full history), then cut
+                    torch.cuda.synchronize()
+                    if cost:
+                        R.direct.SetCostMap(0); R.indirect.SetCostMap(0)
+                        tiles = [float(v) for v in d_cost.tolist()]
+                        assert sum(tiles) > 0, "cost map stayed empty"
+                        R.direct.SetScheduleCosts(tiles, tiles_x, tiles_y)
+                        R.indirect.SetScheduleCosts(tiles, tiles_x, tiles_y)
+                    R.SetShard(comms[rank], plan.bounds, gather_output=True)
+                R.Render(fc, C.c_void_p(st.cuda_stream))
                 torch.cuda.synchronize()
-                if f >= 2:
-                    y0, y1 = plan.rows(rank)
-                    for k, img in (("direct", sf.p["direct"].GetOutput(0)), ("indirect", sf.p["indirect"].GetOutput(0)),
-                                   ("di_res", sf.p["direct"].GetOutput(1)), ("pt_res", sf.p["indirect"].GetOutput(1)), ("taa", sf.p["taa"].GetOutput())):
-                        got = download_image(img, np.uint8, img.texel_bytes).reshape(H, -1)[y0:y1]
-                        want = ref_out[f][k][y0:y1]
-                        if k == "pt_res":       # bytes of an EMPTY reservoir beyond its header are don't-care
-                            g4, w4 = got.reshape(y1 - y0, W, 64), want.reshape(y1 - y0, W, 64)
-                            empty = (w4[..., 0] & 0xf) == 15
-                            g4 = np.where(empty[..., None] & (np.arange(64) >= 16)[None, None, :], 0, g4)
-                            w4 = np.where(empty[..., None] & (np.arange(64) >= 16)[None, None, :], 0, w4)
-                            got, want = g4.reshape(y1 - y0, -1), w4.reshape(y1 - y0, -1)
-                        if not np.array_equal(got, want):
-                            bad = np.argwhere(got != want)[0]
-                            raise AssertionError("rank %d frame %d: %s differs at row %d" % (rank, f, k, y0 + bad[0]))
-            sf.gather_output(stream)
-            torch.cuda.synchronize()
-            full = download_image(sf.p["taa"].GetOutput(), np.uint8, 8).reshape(H, -1)
-            if not np.array_equal(full, ref_out[-1]["taa"]):
-                raise AssertionError("rank %d: gathered image differs" % rank)
-            assert sf.halo.calls >= 3 * 4
+                if f < warm:
+                    continue
+                got = {k: _download(img) for k, img in _planes(R, integrator, display)}
+                if display:
+                    got["exposure"] = _download(R.auto_exposure.GetOutput())
+                for k in got:
+                    g, w = (got[k], want[f][k]) if k == "exposure" else (got[k][y0:y1], want[f][k][y0:y1])
+                    if k == "indirect reservoirs" and integrator == "pt":
+                        # bytes of an EMPTY reservoir beyond its header are don't-care
+                        g4, w4 = g.reshape(y1 - y0, W, 64), w.reshape(y1 - y0, W, 64)
+                        care = ~(((w4[..., 0] & 0xf) == 15)[..., None] & (np.arange(64) >= 16)[None, None, :])
+                        g, w = g4 * care, w4 * care
+                    bad = np.argwhere(g != w)
+                    if bad.size:
+                        raise AssertionError("rank %d frame %d: %s differs, first at (row, byte) %s of strip [%d, %d)" % (
+                            rank, f, k, bad[0].tolist(), y0, y1))
+                for k in ("taa", "display") if rank == 0 else ():
+                    if k in got and not np.array_equal(got[k], want[f][k]):
+                        raise AssertionError("frame %d: %s image gathered on rank 0 differs" % (f, k))
+            sent, calls = comms[rank].stats()
+            assert calls >= (3 if integrator == "gi" else 4) * frames and sent > 0, (sent, calls)
+            # with two streams DirectLighting exchanges its reservoirs on the second comm
+            assert (transports[rank].exchanges[1] >= frames) if two_streams else (transports[rank].exchanges[1] == 0), transports[rank].exchanges
         except BaseException as e:      # noqa: BLE001
             errors.append(e)
             barrier.abort()

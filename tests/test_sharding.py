@@ -1,16 +1,12 @@
-"""Host logic of the strip-sharded frame (zetaray_b200/sharding.py) on CPU: partition properties and the halo
-all-gather under gloo with world_size 2 and 3. No CUDA and no product kernels here -- the GPU-side parity of a
-sharded frame against the unsharded one is tests/test_sharded_gpu.py."""
+"""Strip planning of sharded frames (zetaray_b200/sharding.py) on CPU: partition properties and optimality. No CUDA and no
+product kernels here -- the GPU-side parity of a sharded frame against the unsharded one is tests/test_sharded_1gpu.py (ranks
+as threads on one GPU) and tests/test_sharded_gpu.py (NCCL on 2 and 4 GPUs)."""
 import importlib.util
 import itertools
 import os
-import socket
 
 import numpy as np
 import pytest
-import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -64,90 +60,3 @@ def test_uniform_plan_1080p():
     plan = S.StripPlan.uniform(1080, 8)
     sizes = [b - a for a, b in zip(plan.bounds, plan.bounds[1:])]
     assert sum(sizes) == 1080 and max(sizes) == 160         # 34 bands over 8 ranks: the bottleneck is ceil(34 / 8) = 5 bands
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _blur(img, radius):
-    """vertical box filter with clamped taps: a stand-in for 'reads up to `radius` rows away'"""
-    H = img.shape[0]
-    out = np.zeros_like(img, dtype=np.int64)
-    for dy in range(-radius, radius + 1):
-        idx = np.clip(np.arange(H) + dy, 0, H - 1)
-        out += img[idx].astype(np.int64)
-    return (out % 251).astype(np.uint8)
-
-
-def _worker(rank, world, port, height, bounds, out_dir, mode):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        plan = S.StripPlan(height, bounds)
-        halo = S.HaloExchanger(plan, rank, mode=mode)
-        y0, y1 = plan.rows(rank)
-        rng = np.random.default_rng(1234)
-        truth = [rng.integers(0, 255, size=(height, pitch), dtype=np.uint8) for pitch in (64, 16)]
-        # ---- 1. halo exchange: own rows hold the truth, everything else is poison ----
-        planes = []
-        for t in truth:
-            p = np.full_like(t, 0xEE)
-            p[y0:y1] = t[y0:y1]
-            planes.append(torch.from_numpy(p))
-        halo.exchange(planes)
-        for t, p in zip(truth, planes):
-            p = p.numpy()
-            g0, g1 = plan.rows_with_halo(rank)
-            # the neighbour band is as tall as the neighbour's strip allows (<= 32 rows)
-            lo = y0 - min(32, y0 - plan.bounds[rank - 1]) if rank > 0 else 0
-            hi = y1 + min(32, plan.bounds[rank + 2] - y1) if rank < world - 1 else height
-            assert np.array_equal(p[lo:hi], t[lo:hi]), "halo rows wrong on rank %d" % rank
-            assert np.all(p[:lo] == 0xEE) and np.all(p[hi:] == 0xEE), "rows beyond the halo were touched"
-        # ---- 2. two dependent stencil stages with an exchange between them == the unsharded pipeline ----
-        src = truth[0]
-        full = _blur(_blur(src, 15), 23)
-        a = torch.from_numpy(src.copy())
-        stage1 = np.zeros_like(src)
-        stage1[y0:y1] = _blur(a.numpy(), 15)[y0:y1]           # stage 1 only needs the (replicated) input
-        s1 = torch.from_numpy(stage1)
-        halo.exchange([s1])
-        lo, hi = max(0, y0 - 32), min(height, y1 + 32)
-        # stage 2 on the strip: taps clamp at the IMAGE border, not at the strip, so blur the halo-extended window
-        window = s1.numpy()[lo:hi]
-        ext = np.concatenate([np.repeat(window[:1], 23, 0) if lo == 0 else s1.numpy()[lo - 0:lo], window,
-                              np.repeat(window[-1:], 23, 0) if hi == height else window[:0]])
-        off = 23 if lo == 0 else 0
-        blurred = _blur(ext, 23)[off:off + (hi - lo)]
-        mine = blurred[y0 - lo:y1 - lo]
-        # interior rows (>= 23 rows from the window edge or at the image border) must match exactly
-        assert np.array_equal(mine, full[y0:y1]), "sharded stencil differs on rank %d" % rank
-        # ---- 3. final gather ----
-        res = np.zeros_like(src)
-        res[y0:y1] = mine
-        rt = torch.from_numpy(res)
-        halo.gather_rows(rt)
-        assert np.array_equal(rt.numpy(), full)
-        assert halo.calls == 2
-        if mode == "allgather":
-            assert halo.bytes_sent == 2 * 32 * (64 + 16) + 2 * 32 * 64
-        open(os.path.join(out_dir, "ok%d" % rank), "w").write("ok")
-    finally:
-        dist.destroy_process_group()
-
-
-@pytest.mark.parametrize("world,height,bounds", [
-    (2, 200, [0, 96, 200]),
-    (3, 200, [0, 32, 128, 200]),          # a one-band strip in the middle: its top and bottom bands coincide
-    (2, 1080, [0, 544, 1080]),
-])
-@pytest.mark.parametrize("mode", ["p2p", "allgather"])
-def test_halo_exchange_gloo(tmp_path, world, height, bounds, mode):
-    port = _free_port()
-    mp.spawn(_worker, args=(world, port, height, bounds, str(tmp_path), mode), nprocs=world, join=True)
-    assert all(os.path.exists(tmp_path / ("ok%d" % r)) for r in range(world))

@@ -181,6 +181,14 @@ HALO_EXCHANGE_FN = C.CFUNCTYPE(None, C.c_void_p, C.POINTER(Image2D), C.c_int, C.
 # zr_reduce_u32_fn (include/zr_abi.h "AutoExposure")
 REDUCE_U32_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p)
 
+
+class CommTransport(C.Structure):
+    """zr_comm_transport (include/zr_abi.h "Strip-sharded frames"): every callback returns a zr_status."""
+    _fields_ = [("exchange_halos", C.CFUNCTYPE(i32, vp, C.c_int, C.POINTER(u32), u32, C.POINTER(Image2D), C.c_int, vp)),
+                ("gather_rows", C.CFUNCTYPE(i32, vp, C.POINTER(u32), C.POINTER(Image2D), C.c_int, vp)),
+                ("allreduce_u32", C.CFUNCTYPE(i32, vp, C.c_int, vp, u32, vp))]
+
+
 # zr_alias_entry (RT::EmissiveLumenAliasTableEntry) as a numpy record
 ALIAS_ENTRY = np.dtype([("CachedP_Orig", "<f4"), ("CachedP_Alias", "<f4"), ("P_Curr", "<f4"), ("Alias", "<u4")])
 

@@ -2,6 +2,8 @@
 // between neighbouring strips, issued from C++ on the stream the producing kernels run on (no host callback, no packing: a band is
 // a contiguous row range of a plane). NCCL is bound at run time with dlopen / dlsym (libnccl.so.2: torch's bundled copy when the
 // host process is a torch.distributed rank, the system library otherwise), so the library has no link-time dependency on it.
+// A host without NCCL supplies its own transport instead (zr_comm_create_transport); every zr_comm_* entry checks its arguments,
+// returns early at world == 1 and counts its traffic in one place, then hands the bands to NCCL or to that transport.
 #include <dlfcn.h>
 #include <cuda_runtime.h>
 #include <cstring>
@@ -61,8 +63,76 @@ struct zr_comm
 {
     int rank = 0, world = 1;
     NcclComm comm[2] = { nullptr, nullptr };       // [0] main stream, [1] second stream (DirectLighting): never shared between streams
+    zr_comm_transport transport{};                  // set (and comm[] unused) for a comm made by zr_comm_create_transport
+    void* user = nullptr;
     uint64_t bytesSent = 0, calls = 0;
+    bool external() const { return transport.exchange_halos != nullptr; }
 };
+
+namespace
+{
+    // one grouped call (zr_comm_exchange_halos)
+    zr_status NcclExchangeHalos(zr_comm* c, int which_comm, const uint32_t* bounds, uint32_t halo, const zr_image2d* planes, int n_planes,
+        cudaStream_t stream)
+    {
+        NcclApi& a = Api();
+        const int r = c->rank;
+        auto bands = [&](int q, uint32_t& t0, uint32_t& t1, uint32_t& b0, uint32_t& b1)
+        {
+            const uint32_t y0 = bounds[q], y1 = bounds[q + 1];
+            t0 = y0; t1 = y0 + halo < y1 ? y0 + halo : y1;
+            b0 = y1 > y0 + halo ? y1 - halo : y0; b1 = y1;
+        };
+        uint32_t t0, t1, b0, b1;
+        bands(r, t0, t1, b0, b1);
+        ZR_NCCL(a.GroupStart());
+        for (int i = 0; i < n_planes; i++)
+        {
+            unsigned char* base = (unsigned char*)planes[i].d_ptr;
+            const size_t pitch = planes[i].pitch_bytes;
+            if (r > 0)
+            {
+                uint32_t nt0, nt1, nb0, nb1;
+                bands(r - 1, nt0, nt1, nb0, nb1);
+                ZR_NCCL(a.Send(base + (size_t)t0 * pitch, (size_t)(t1 - t0) * pitch, NCCL_UINT8, r - 1, c->comm[which_comm], stream));
+                ZR_NCCL(a.Recv(base + (size_t)nb0 * pitch, (size_t)(nb1 - nb0) * pitch, NCCL_UINT8, r - 1, c->comm[which_comm], stream));
+            }
+            if (r < c->world - 1)
+            {
+                uint32_t nt0, nt1, nb0, nb1;
+                bands(r + 1, nt0, nt1, nb0, nb1);
+                ZR_NCCL(a.Send(base + (size_t)b0 * pitch, (size_t)(b1 - b0) * pitch, NCCL_UINT8, r + 1, c->comm[which_comm], stream));
+                ZR_NCCL(a.Recv(base + (size_t)nt0 * pitch, (size_t)(nt1 - nt0) * pitch, NCCL_UINT8, r + 1, c->comm[which_comm], stream));
+            }
+        }
+        ZR_NCCL(a.GroupEnd());
+        return ZR_OK;
+    }
+
+    zr_status NcclGatherRows(zr_comm* c, const uint32_t* bounds, const zr_image2d* plane, int root, cudaStream_t stream)
+    {
+        NcclApi& a = Api();
+        unsigned char* base = (unsigned char*)plane->d_ptr;
+        const size_t pitch = plane->pitch_bytes;
+        ZR_NCCL(a.GroupStart());
+        if (c->rank == root)
+        {
+            for (int q = 0; q < c->world; q++)
+                if (q != root)
+                    ZR_NCCL(a.Recv(base + (size_t)bounds[q] * pitch, (size_t)(bounds[q + 1] - bounds[q]) * pitch, NCCL_UINT8, q, c->comm[0], stream));
+        }
+        else
+            ZR_NCCL(a.Send(base + (size_t)bounds[c->rank] * pitch, (size_t)(bounds[c->rank + 1] - bounds[c->rank]) * pitch, NCCL_UINT8, root, c->comm[0], stream));
+        ZR_NCCL(a.GroupEnd());
+        return ZR_OK;
+    }
+
+    zr_status TransportStatus(zr_status s, const char* what)
+    {
+        if (s != ZR_OK) zr::set_error("%s: the caller's transport returned %d", what, (int)s);
+        return s;
+    }
+}
 
 extern "C"
 {
@@ -97,6 +167,21 @@ extern "C"
         return ZR_OK;
     }
 
+    zr_status zr_comm_create_transport(const zr_comm_transport* t, void* user, int rank, int world, zr_comm** out)
+    {
+        if (!t || !out || !t->exchange_halos || !t->gather_rows || !t->allreduce_u32 || world < 1 || rank < 0 || rank >= world)
+        {
+            zr::set_error("zr_comm_create_transport: bad args (three callbacks and 0 <= rank < world)");
+            return ZR_ERR_INVALID_ARG;
+        }
+        zr_comm* c = new zr_comm();
+        c->rank = rank; c->world = world;
+        c->transport = *t;
+        c->user = user;
+        *out = c;
+        return ZR_OK;
+    }
+
     void zr_comm_destroy(zr_comm* c)
     {
         if (!c) return;
@@ -120,72 +205,34 @@ extern "C"
     }
 
     // Makes the boundary bands of `planes` coherent between neighbouring strips: this rank's top / bottom `halo` rows go to the strip
-    // above / below, their facing bands arrive in the rows just outside [bounds[rank], bounds[rank + 1]). One grouped call.
+    // above / below, their facing bands arrive in the rows just outside [bounds[rank], bounds[rank + 1]).
     zr_status zr_comm_exchange_halos(zr_comm* c, int which_comm, const uint32_t* bounds, uint32_t halo, const zr_image2d* planes, int n_planes,
-        void* stream_)
+        void* stream)
     {
         if (!c || !bounds || !planes || n_planes < 1 || which_comm < 0 || which_comm > 1) return ZR_ERR_INVALID_ARG;
         if (c->world == 1) return ZR_OK;
-        NcclApi& a = Api();
-        cudaStream_t stream = (cudaStream_t)stream_;
-        const int r = c->rank;
-        auto bands = [&](int q, uint32_t& t0, uint32_t& t1, uint32_t& b0, uint32_t& b1)
-        {
-            const uint32_t y0 = bounds[q], y1 = bounds[q + 1];
-            t0 = y0; t1 = y0 + halo < y1 ? y0 + halo : y1;
-            b0 = y1 > y0 + halo ? y1 - halo : y0; b1 = y1;
-        };
-        uint32_t t0, t1, b0, b1;
-        bands(r, t0, t1, b0, b1);
-        ZR_NCCL(a.GroupStart());
-        for (int i = 0; i < n_planes; i++)
-        {
-            unsigned char* base = (unsigned char*)planes[i].d_ptr;
-            const size_t pitch = planes[i].pitch_bytes;
-            if (r > 0)
-            {
-                uint32_t nt0, nt1, nb0, nb1;
-                bands(r - 1, nt0, nt1, nb0, nb1);
-                ZR_NCCL(a.Send(base + (size_t)t0 * pitch, (size_t)(t1 - t0) * pitch, NCCL_UINT8, r - 1, c->comm[which_comm], stream));
-                ZR_NCCL(a.Recv(base + (size_t)nb0 * pitch, (size_t)(nb1 - nb0) * pitch, NCCL_UINT8, r - 1, c->comm[which_comm], stream));
-                c->bytesSent += (size_t)(t1 - t0) * pitch;
-            }
-            if (r < c->world - 1)
-            {
-                uint32_t nt0, nt1, nb0, nb1;
-                bands(r + 1, nt0, nt1, nb0, nb1);
-                ZR_NCCL(a.Send(base + (size_t)b0 * pitch, (size_t)(b1 - b0) * pitch, NCCL_UINT8, r + 1, c->comm[which_comm], stream));
-                ZR_NCCL(a.Recv(base + (size_t)nt0 * pitch, (size_t)(nt1 - nt0) * pitch, NCCL_UINT8, r + 1, c->comm[which_comm], stream));
-                c->bytesSent += (size_t)(b1 - b0) * pitch;
-            }
-        }
-        ZR_NCCL(a.GroupEnd());
+        const zr_status s = c->external()
+            ? TransportStatus(c->transport.exchange_halos(c->user, which_comm, bounds, halo, planes, n_planes, stream), "zr_comm_exchange_halos")
+            : NcclExchangeHalos(c, which_comm, bounds, halo, planes, n_planes, (cudaStream_t)stream);
+        if (s != ZR_OK) return s;
+        // both bands are min(halo, strip height) rows; the first strip has no band above, the last none below
+        const uint32_t rows = bounds[c->rank + 1] - bounds[c->rank] < halo ? bounds[c->rank + 1] - bounds[c->rank] : halo;
+        const int bands = (c->rank > 0) + (c->rank < c->world - 1);
+        for (int i = 0; i < n_planes; i++) c->bytesSent += (uint64_t)bands * rows * planes[i].pitch_bytes;
         c->calls++;
         return ZR_OK;
     }
 
     // Every rank's own rows of `plane` arrive on rank `root` (the other ranks keep only their strip).
-    zr_status zr_comm_gather_rows(zr_comm* c, const uint32_t* bounds, const zr_image2d* plane, int root, void* stream_)
+    zr_status zr_comm_gather_rows(zr_comm* c, const uint32_t* bounds, const zr_image2d* plane, int root, void* stream)
     {
         if (!c || !bounds || !plane || root < 0 || root >= c->world) return ZR_ERR_INVALID_ARG;
         if (c->world == 1) return ZR_OK;
-        NcclApi& a = Api();
-        cudaStream_t stream = (cudaStream_t)stream_;
-        unsigned char* base = (unsigned char*)plane->d_ptr;
-        const size_t pitch = plane->pitch_bytes;
-        ZR_NCCL(a.GroupStart());
-        if (c->rank == root)
-        {
-            for (int q = 0; q < c->world; q++)
-                if (q != root)
-                    ZR_NCCL(a.Recv(base + (size_t)bounds[q] * pitch, (size_t)(bounds[q + 1] - bounds[q]) * pitch, NCCL_UINT8, q, c->comm[0], stream));
-        }
-        else
-        {
-            ZR_NCCL(a.Send(base + (size_t)bounds[c->rank] * pitch, (size_t)(bounds[c->rank + 1] - bounds[c->rank]) * pitch, NCCL_UINT8, root, c->comm[0], stream));
-            c->bytesSent += (size_t)(bounds[c->rank + 1] - bounds[c->rank]) * pitch;
-        }
-        ZR_NCCL(a.GroupEnd());
+        const zr_status s = c->external()
+            ? TransportStatus(c->transport.gather_rows(c->user, bounds, plane, root, stream), "zr_comm_gather_rows")
+            : NcclGatherRows(c, bounds, plane, root, (cudaStream_t)stream);
+        if (s != ZR_OK) return s;
+        if (c->rank != root) c->bytesSent += (uint64_t)(bounds[c->rank + 1] - bounds[c->rank]) * plane->pitch_bytes;
         return ZR_OK;
     }
 
@@ -193,6 +240,8 @@ extern "C"
     {
         if (!c || !d_values || which_comm < 0 || which_comm > 1) return ZR_ERR_INVALID_ARG;
         if (c->world == 1) return ZR_OK;
+        if (c->external())
+            return TransportStatus(c->transport.allreduce_u32(c->user, which_comm, d_values, n, stream), "zr_comm_allreduce_u32");
         ZR_NCCL(Api().AllReduce(d_values, d_values, n, NCCL_UINT32, NCCL_SUM, c->comm[which_comm], (cudaStream_t)stream));
         return ZR_OK;
     }

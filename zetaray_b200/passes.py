@@ -312,7 +312,8 @@ class Display(_Pass):
 
 class Comm:
     """zr_comm: halo transport between strips (NCCL, bound inside the library). `Comm.from_torch()` distributes the id through an
-    initialised torch.distributed process group; any other out-of-band channel works with Comm.unique_id() / Comm(id, rank, world)."""
+    initialised torch.distributed process group; any other out-of-band channel works with Comm.unique_id() / Comm(id, rank, world).
+    `Comm.from_transport()` moves the bands with the caller's own functions instead."""
 
     def __init__(self, id256, rank, world):
         self.handle = C.c_void_p()
@@ -338,6 +339,18 @@ class Comm:
         t = t.to(dev)
         dist.broadcast(t, 0, group=group)
         return cls(bytes(t.cpu().numpy().tobytes()), rank, world)
+
+    @classmethod
+    def from_transport(cls, exchange_halos, gather_rows, allreduce_u32, rank, world):
+        """zr_comm_create_transport: three callables taking the arguments of the _lib.CommTransport fields and returning a
+        zr_status (0 = OK). An exception cannot cross the C frames that call them: catch it and return an error status.
+        The callables stay alive as long as this Comm."""
+        self = cls.__new__(cls)
+        self.handle, self.rank, self.world = C.c_void_p(), rank, world
+        self._transport = _lib.CommTransport(*(ftype(fn) for (_, ftype), fn in zip(_lib.CommTransport._fields_,
+                                                                                (exchange_halos, gather_rows, allreduce_u32))))
+        check(lib.zr_comm_create_transport(C.byref(self._transport), None, int(rank), int(world), C.byref(self.handle)))
+        return self
 
     def allreduce_u32(self, d_values, n, stream=None, which_comm=0):
         """In-place sum of n uint32 values (device pointer) over every rank."""
