@@ -51,7 +51,8 @@ ZR_API const char* zr_last_error(void);
  * renderer (zr_renderer_set_shard) and zr_gi_pass_set_rows / set_halo_exchange. 1.3 removed two
  * measurement and test hooks: the ReSTIR PT execution-model switch and the two-dispatch compositing entry point. 1.4 removed
  * the stage-limited ReSTIR PT render and its stage enum, which nothing called. 1.6 added the AutoExposure and Display passes,
- * zr_renderer_set_display / get_display_output and zr_comm_allreduce_u32. 1.7 added zr_comm_create_transport (zr_comm_transport). */
+ * zr_renderer_set_display / get_display_output and zr_comm_allreduce_u32. 1.7 added zr_comm_create_transport (zr_comm_transport). 1.8
+ * added zr_svgf_pass_set_rows / set_halo_exchange, and zr_renderer_set_shard runs the SVGF stage sharded instead of refusing it. */
 ZR_API uint32_t zr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -279,8 +280,8 @@ typedef struct zr_image2d
  * ReSTIR_PT_Sort.hlsl:10 and a multiple of every thread-group height), one strip per device. Every pass has
  * set_rows(y0, y1): it then computes and writes rows [y0, y1) only, while reading up to 32 rows beyond them
  * (spatial neighbours <= 15 px for ReSTIR PT, Util.hlsli:9; <= 23 px for ReSTIR DI, Resampling.hlsli:418-423;
- * 1-2 px for the stencils). The lighting passes call the halo-exchange hook at the points where rows they just
- * wrote are about to be read by other strips (after temporal resampling and after every spatial pass); the hook
+ * 1-2 px for the stencils). The lighting passes and the SVGF pass call the halo-exchange hook at the points where rows they
+ * just wrote are about to be read by other strips (after temporal resampling and after every spatial or a-trous pass); the hook
  * must make the 32 rows either side of [y0, y1) of each plane coherent across devices on `stream` (this
  * repository: one NCCL all-gather per call, zetaray_b200/sharding.py). */
 typedef void (*zr_halo_exchange_fn)(void* user, const zr_image2d* planes, int n_planes, void* stream);
@@ -581,6 +582,13 @@ ZR_API zr_status zr_svgf_pass_resize(zr_svgf_pass* p, uint32_t width, uint32_t h
 ZR_API zr_status zr_svgf_pass_reset_temporal(zr_svgf_pass* p);
 ZR_API zr_status zr_svgf_pass_default_params(zr_svgf_params* out);
 ZR_API zr_status zr_svgf_pass_set_params(zr_svgf_pass* p, const zr_svgf_params* params);
+/* multi-GPU: rows [y0, y1) this rank owns. The hook runs num_passes + 1 times per render: after the temporal stage on colour +
+ * variance, guide and history (the first a-trous pass reads colour + variance `radius` rows beyond the strip, every pass reads the
+ * guide up to 32 rows beyond, next frame's reprojection reads guide and history), after every a-trous pass k but the last on the
+ * colour + variance plane it wrote (pass k + 1 reads it radius * 2^(k+1) <= 32 rows beyond), and after the last one on the denoised
+ * output (TAA reads it one row beyond). The internal planes it receives are padded: pitch_bytes >= width * texel_bytes. */
+ZR_API zr_status zr_svgf_pass_set_rows(zr_svgf_pass* p, uint32_t y0, uint32_t y1);
+ZR_API zr_status zr_svgf_pass_set_halo_exchange(zr_svgf_pass* p, zr_halo_exchange_fn fn, void* user);
 ZR_API zr_status zr_svgf_pass_render(zr_svgf_pass* p, const zr_frame_inputs* in, const void* d_signal, void* stream);
 ZR_API zr_status zr_svgf_pass_get_output(zr_svgf_pass* p, zr_svgf_output id, zr_image2d* out);     /* internal planes: pitch_bytes > width * texel */
 ZR_API void zr_svgf_pass_destroy(zr_svgf_pass* p);
@@ -712,10 +720,10 @@ ZR_API zr_status zr_renderer_render(zr_renderer* r, const zr_frame_constants* fr
 /* optional SVGF stage between Compositing and TAA (BASELINE config 3); *out_pass (may be NULL) receives the pass for set_params */
 ZR_API zr_status zr_renderer_set_denoiser(zr_renderer* r, int enable, zr_svgf_pass** out_pass);
 /* Strip-sharded frame: this renderer computes rows [bounds[rank], bounds[rank + 1]) only (bounds: multiples of 32 except the last;
- * any integrator, without the SVGF stage); halo bands move through `comm` at the exchange points of a frame (ReSTIR PT: four, ReSTIR
- * GI: three, path tracer: two), the finished image is gathered on
- * rank 0 (gather_output != 0). comm == NULL returns to the whole frame. History must be complete when the cut happens: render the
- * warm-up frames unsharded on every rank. */
+ * any integrator, with or without the SVGF stage); halo bands move through `comm` at the exchange points of a frame (ReSTIR PT: four,
+ * ReSTIR GI: three, path tracer: two; the SVGF stage adds num_passes + 1), the finished image is gathered on rank 0
+ * (gather_output != 0). A denoiser enabled later follows the current strip. comm == NULL returns to the whole frame. History must be
+ * complete when the cut happens: render the warm-up frames unsharded on every rank. */
 ZR_API zr_status zr_renderer_set_shard(zr_renderer* r, zr_comm* comm, const uint32_t* bounds, int gather_output);
 ZR_API zr_status zr_renderer_get_output(zr_renderer* r, zr_image2d* out);      /* TAA output, RGBA16F */
 /* Optional post-processing (ZetaRenderer/Default/PostProcessor.cpp): enable != 0 creates an AutoExposure pass that reads the TAA

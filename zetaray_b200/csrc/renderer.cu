@@ -74,6 +74,16 @@ struct zr_renderer
         return s;
     }
 
+    // the SVGF pass is created by zr_renderer_set_denoiser, possibly after the cut: it follows the renderer's current strip
+    zr_status ApplyShardToSVGF()
+    {
+        if (!svgf) return ZR_OK;
+        const bool sharded = comm && world > 1;
+        zr_status s = sharded ? zr_svgf_pass_set_rows(svgf, bounds[rank], bounds[rank + 1]) : zr_svgf_pass_set_rows(svgf, 0, height);
+        if (s == ZR_OK) s = zr_svgf_pass_set_halo_exchange(svgf, sharded ? HaloHook : nullptr, &hookMain);
+        return s;
+    }
+
     zr_status ApplyShardToDisplay()
     {
         if (!ae) return ZR_OK;
@@ -216,6 +226,7 @@ extern "C"
         {
             s = zr_svgf_pass_render(r->svgf, &in, comp.d_ptr, stream);
             if (s != ZR_OK) return s;
+            if (r->hookStatus != ZR_OK) { s = r->hookStatus; r->hookStatus = ZR_OK; return s; }
             s = zr_svgf_pass_get_output(r->svgf, ZR_SVGF_DENOISED, &comp);
             if (s != ZR_OK) return s;
         }
@@ -283,7 +294,12 @@ extern "C"
     {
         if (!r) return ZR_ERR_INVALID_ARG;
         zr_status s = ZR_OK;
-        if (enable && !r->svgf) s = zr_svgf_pass_create(r->width, r->height, &r->svgf);
+        if (enable && !r->svgf)
+        {
+            s = zr_svgf_pass_create(r->width, r->height, &r->svgf);
+            if (s == ZR_OK) s = r->ApplyShardToSVGF();
+            if (s != ZR_OK && r->svgf) { zr_svgf_pass_destroy(r->svgf); r->svgf = nullptr; }
+        }
         if (!enable && r->svgf) { zr_svgf_pass_destroy(r->svgf); r->svgf = nullptr; }
         if (out_pass) *out_pass = r->svgf;
         return s;
@@ -326,15 +342,11 @@ extern "C"
             if (s == ZR_OK) s = zr_direct_pass_set_halo_exchange(r->direct, nullptr, nullptr);
             if (s == ZR_OK) s = zr_indirect_pass_set_halo_exchange(r->indirect, nullptr, nullptr);
             if (s == ZR_OK) s = r->ApplyShardToGI();
+            if (s == ZR_OK) s = r->ApplyShardToSVGF();
             if (s == ZR_OK) s = r->ApplyShardToDisplay();
             return s;
         }
         if (!bounds) { zr::set_error("zr_renderer_set_shard: bounds missing"); return ZR_ERR_INVALID_ARG; }
-        if (r->svgf)
-        {
-            zr::set_error("zr_renderer_set_shard: sharded frames run without the SVGF stage (its five a-trous passes reach 62 rows, beyond the 32-row halo)");
-            return ZR_ERR_UNSUPPORTED;
-        }
         int rank = 0, world = 1;
         s = zr_comm_rank(comm, &rank, &world);
         if (s != ZR_OK) return s;
@@ -358,6 +370,7 @@ extern "C"
         if (s == ZR_OK) s = zr_direct_pass_set_halo_exchange(r->direct, world > 1 ? zr_renderer::HaloHook : nullptr, &r->hookSide);
         if (s == ZR_OK) s = zr_indirect_pass_set_halo_exchange(r->indirect, world > 1 ? zr_renderer::HaloHook : nullptr, &r->hookMain);
         if (s == ZR_OK) s = r->ApplyShardToGI();
+        if (s == ZR_OK) s = r->ApplyShardToSVGF();
         if (s == ZR_OK) s = r->ApplyShardToDisplay();
         return s;
     }

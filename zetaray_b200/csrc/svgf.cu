@@ -11,8 +11,13 @@
 // tap), filtered from shared memory, and the result tile leaves through one cp.async.bulk.tensor.4d store (UTMASTG.4D). Every pass
 // therefore reads 1.2-1.4x and writes 1.0x its algorithmic bytes from L2 / HBM at any step, with no strided global access.
 // Step 1 is the same kernel over a plain 2-D map (64 x 16 pixel tiles).
+//
+// Strip-sharded frames (zr_svgf_pass_set_rows / set_halo_exchange): the temporal stage computes the strip's rows, every a-trous
+// pass launches only the tiles whose output rows meet the strip, and the pass calls the halo hook after each stage on the planes
+// the next stage reads beyond the strip. One pass reaches at most R * 2^k <= 32 rows, so the exchange before it fits the halo.
 #include "zr_common.cuh"
 #include "zr_planes.h"
+#include "zr_schedule.h"
 #include "zr_tma.cuh"
 #include <cstdlib>
 
@@ -30,15 +35,16 @@ namespace
     ZR_D uint2 PackCV(float3 c, float var) { return make_uint2(pack_half2(c.x, c.y), pack_half2(c.z, var)); }
 
     // -----------------------------------------------------------------------------------------------------------------
-    // temporal accumulation + variance (orc_svgf_temporal). Internal planes are padded to `pitch` pixels per row.
+    // temporal accumulation + variance (orc_svgf_temporal) of rows [rowBegin, rowEnd), rowEnd <= height. Internal planes are padded
+    // to `pitch` pixels per row. The 3x3 variance fallback reads `core` and `color` one row beyond the rows it computes.
     // -----------------------------------------------------------------------------------------------------------------
     __global__ void __launch_bounds__(256) k_svgf_temporal(zr_frame_constants fc, const uint4* __restrict__ core, const uint2* __restrict__ me,
         const float4* __restrict__ color, const uint2* __restrict__ prevGuide, const uint4* __restrict__ histPrev, int historyValid,
-        uint4* __restrict__ histCurr, uint2* __restrict__ cv, uint2* __restrict__ guide, uint32_t pitch)
+        uint4* __restrict__ histCurr, uint2* __restrict__ cv, uint2* __restrict__ guide, uint32_t pitch, uint32_t rowBegin, uint32_t rowEnd)
     {
         const int W = (int)fc.RenderWidth, H = (int)fc.RenderHeight;
-        const int x = (int)(blockIdx.x * 32 + (threadIdx.x & 31)), y = (int)(blockIdx.y * 8 + (threadIdx.x >> 5));
-        if (x >= W || y >= H) return;
+        const int x = (int)(blockIdx.x * 32 + (threadIdx.x & 31)), y = (int)(rowBegin + blockIdx.y * 8 + (threadIdx.x >> 5));
+        if (x >= W || y >= (int)rowEnd) return;
         const size_t idx = (size_t)y * W + x, pidxOut = (size_t)y * pitch + x;
         const uint4 cr = ld128(&core[idx]);
         const float z = asfloat(cr.x);
@@ -134,10 +140,12 @@ namespace
 
     template<int R, int P, bool LAST>
     // The tensor maps are read from global memory (one address per (pass, plane), uploaded once when the pass is sized) instead of
-    // travelling as 3 x 128 bytes of __grid_constant__ parameters with each of the five launches.
+    // travelling as 3 x 128 bytes of __grid_constant__ parameters with each of the five launches. The pass computes output rows
+    // [rowBegin, rowEnd), rowEnd <= H; blockIdx.x = tile column + tilesU * (tile row - first tile row of the phase meeting those rows);
+    // tilesV = tile rows of the whole frame.
     __global__ void __launch_bounds__(512, 2) k_svgf_atrous(const CUtensorMap* __restrict__ pMapIn, const CUtensorMap* __restrict__ pMapGuide,
         const CUtensorMap* __restrict__ pMapOut, float4* __restrict__ outF, uint32_t W, uint32_t H, uint32_t step, uint32_t tilesU,
-        SvgfParamsDev prm)
+        uint32_t tilesV, uint32_t rowBegin, uint32_t rowEnd, SvgfParamsDev prm)
     {
         using T = AtrousTile<R, P>;
         extern __shared__ __align__(128) unsigned char smem[];
@@ -150,9 +158,17 @@ namespace
         float* s_lum = reinterpret_cast<float*>(s_zn + T::NS);
         uint64_t* bar = reinterpret_cast<uint64_t*>(smem + T::OFF_BAR);
         const uint32_t t = threadIdx.x;
-        const int tu = (int)(blockIdx.x % tilesU), tv = (int)(blockIdx.x / tilesU);
         // phase of the sub-lattice: x-phases 2 * pair, 2 * pair + 1; y-phase py
         const int pair = P == 2 ? (int)(blockIdx.y % (step / 2)) : 0, py = P == 2 ? (int)(blockIdx.y / (step / 2)) : 0;
+        // Tile rows are selected per y-phase: from the phase's first tile row holding an image row >= rowBegin, as many as the phase
+        // that needs most (the host's count), so a phase may run one tile row past the strip, but none past the frame. A strip's
+        // tiles also hold rows outside the strip, and intermediate passes store them whole: those rows may be computed from stale
+        // bands. That is harmless: before the next pass reads them the halo exchange overwrites the 32 rows either side of the
+        // strip, and no pass reads further than 32 rows beyond it. The whole frame (rowBegin = 0, rowEnd = H) runs every tile.
+        // (step is a power of two: a shift, not an integer division, in every block's prologue)
+        const uint32_t vBegin = rowBegin > (uint32_t)py ? (rowBegin - (uint32_t)py + step - 1) >> (__ffs(step) - 1) : 0u;
+        const int tu = (int)(blockIdx.x % tilesU), tv = (int)(vBegin / T::TV + blockIdx.x / tilesU);
+        if (tv >= (int)tilesV) return;
         const int u0 = tu * T::TU, v0 = tv * T::TV;
         if (t == 0)
         {
@@ -250,7 +266,7 @@ namespace
                 int x, y;
                 if (P == 2) { x = (u0 + (ocol >> 1)) * (int)step + 2 * pair + (ocol & 1); y = (v0 + ov) * (int)step + py; }
                 else { x = u0 + ocol; y = v0 + ov; }
-                if (x < (int)W && y < (int)H)
+                if (x < (int)W && y >= (int)rowBegin && y < (int)rowEnd)
                     outF[(size_t)y * W + x] = res;
             }
             else
@@ -292,7 +308,9 @@ struct zr_svgf_pass
     int cur = 0;
     bool historyValid = false;
     zr_svgf_params params = Defaults();
+    zr::StripRows strip{ "zr_svgf_pass" };
     const CUtensorMap* DevMap(int kind, int k, int plane) const { return sz.d_maps + ((kind * MAX_PASSES + k) * 2 + plane); }
+    zr_image2d Padded(void* d_plane, uint32_t texelBytes) const { return zr_image2d{ d_plane, width, height, sz.pitch * texelBytes, texelBytes }; }
 
     static zr_svgf_params Defaults() { zr_svgf_params p{}; p.sigma_z = 0.02f; p.k_n = 16.0f; p.sigma_l = 4.0f; p.radius = 2; p.num_passes = 5; return p; }
 
@@ -374,6 +392,7 @@ struct zr_svgf_pass
         ZR_TRY(EncodeMaps(next, params.radius));
         sz = std::move(next);
         width = w; height = h;
+        strip.ForgetRows();
         historyValid = false; cur = 0;
         return ZR_OK;
     }
@@ -385,8 +404,16 @@ struct zr_svgf_pass
         return ZR_OK;
     }
 
+    // tile rows of `tileRows` lattice rows each that hold image rows [y0, y1) of y-phase py (lattice row v = image row v s + py),
+    // counted from the first such tile row
+    static uint32_t PhaseTileRows(uint32_t y0, uint32_t y1, uint32_t s, uint32_t py, uint32_t tileRows)
+    {
+        const uint32_t vBegin = y0 > py ? (y0 - py + s - 1) / s : 0, vEnd = y1 > py ? (y1 - py + s - 1) / s : 0;
+        return vEnd > vBegin ? (vEnd + tileRows - 1) / tileRows - vBegin / tileRows : 0;
+    }
+
     template<int R>
-    zr_status LaunchAtrous(int k, int inPlane, bool last, cudaStream_t stream)
+    zr_status LaunchAtrous(int k, int inPlane, bool last, uint32_t y0, uint32_t y1, cudaStream_t stream)
     {
         using namespace zr;
         const uint32_t s = 1u << k;
@@ -399,17 +426,20 @@ struct zr_svgf_pass
         {
             using T = AtrousTile<R, 1>;
             const uint32_t tilesU = (width + T::TU - 1) / T::TU, tilesV = (height + T::TV - 1) / T::TV;
-            if (last) k_svgf_atrous<R, 1, true><<<dim3(tilesU * tilesV, 1), 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, prm);
-            else k_svgf_atrous<R, 1, false><<<dim3(tilesU * tilesV, 1), 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, prm);
+            const dim3 grid(tilesU * PhaseTileRows(y0, y1, 1, 0, T::TV), 1);
+            if (last) k_svgf_atrous<R, 1, true><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, tilesV, y0, y1, prm);
+            else k_svgf_atrous<R, 1, false><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, tilesV, y0, y1, prm);
         }
         else
         {
             using T = AtrousTile<R, 2>;
             const uint32_t latW = (width + s - 1) / s, latH = (height + s - 1) / s;
             const uint32_t tilesU = (latW + T::TU - 1) / T::TU, tilesV = (latH + T::TV - 1) / T::TV;
-            const dim3 grid(tilesU * tilesV, (s / 2) * s);
-            if (last) k_svgf_atrous<R, 2, true><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, prm);
-            else k_svgf_atrous<R, 2, false><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, prm);
+            uint32_t rowsOfTiles = 0;
+            for (uint32_t py = 0; py < s; py++) rowsOfTiles = std::max(rowsOfTiles, PhaseTileRows(y0, y1, s, py, T::TV));
+            const dim3 grid(tilesU * rowsOfTiles, (s / 2) * s);
+            if (last) k_svgf_atrous<R, 2, true><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, tilesV, y0, y1, prm);
+            else k_svgf_atrous<R, 2, false><<<grid, 512, T::BYTES, stream>>>(mIn, mG, mOut, sz.d_out, width, height, s, tilesU, tilesV, y0, y1, prm);
         }
         ZR_LAUNCH_CHECK();
         if (getenv("ZR_SVGF_DEBUG"))
@@ -431,20 +461,27 @@ struct zr_svgf_pass
         const zr_status fs = check_frame_size("zr_svgf_pass", in->frame, width, height);
         if (fs != ZR_OK) return fs;
         cur = 1 - cur;
+        const uint32_t y0 = strip.rowBegin, y1 = strip.ClampedRowEnd(height);
         {
             ZR_PROF("k_svgf_temporal", stream);
-            k_svgf_temporal<<<dim3((width + 31) / 32, (height + 7) / 8), 256, 0, stream>>>(in->frame, (const uint4*)in->curr.d_core,
+            k_svgf_temporal<<<dim3((width + 31) / 32, (y1 - y0 + 7) / 8), 256, 0, stream>>>(in->frame, (const uint4*)in->curr.d_core,
                 (const uint2*)in->curr.d_motion_emissive, (const float4*)d_signal, sz.d_guide[1 - cur], sz.d_hist[1 - cur], historyValid ? 1 : 0,
-                sz.d_hist[cur], sz.d_cv[0], sz.d_guide[cur], sz.pitch);
+                sz.d_hist[cur], sz.d_cv[0], sz.d_guide[cur], sz.pitch, y0, y1);
             ZR_LAUNCH_CHECK();
         }
+        // the a-trous passes read colour + variance and the guide beyond the strip; next frame's reprojection reads guide + history
+        const zr_image2d temporalOut[3] = { Padded(sz.d_cv[0], 8u), Padded(sz.d_guide[cur], 8u), Padded(sz.d_hist[cur], 16u) };
+        strip.Exchange(temporalOut, 3, stream);
         int plane = 0;
         for (uint32_t k = 0; k < params.num_passes; k++)
         {
             const bool last = k + 1 == params.num_passes;
-            zr_status st = params.radius == 2 ? LaunchAtrous<2>((int)k, plane, last, stream) : LaunchAtrous<1>((int)k, plane, last, stream);
+            zr_status st = params.radius == 2 ? LaunchAtrous<2>((int)k, plane, last, y0, y1, stream) : LaunchAtrous<1>((int)k, plane, last, y0, y1, stream);
             if (st != ZR_OK) return st;
             plane = 1 - plane;
+            // the next pass reads the plane just written beyond the strip; after the last one, TAA reads the denoised signal there
+            const zr_image2d written = last ? zr_image2d{ sz.d_out, width, height, width * 16u, 16u } : Padded(sz.d_cv[plane], 8u);
+            strip.Exchange(&written, 1, stream);
         }
         historyValid = true;
         return ZR_OK;
@@ -470,6 +507,8 @@ extern "C"
         p->params = *params;
         return ZR_OK;
     }
+    zr_status zr_svgf_pass_set_rows(zr_svgf_pass* p, uint32_t y0, uint32_t y1) { return p ? p->strip.SetRows(y0, y1, p->height) : ZR_ERR_INVALID_ARG; }
+    zr_status zr_svgf_pass_set_halo_exchange(zr_svgf_pass* p, zr_halo_exchange_fn fn, void* user) { return p ? p->strip.SetHaloExchange(fn, user) : ZR_ERR_INVALID_ARG; }
     zr_status zr_svgf_pass_render(zr_svgf_pass* p, const zr_frame_inputs* in, const void* d_signal, void* stream)
     {
         if (!p) return ZR_ERR_INVALID_ARG;
@@ -482,9 +521,9 @@ extern "C"
         switch (id)
         {
         case ZR_SVGF_DENOISED: *out = zr_image2d{ p->sz.d_out, w, h, w * 16u, 16u }; break;
-        case ZR_SVGF_ACCUMULATED: *out = zr_image2d{ p->sz.d_cv[0], w, h, p->sz.pitch * 8u, 8u }; break;       // only valid with num_passes == 1 .. see header
-        case ZR_SVGF_GUIDE: *out = zr_image2d{ p->sz.d_guide[p->cur], w, h, p->sz.pitch * 8u, 8u }; break;
-        case ZR_SVGF_HISTORY: *out = zr_image2d{ p->sz.d_hist[p->cur], w, h, p->sz.pitch * 16u, 16u }; break;
+        case ZR_SVGF_ACCUMULATED: *out = p->Padded(p->sz.d_cv[0], 8u); break;       // only valid with num_passes == 1 .. see header
+        case ZR_SVGF_GUIDE: *out = p->Padded(p->sz.d_guide[p->cur], 8u); break;
+        case ZR_SVGF_HISTORY: *out = p->Padded(p->sz.d_hist[p->cur], 16u); break;
         default: zr::set_error("zr_svgf_pass_get_output: unknown output id"); return ZR_ERR_INVALID_ARG;
         }
         return ZR_OK;

@@ -1,4 +1,5 @@
-// zr_schedule.h -- host side: which thread blocks a lighting kernel launches, and in which order.
+// zr_schedule.h -- host side: the rows a strip-sharded pass owns and its halo hook; which thread blocks a lighting kernel
+// launches, and in which order.
 //
 // A lighting kernel's blocks differ in cost by orders of magnitude (sky vs. the inside of the box) and only one or
 // two of them fit on an SM, so the hardware's in-order block dispatch leaves a tail in which a few SMs finish the
@@ -111,28 +112,18 @@ inline std::vector<uint32_t> ScheduleSwizzled(uint32_t dispX, uint32_t dispY, ui
     return blocks;
 }
 
-// What a lighting pass keeps for strip-sharded frames (SURVEY 8e): the rows it owns, the hook that makes rows it just wrote
-// coherent across strips, the optional cost map and tile costs, and its kernels' block table. `pass` ("zr_direct_pass", ...)
-// prefixes the error messages of the pass's set_* entry points.
-struct LightingStrip
+// What a pass that runs strip-sharded keeps (SURVEY 8e): the rows it owns and the hook that makes rows it just wrote coherent
+// across strips. `pass` ("zr_direct_pass", ...) prefixes the error messages of the pass's set_* entry points.
+struct StripRows
 {
     const char* pass;
     uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
     zr_halo_exchange_fn exchange = nullptr;
     void* exchangeUser = nullptr;
-    unsigned long long* d_costMap = nullptr;
-    TileCosts tileCosts;
-    BlockSchedule sched;
 
-    explicit LightingStrip(const char* passName) : pass(passName) {}
-    // after a resize: the rows, cost map, tile costs and block table described the old frame; the halo hook stays
-    void ForgetSize()
-    {
-        rowBegin = 0; rowEnd = 0xffffffffu;
-        d_costMap = nullptr;
-        tileCosts = TileCosts{};
-        sched.Release();
-    }
+    explicit StripRows(const char* passName) : pass(passName) {}
+    // after a resize: the rows described the old frame; the halo hook stays
+    void ForgetRows() { rowBegin = 0; rowEnd = 0xffffffffu; }
     uint32_t ClampedRowEnd(uint32_t height) const { return rowEnd < height ? rowEnd : height; }
 
     zr_status SetRows(uint32_t y0, uint32_t y1, uint32_t height)
@@ -145,6 +136,35 @@ struct LightingStrip
     {
         exchange = fn; exchangeUser = user;
         return ZR_OK;
+    }
+    // hands the hook n planes (their own pitches); nothing happens without a hook
+    void Exchange(const zr_image2d* planes, int n, cudaStream_t stream) const
+    {
+        if (exchange) exchange(exchangeUser, planes, n, stream);
+    }
+    // one unpadded width x height plane of texelBytes-sized texels
+    void Exchange(void* d_plane, uint32_t width, uint32_t height, uint32_t texelBytes, cudaStream_t stream) const
+    {
+        const zr_image2d plane{ d_plane, width, height, width * texelBytes, texelBytes };
+        Exchange(&plane, 1, stream);
+    }
+};
+
+// What a lighting pass keeps on top of its rows and hook: the optional cost map and tile costs, and its kernels' block table.
+struct LightingStrip : StripRows
+{
+    unsigned long long* d_costMap = nullptr;
+    TileCosts tileCosts;
+    BlockSchedule sched;
+
+    explicit LightingStrip(const char* passName) : StripRows(passName) {}
+    // after a resize: the rows, cost map, tile costs and block table described the old frame; the halo hook stays
+    void ForgetSize()
+    {
+        ForgetRows();
+        d_costMap = nullptr;
+        tileCosts = TileCosts{};
+        sched.Release();
     }
     zr_status SetCostMap(void* d_cycles)
     {
@@ -163,13 +183,6 @@ struct LightingStrip
         tileCosts.tilesX = h_tile_cost ? tiles_x : 0;
         tileCosts.version++;
         return ZR_OK;
-    }
-    // hands the hook one width x height plane of texelBytes-sized texels; nothing happens without a hook
-    void Exchange(void* d_plane, uint32_t width, uint32_t height, uint32_t texelBytes, cudaStream_t stream) const
-    {
-        if (!exchange) return;
-        const zr_image2d plane{ d_plane, width, height, width * texelBytes, texelBytes };
-        exchange(exchangeUser, &plane, 1, stream);
     }
     // sched for a kernel whose blocks are groupsPerBlock swizzled groups of groupW x groupH pixels; the table is rebuilt and
     // uploaded only when the rows or the tile costs changed
