@@ -4,7 +4,8 @@
 //   Compositing            ZetaRenderPass/Compositing/Compositing.hlsl:30-126
 //   FilterFirefly          ZetaRenderPass/Compositing/FireflyFilter.hlsl:35-124
 //   TAA                    ZetaRenderPass/TAA/TAA.hlsl:29-189, Common/Common.hlsli:65-102 (Catmull-Rom)
-// Parity unpinned: the reference has no tests or golden images for these passes.
+// The reference has no tests or golden images for these passes; oracle/indep_post.py is an independent float64 truth of them,
+// and tests/test_post_oracle.py holds this file to it.
 // Documented deviations (DESIGN.md): sky/sun-disk background for invalid pixels is out of scope
 // (writes 0); the firefly filter reads an input image and writes a separate output (the reference
 // filters in place and races with itself); bilinear history taps use exact float weights.
