@@ -282,8 +282,8 @@ typedef struct zr_image2d
  * (spatial neighbours <= 15 px for ReSTIR PT, Util.hlsli:9; <= 23 px for ReSTIR DI, Resampling.hlsli:418-423;
  * 1-2 px for the stencils). The lighting passes and the SVGF pass call the halo-exchange hook at the points where rows they
  * just wrote are about to be read by other strips (after temporal resampling and after every spatial or a-trous pass); the hook
- * must make the 32 rows either side of [y0, y1) of each plane coherent across devices on `stream` (this
- * repository: one NCCL all-gather per call, zetaray_b200/sharding.py). */
+ * must make the 32 rows either side of [y0, y1) of each plane coherent across devices on `stream` (the renderer's hook:
+ * zr_comm_exchange_halos, one grouped send / recv of the boundary bands with the neighbouring strips, csrc/comm.cu). */
 typedef void (*zr_halo_exchange_fn)(void* user, const zr_image2d* planes, int n_planes, void* stream);
 
 /* ------------------------------------------------------------------------------------------

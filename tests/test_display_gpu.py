@@ -1,14 +1,14 @@
 """AutoExposure and Display (csrc/display.cu) against the CPU oracle (oracle/orc_display.cpp), bit for bit: the luminance
 histogram, the exposure state over a frame sequence, the RGBA8 display image for every tone mapper; the renderer's optional
-display stage; error paths; and strip-sharded frames (threads on one GPU, NCCL on 2 and 4 GPUs)."""
+display stage; error paths; and a lone AutoExposure + Display pair in strip-sharded frames (threads on one GPU; the renderer's
+display stage in sharded frames is tested with the rest of the frame in tests/test_sharded_1gpu.py and tests/test_sharded_gpu.py)."""
 import ctypes as C
-import os
-import threading
 
 import numpy as np
 import pytest
 
 from tests.orc import ptr
+from tests.sharded_util import ThreadTransport, compare_strip, host_rows, run_threads
 from tests.test_display_oracle import load_lut, ae_params
 
 pytestmark = pytest.mark.gpu
@@ -155,11 +155,6 @@ def test_display_matches_oracle_every_tonemapper(oracle, w, h):
             assert len(np.unique(out & 0xff)) > min(50, w * h // 4)
 
 
-def _rows_of(img, dtype, comps):
-    from zetaray_b200.passes import download_image
-    return download_image(img, dtype, comps)
-
-
 def test_renderer_display_stage_on_cornell(oracle):
     """Enabling the stage leaves the TAA output byte-identical, and the display image is the oracle applied to the frame's own
     TAA input (exposure) and output (display), frame after frame."""
@@ -181,9 +176,9 @@ def test_renderer_display_stage_on_cornell(oracle):
         plain.Render(fc)
         R.Render(fc)
         check(lib.zr_stream_synchronize(None))
-        taa = _rows_of(R.GetOutput(), np.uint16, 4)
-        assert taa.tobytes() == _rows_of(plain.GetOutput(), np.uint16, 4).tobytes(), "frame %d: TAA output changed" % fr
-        comp = _rows_of(R.compositing.GetOutput(), np.float32, 4)
+        taa = host_rows(R.GetOutput())
+        assert taa.tobytes() == host_rows(plain.GetOutput()).tobytes(), "frame %d: TAA output changed" % fr
+        comp = host_rows(R.compositing.GetOutput())
         hist = np.zeros(256, dtype=np.uint32)
         oracle.orc_lum_histogram(ptr(comp), C.c_uint32(w), C.c_uint32(0), C.c_uint32(h), C.byref(R.auto_exposure.params), ptr(hist))
         oracle.orc_exposure(ptr(hist), C.c_uint32(w * h), C.byref(R.auto_exposure.params), C.c_float(fc.dt), ptr(state))
@@ -191,7 +186,7 @@ def test_renderer_display_stage_on_cornell(oracle):
         assert got_state.tobytes() == state.tobytes(), "frame %d: %s vs %s" % (fr, got_state, state)
         ref = np.zeros(w * h, dtype=np.uint32)
         oracle.orc_display(ptr(taa), C.c_uint32(w), C.c_uint32(0), C.c_uint32(h), C.byref(R.display.params), ptr(state), ptr(lut), ptr(ref))
-        got = _rows_of(R.GetDisplayOutput(), np.uint32, 1).reshape(-1)
+        got = host_rows(R.GetDisplayOutput()).view(np.uint32).reshape(-1)
         assert got.tobytes() == ref.tobytes(), "frame %d: display image differs from the oracle" % fr
     assert len(np.unique(got & 0xffffff)) > 100
     R.SetDisplay(False)
@@ -225,8 +220,6 @@ def test_errors_and_resize():
         for k, v in bad.items():
             setattr(p, k, v)
         assert lib.zr_auto_exposure_pass_set_params(ae.handle, C.byref(p)) == 1, bad
-    assert lib.zr_auto_exposure_pass_set_rows(ae.handle, 10, 10) == 1
-    assert lib.zr_auto_exposure_pass_set_rows(ae.handle, h, h + 1) == 1
     # resize: new size, state back to {0, 0}, dt == 0 rejected again
     ae.OnWindowResized(2 * w, h)
     assert not _download(ae.GetOutput().d_ptr, np.zeros(2, dtype=np.float32)).any()
@@ -267,36 +260,10 @@ def test_errors_and_resize():
     assert disp_render(_fi(w // 2, h)) == 0                               # the LUT survives a resize
 
 
-class ThreadSum:
-    """Reduce hook for ranks that are host threads on one GPU: every rank's bins are summed through host memory."""
-
-    def __init__(self, rank, shared, barrier, errors):
-        from zetaray_b200 import _lib
-        self.rank, self.shared, self.barrier, self.errors = rank, shared, barrier, errors
-        self.fn = _lib.REDUCE_U32_FN(self._hook)
-        self.calls = 0
-
-    def reduce(self, d_values, n, stream):
-        from zetaray_b200 import lib, check
-        st = C.c_void_p(stream)
-        self.shared[self.rank] = _download(d_values, np.zeros(n, dtype=np.uint32), st)
-        self.barrier.wait()
-        total = np.sum([self.shared[q] for q in sorted(self.shared)], axis=0, dtype=np.uint32)
-        self.barrier.wait()
-        check(lib.zr_memcpy_h2d(C.c_void_p(d_values), ptr(total), C.c_size_t(total.nbytes), st))
-        check(lib.zr_stream_synchronize(st))
-        self.calls += 1
-
-    def _hook(self, user, d_values, n, stream):
-        try:
-            self.reduce(d_values, n, stream)
-        except BaseException as e:      # noqa: BLE001  (nothing propagates out of a ctypes callback)
-            self.errors.append(e)
-            self.barrier.abort()
-
-
 @pytest.mark.parametrize("bounds", [[0, 96, 200], [0, 64, 128, 200]])
 def test_sharded_threads_equal_unsharded(bounds):
+    """AutoExposure and Display over each rank's rows, the histogram summed over the ranks: every rank's exposure and its rows of
+    the display image equal the whole-frame passes'."""
     import torch
     from zetaray_b200.passes import AutoExposure, Display
     from tests.gpu_util import dev
@@ -312,107 +279,27 @@ def test_sharded_threads_equal_unsharded(bounds):
         disp.SetLUT(lut)
         return ae, disp
 
-    ae, disp = passes()
-    ref = []
-    s0 = torch.cuda.Stream()
-    for f in range(3):
+    def render(ae, disp, f, stream):
         fi = _fi(W, H, 1 / 60 + f * 0.01)
-        ae.Render(fi, d_sigs[f].data_ptr(), C.c_void_p(s0.cuda_stream))
-        disp.Render(fi, d_taas[f].data_ptr(), ae.GetOutput().d_ptr, C.c_void_p(s0.cuda_stream))
+        ae.Render(fi, d_sigs[f].data_ptr(), C.c_void_p(stream.cuda_stream))
+        disp.Render(fi, d_taas[f].data_ptr(), ae.GetOutput().d_ptr, C.c_void_p(stream.cuda_stream))
         torch.cuda.synchronize()
-        ref.append((_download(ae.GetOutput().d_ptr, np.zeros(2, dtype=np.float32)),
-                    _rows_of(disp.GetOutput(), np.uint32, 1).reshape(H, W)))
+        return {"exposure": host_rows(ae.GetOutput()), "display": host_rows(disp.GetOutput())}
 
-    shared, barrier, errors = {}, threading.Barrier(world), []
+    ae, disp = passes()
+    s0 = torch.cuda.Stream()
+    want = [render(ae, disp, f, s0) for f in range(3)]
+    transports = ThreadTransport.group(world)
 
     def rank_main(rank):
-        try:
-            torch.cuda.set_device(0)
-            st = torch.cuda.Stream()
-            ae, disp = passes()
-            y0, y1 = bounds[rank], bounds[rank + 1]
-            ae.SetRows(y0, y1)
-            disp.SetRows(y0, y1)
-            hook = ThreadSum(rank, shared, barrier, errors)
-            ae.SetReduce(hook.fn)
-            for f in range(3):
-                fi = _fi(W, H, 1 / 60 + f * 0.01)
-                ae.Render(fi, d_sigs[f].data_ptr(), C.c_void_p(st.cuda_stream))
-                disp.Render(fi, d_taas[f].data_ptr(), ae.GetOutput().d_ptr, C.c_void_p(st.cuda_stream))
-                torch.cuda.synchronize()
-                state = _download(ae.GetOutput().d_ptr, np.zeros(2, dtype=np.float32))
-                if state.tobytes() != ref[f][0].tobytes():
-                    raise AssertionError("rank %d frame %d: exposure %s, unsharded %s" % (rank, f, state, ref[f][0]))
-                img = _rows_of(disp.GetOutput(), np.uint32, 1).reshape(H, W)
-                if not np.array_equal(img[y0:y1], ref[f][1][y0:y1]):
-                    raise AssertionError("rank %d frame %d: display strip differs" % (rank, f))
-            assert hook.calls == 3
-        except BaseException as e:      # noqa: BLE001
-            errors.append(e)
-            barrier.abort()
-
-    threads = [threading.Thread(target=rank_main, args=(r,)) for r in range(world)]
-    for t in threads:
-        t.start()
-    for t in threads:
-        t.join()
-    assert not errors, errors[0]
-
-
-def _worker_nccl(rank, world, port, W, H, out_dir):
-    import torch
-    import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
-    try:
-        from zetaray_b200.passes import Scene, Renderer, Comm
-        from zetaray_b200.sharding import StripPlan
-        from tests import scene_util, rpt_util
-        stream = torch.cuda.Stream()
-        torch.cuda.set_stream(stream)
-        st = C.c_void_p(stream.cuda_stream)
-        lut = load_lut()
-        scene = Scene(scene_util.glossy_cornell())
-        A = Renderer(scene, W, H, two_streams=False)
-        B = Renderer(scene, W, H, two_streams=True)
-        for r in (A, B):
-            r.SetDisplay(True, lut=lut)
-        comm = Comm.from_torch()
-        seq = rpt_util.FrameSequence(W, H)
-        for _ in range(2):
-            fc = seq.next()
-            fc.dt = 1 / 60
-            A.Render(fc, st); B.Render(fc, st)
-        plan = StripPlan.uniform(H, world)
-        B.SetShard(comm, plan.bounds, gather_output=True)
-        y0, y1 = plan.rows(rank)
+        ae, disp = passes()
+        y0, y1 = bounds[rank], bounds[rank + 1]
+        ae.SetRows(y0, y1)
+        disp.SetRows(y0, y1)
+        ae.SetReduce(transports[rank].reduce_fn())
+        st = torch.cuda.Stream()
         for f in range(3):
-            fc = seq.next()
-            fc.dt = 1 / 60
-            A.Render(fc, st); B.Render(fc, st)
-            torch.cuda.synchronize()
-            ea = _download(A.auto_exposure.GetOutput().d_ptr, np.zeros(2, dtype=np.float32))
-            eb = _download(B.auto_exposure.GetOutput().d_ptr, np.zeros(2, dtype=np.float32))
-            assert ea.tobytes() == eb.tobytes(), "rank %d frame %d: exposure %s vs %s" % (rank, f, eb, ea)
-            da = _rows_of(A.GetDisplayOutput(), np.uint32, 1).reshape(H, W)
-            db = _rows_of(B.GetDisplayOutput(), np.uint32, 1).reshape(H, W)
-            assert np.array_equal(da[y0:y1], db[y0:y1]), "rank %d frame %d: display strip differs" % (rank, f)
-            if rank == 0:
-                assert np.array_equal(da, db), "frame %d: display image gathered on rank 0 differs" % f
-                assert _rows_of(A.GetOutput(), np.uint16, 4).tobytes() == _rows_of(B.GetOutput(), np.uint16, 4).tobytes()
-        open(os.path.join(out_dir, "ok%d" % rank), "w").write("%s" % plan.bounds)
-    finally:
-        dist.destroy_process_group()
+            compare_strip(render(ae, disp, f, st), want[f], y0, y1, "rank %d frame %d" % (rank, f))
+        assert transports[rank].reductions == 3
 
-
-@pytest.mark.parametrize("world", [2, 4])
-def test_native_sharded_display_equals_unsharded(tmp_path, world):
-    import torch
-    import torch.multiprocessing as mp
-    from tests.test_sharded_gpu import _free_port
-    if torch.cuda.device_count() < world:
-        pytest.skip("needs %d GPUs" % world)
-    mp.spawn(_worker_nccl, args=(world, _free_port(), 416, 296, str(tmp_path)), nprocs=world, join=True)
-    assert all(os.path.exists(tmp_path / ("ok%d" % r)) for r in range(world))
+    run_threads(transports, rank_main)

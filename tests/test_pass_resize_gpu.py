@@ -1,5 +1,5 @@
-"""Pass resize on the device: a resized pass matches one created at the new size, a failed resize changes nothing, a resize forgets
-the cost map, and zero sizes are refused. Cornell box at small sizes; outputs are compared byte for byte."""
+"""Pass resize on the device: a resized pass matches one created at the new size (also when it had a row range, which the resize
+returns to the whole frame), a failed resize changes nothing, a resize forgets the cost map, and zero sizes are refused. Cornell box at small sizes; outputs are compared byte for byte."""
 import ctypes as C
 
 import numpy as np
@@ -10,6 +10,8 @@ A, B = (64, 48), (96, 40)
 HUGE = 1 << 20                  # 2^20 x 2^20 pixels: no plane of that size fits on any device
 ZR_ERR_INVALID_ARG, ZR_ERR_OUT_OF_MEMORY = 1, 5
 KINDS = ["direct", "indirect", "gi", "pathtracer", "compositing", "taa", "svgf"]
+# AutoExposure's planes do not grow with the image, so no size makes its resize fail
+RESIZE_KINDS = KINDS + ["auto_exposure", "display"]
 
 
 class _World:
@@ -32,6 +34,7 @@ class _World:
             self.sizes[size] = (GBuffers(*size), rpt_util.FrameSequence(*size))
         gb, seq = self.sizes[size]
         fc = seq.next()
+        fc.dt = 1 / 60                  # AutoExposure's time step
         gb.flip()
         fi = _lib.FrameInputs()
         fi.frame = fc
@@ -57,13 +60,16 @@ class _Pass:
         from zetaray_b200 import passes as P
         self.kind = kind
         cls = {"direct": P.DirectLighting, "indirect": P.IndirectLighting, "gi": P.IndirectLightingGI, "pathtracer": P.IndirectLightingGI,
-               "compositing": P.Compositing, "taa": P.TAA, "svgf": P.SVGF}[kind]
+               "compositing": P.Compositing, "taa": P.TAA, "svgf": P.SVGF, "auto_exposure": P.AutoExposure, "display": P.Display}[kind]
         self.p = cls(*size)
         if kind == "pathtracer":
             self.p.SetMethod(0)     # ZR_INTEGRATOR_PATH_TRACING
+        if kind == "display":
+            from tests.test_display_oracle import load_lut
+            self.p.SetLUT(load_lut())
         self.prefix = self.p.prefix
         self.ids = {"direct": [0, 1, 2], "indirect": [0, 1, 2, 3, 4, 6], "gi": [0, 1, 2], "pathtracer": [0, 1, 2],
-                    "compositing": [None], "taa": [None], "svgf": [0, 1, 2, 3]}[kind]
+                    "compositing": [None], "taa": [None], "svgf": [0, 1, 2, 3], "auto_exposure": [None], "display": [None]}[kind]
         self.lib = lib
 
     def render(self, world, size):
@@ -75,8 +81,10 @@ class _Pass:
     def feed(self, fi, sig):
         if self.kind == "compositing":
             self.p.Render(fi, sig[0].data_ptr(), sig[1].data_ptr())
-        elif self.kind in ("taa", "svgf"):
+        elif self.kind in ("taa", "svgf", "auto_exposure"):
             self.p.Render(fi, sig[0].data_ptr())
+        elif self.kind == "display":
+            self.p.Render(fi, sig[0].data_ptr(), sig[1].data_ptr())     # signal read as half4, exposure as float2
         else:
             self.p.Render(fi)
 
@@ -127,15 +135,16 @@ def world():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("kind", KINDS)
+@pytest.mark.parametrize("kind", RESIZE_KINDS)
 def test_resize_equals_fresh(world, kind):
     from zetaray_b200 import check
     p = _Pass(kind, A)
     for _ in range(3):
         p.render(world, A)
+    p.p.SetRows(16, 32)                 # the first resize returns the pass to the whole frame; the second one starts there
     for size in (B, A):
         check(p.resize(*size))
-        assert p.size() == size
+        assert p.size() == (size if kind != "auto_exposure" else (1, 1))        # AutoExposure's output is its 1 x 1 state
         fresh = _Pass(kind, size)
         _render_both(world, size, p, fresh, 3)
         _assert_same(p, fresh, "%s resized to %dx%d" % ((kind,) + size))

@@ -13,6 +13,7 @@
 #include <cmath>
 #include "zr_common.cuh"
 #include "zr_planes.h"
+#include "zr_schedule.h"
 
 namespace zr
 {
@@ -244,7 +245,7 @@ struct zr_auto_exposure_pass
         float2* d_state = nullptr;          // {exposure, adapted luminance}
     } sz;
     zr_auto_exposure_params params = Defaults();
-    uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
+    zr::StripRows strip{ "zr_auto_exposure_pass" };
     bool hasHistory = false;                // a frame ran since create / resize / reset
     zr_reduce_u32_fn reduce = nullptr;
     void* reduceUser = nullptr;
@@ -267,7 +268,7 @@ struct zr_auto_exposure_pass
         ZR_TRY(next.planes.Clear());
         sz = std::move(next);
         width = w; height = h;
-        rowBegin = 0; rowEnd = 0xffffffffu;
+        strip.ForgetRows();
         hasHistory = false;
         return ZR_OK;
     }
@@ -298,8 +299,7 @@ struct zr_auto_exposure_pass
             return ZR_ERR_INVALID_ARG;
         }
         const LumMap m{ params.min_lum, params.max_lum - params.min_lum, params.lum_map_exp };
-        const uint32_t y1 = rowEnd < height ? rowEnd : height;
-        const size_t begin = (size_t)rowBegin * width, end = (size_t)y1 * width;
+        const size_t begin = (size_t)strip.rowBegin * width, end = (size_t)strip.ClampedRowEnd(height) * width;
         const size_t chunk = (size_t)HIST_THREADS * HIST_UNROLL;
         const size_t blocksNeeded = (end - begin + chunk - 1) / chunk;
         const uint32_t blocks = (uint32_t)(blocksNeeded < maxBlocks ? blocksNeeded : maxBlocks);
@@ -328,7 +328,7 @@ struct zr_display_pass
     zr::Planes lutPlanes{ "zr_display_pass" };
     uint32_t* d_lut = nullptr;              // Tony McMapface, packed R9G9B9E5; NULL until set_lut
     zr_display_params params = Defaults();
-    uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
+    zr::StripRows strip{ "zr_display_pass" };
 
     static zr_display_params Defaults() { return zr_display_params{ ZR_TONEMAPPER_NEUTRAL, 1u, 1.0f, 1.0f }; }     // Display.cpp:70-74
     zr_status Setup() { return ZR_OK; }
@@ -339,7 +339,7 @@ struct zr_display_pass
         ZR_TRY(next.planes.Clear());
         sz = std::move(next);
         width = w; height = h;
-        rowBegin = 0; rowEnd = 0xffffffffu;
+        strip.ForgetRows();
         return ZR_OK;
     }
     zr_status SetLut(const uint32_t* h_lut, uint32_t dim)
@@ -388,8 +388,7 @@ struct zr_display_pass
             return ZR_ERR_INVALID_ARG;
         }
         const DisplayArgs a{ params.tonemapper, params.auto_exposure ? 1u : 0u, params.saturation, params.agx_exp };
-        const uint32_t y1 = rowEnd < height ? rowEnd : height;
-        const size_t begin = (size_t)rowBegin * width, end = (size_t)y1 * width;
+        const size_t begin = (size_t)strip.rowBegin * width, end = (size_t)strip.ClampedRowEnd(height) * width;
         ZR_PROF("k_display", stream);
         k_display<<<(uint32_t)((end - begin + 255) / 256), 256, 0, stream>>>((const uint2*)d_signal, (const float2*)d_exposure, d_lut,
             sz.d_out, begin, end, a);
@@ -422,12 +421,7 @@ extern "C"
         if (!p) return ZR_ERR_INVALID_ARG;
         return p->Render(in, d_signal, (cudaStream_t)stream);
     }
-    zr_status zr_auto_exposure_pass_set_rows(zr_auto_exposure_pass* p, uint32_t y0, uint32_t y1)
-    {
-        if (!p || y0 >= y1 || y0 >= p->height) { zr::set_error("zr_auto_exposure_pass_set_rows: empty row range"); return ZR_ERR_INVALID_ARG; }
-        p->rowBegin = y0; p->rowEnd = y1;
-        return ZR_OK;
-    }
+    zr_status zr_auto_exposure_pass_set_rows(zr_auto_exposure_pass* p, uint32_t y0, uint32_t y1) { return p ? p->strip.SetRows(y0, y1, p->height) : ZR_ERR_INVALID_ARG; }
     zr_status zr_auto_exposure_pass_set_reduce(zr_auto_exposure_pass* p, zr_reduce_u32_fn fn, void* user)
     {
         if (!p) return ZR_ERR_INVALID_ARG;
@@ -466,12 +460,7 @@ extern "C"
         if (!p) return ZR_ERR_INVALID_ARG;
         return p->Render(in, d_signal, d_exposure, (cudaStream_t)stream);
     }
-    zr_status zr_display_pass_set_rows(zr_display_pass* p, uint32_t y0, uint32_t y1)
-    {
-        if (!p || y0 >= y1 || y0 >= p->height) { zr::set_error("zr_display_pass_set_rows: empty row range"); return ZR_ERR_INVALID_ARG; }
-        p->rowBegin = y0; p->rowEnd = y1;
-        return ZR_OK;
-    }
+    zr_status zr_display_pass_set_rows(zr_display_pass* p, uint32_t y0, uint32_t y1) { return p ? p->strip.SetRows(y0, y1, p->height) : ZR_ERR_INVALID_ARG; }
     zr_status zr_display_pass_get_output(zr_display_pass* p, zr_image2d* out)
     {
         if (!p || !out) return ZR_ERR_INVALID_ARG;

@@ -11,6 +11,7 @@
 // place (the reference's in-place UAV update races with its own neighbour reads).
 #include "zr_common.cuh"
 #include "zr_planes.h"
+#include "zr_schedule.h"
 
 namespace zr
 {
@@ -330,12 +331,7 @@ struct zr_compositing_pass
         float4* d_composited = nullptr;     // output of compositing (fused with the firefly filter when it is on); never cleared
     } sz;
     zr_compositing_params params{ 1, 1, 1 };
-    uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
-    void SetRows(zr::PostParams& p, dim3& grid) const
-    {
-        p.rowBegin = rowBegin; p.rowEnd = rowEnd < height ? rowEnd : height;
-        grid = dim3((width + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8);
-    }
+    zr::StripRows strip{ "zr_compositing_pass" };
 
     zr_status Setup() { return ZR_OK; }
     zr_status OnWindowResized(uint32_t w, uint32_t h)
@@ -344,7 +340,7 @@ struct zr_compositing_pass
         ZR_TRY(next.planes.Alloc(next.d_composited, (size_t)w * h, false));
         sz = std::move(next);
         width = w; height = h;
-        rowBegin = 0; rowEnd = 0xffffffffu;
+        strip.ForgetRows();
         return ZR_OK;
     }
     zr_status Render(const zr_frame_inputs* in, const void* d_direct, const void* d_indirect, cudaStream_t stream)
@@ -360,8 +356,7 @@ struct zr_compositing_pass
         PostParams p = make_params(in->frame);
         const float4* direct = params.emissive_di ? (const float4*)d_direct : nullptr;
         const float4* indirect = params.indirect ? (const float4*)d_indirect : nullptr;
-        dim3 grid;
-        SetRows(p, grid);
+        p.rowBegin = strip.rowBegin; p.rowEnd = strip.ClampedRowEnd(height);
         if (params.firefly_filter)
         {
             const dim3 tgrid((width + FF_TW - 1) / FF_TW, (p.rowEnd - p.rowBegin + FF_TH - 1) / FF_TH);
@@ -373,6 +368,7 @@ struct zr_compositing_pass
         else
         {
             ZR_PROF("k_compositing", stream);
+            const dim3 grid((width + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8);
             k_compositing<<<grid, 256, 0, stream>>>((const uint4*)in->curr.d_core, direct, indirect, sz.d_composited, p);
             ZR_LAUNCH_CHECK();
         }
@@ -392,7 +388,7 @@ struct zr_taa_pass
     int outIdx = 0;
     bool isTemporalTexValid = false;
     float blendWeight = 0.1f;       // DefaultParamVals::BlendWeight
-    uint32_t rowBegin = 0, rowEnd = 0xffffffffu;
+    zr::StripRows strip{ "zr_taa_pass" };
 
     zr_status Setup() { return ZR_OK; }
     zr_status OnWindowResized(uint32_t w, uint32_t h)
@@ -402,7 +398,7 @@ struct zr_taa_pass
         ZR_TRY(next.planes.Clear());
         sz = std::move(next);
         width = w; height = h;
-        rowBegin = 0; rowEnd = 0xffffffffu;
+        strip.ForgetRows();
         isTemporalTexValid = false;
         return ZR_OK;
     }
@@ -419,7 +415,7 @@ struct zr_taa_pass
         PostParams p = make_params(in->frame);
         p.blendWeight = blendWeight;
         p.temporalIsValid = isTemporalTexValid ? 1u : 0u;
-        p.rowBegin = rowBegin; p.rowEnd = rowEnd < height ? rowEnd : height;
+        p.rowBegin = strip.rowBegin; p.rowEnd = strip.ClampedRowEnd(height);
         dim3 grid((width + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8);
         outIdx ^= 1;
         ZR_PROF("k_taa", stream);
@@ -447,12 +443,7 @@ extern "C"
         if (!p) return ZR_ERR_INVALID_ARG;
         return p->Render(in, d_direct, d_indirect, (cudaStream_t)stream);
     }
-    zr_status zr_compositing_pass_set_rows(zr_compositing_pass* p, uint32_t y0, uint32_t y1)
-    {
-        if (!p || y0 >= y1 || y0 >= p->height) { zr::set_error("zr_compositing_pass_set_rows: empty row range"); return ZR_ERR_INVALID_ARG; }
-        p->rowBegin = y0; p->rowEnd = y1;
-        return ZR_OK;
-    }
+    zr_status zr_compositing_pass_set_rows(zr_compositing_pass* p, uint32_t y0, uint32_t y1) { return p ? p->strip.SetRows(y0, y1, p->height) : ZR_ERR_INVALID_ARG; }
     zr_status zr_compositing_pass_get_output(zr_compositing_pass* p, zr_image2d* out)
     {
         if (!p || !out) return ZR_ERR_INVALID_ARG;
@@ -463,12 +454,7 @@ extern "C"
 
     zr_status zr_taa_pass_create(uint32_t width, uint32_t height, zr_taa_pass** out) { return zr::CreatePass("zr_taa_pass", width, height, out); }
     zr_status zr_taa_pass_resize(zr_taa_pass* p, uint32_t width, uint32_t height) { return zr::ResizePass("zr_taa_pass", p, width, height); }
-    zr_status zr_taa_pass_set_rows(zr_taa_pass* p, uint32_t y0, uint32_t y1)
-    {
-        if (!p || y0 >= y1 || y0 >= p->height) { zr::set_error("zr_taa_pass_set_rows: empty row range"); return ZR_ERR_INVALID_ARG; }
-        p->rowBegin = y0; p->rowEnd = y1;
-        return ZR_OK;
-    }
+    zr_status zr_taa_pass_set_rows(zr_taa_pass* p, uint32_t y0, uint32_t y1) { return p ? p->strip.SetRows(y0, y1, p->height) : ZR_ERR_INVALID_ARG; }
     zr_status zr_taa_pass_set_blend_weight(zr_taa_pass* p, float w)
     {
         if (!p) return ZR_ERR_INVALID_ARG;

@@ -64,34 +64,36 @@ struct zr_renderer
         if (s != ZR_OK) r->hookStatus = s;
     }
 
-    // the GI pass object is created lazily (first SetMethod): it follows the renderer's current strip
-    zr_status ApplyShardToGI()
+    // Applies the current strip to every pass that exists: zr_renderer_set_shard, and the entry points that create the GI, SVGF and
+    // display passes (possibly after the cut). Sharded, each pass gets the rows it computes and its hook; otherwise the whole frame
+    // and no hook. Re-applying unchanged rows and hooks rebuilds nothing.
+    zr_status ApplyShard()
     {
-        if (!gi) return ZR_OK;
-        const bool sharded = comm && world > 1;
-        zr_status s = sharded ? zr_gi_pass_set_rows(gi, bounds[rank], bounds[rank + 1]) : zr_gi_pass_set_rows(gi, 0, height);
-        if (s == ZR_OK) s = zr_gi_pass_set_halo_exchange(gi, sharded ? HaloHook : nullptr, &hookMain);
-        return s;
-    }
-
-    // the SVGF pass is created by zr_renderer_set_denoiser, possibly after the cut: it follows the renderer's current strip
-    zr_status ApplyShardToSVGF()
-    {
-        if (!svgf) return ZR_OK;
-        const bool sharded = comm && world > 1;
-        zr_status s = sharded ? zr_svgf_pass_set_rows(svgf, bounds[rank], bounds[rank + 1]) : zr_svgf_pass_set_rows(svgf, 0, height);
-        if (s == ZR_OK) s = zr_svgf_pass_set_halo_exchange(svgf, sharded ? HaloHook : nullptr, &hookMain);
-        return s;
-    }
-
-    zr_status ApplyShardToDisplay()
-    {
-        if (!ae) return ZR_OK;
         const bool sharded = comm && world > 1;
         const uint32_t y0 = sharded ? bounds[rank] : 0, y1 = sharded ? bounds[rank + 1] : height;
-        zr_status s = zr_auto_exposure_pass_set_rows(ae, y0, y1);
-        if (s == ZR_OK) s = zr_auto_exposure_pass_set_reduce(ae, sharded ? ReduceHook : nullptr, this);
-        if (s == ZR_OK) s = zr_display_pass_set_rows(display, y0, y1);
+        zr_halo_exchange_fn hook = sharded ? HaloHook : nullptr;
+        // the G-buffer halo is re-rendered locally; the TAA neighbourhood reads the composited signal one row beyond the strip
+        zr_status s = zr_gbuffer_pass_set_rows(gbufferPass, y0 > HALO ? y0 - HALO : 0, y1 + HALO < height ? y1 + HALO : height);
+        if (s == ZR_OK) s = zr_direct_pass_set_rows(direct, y0, y1);
+        if (s == ZR_OK) s = zr_indirect_pass_set_rows(indirect, y0, y1);
+        if (s == ZR_OK) s = zr_compositing_pass_set_rows(compositing, y0 > 0 ? y0 - 1 : 0, y1 + 1 < height ? y1 + 1 : height);
+        if (s == ZR_OK) s = zr_taa_pass_set_rows(taa, y0, y1);
+        if (s == ZR_OK) s = zr_direct_pass_set_halo_exchange(direct, hook, &hookSide);
+        if (s == ZR_OK) s = zr_indirect_pass_set_halo_exchange(indirect, hook, &hookMain);
+        if (s == ZR_OK && gi) s = zr_gi_pass_set_rows(gi, y0, y1);
+        if (s == ZR_OK && gi) s = zr_gi_pass_set_halo_exchange(gi, hook, &hookMain);
+        if (s == ZR_OK && svgf) s = zr_svgf_pass_set_rows(svgf, y0, y1);
+        if (s == ZR_OK && svgf) s = zr_svgf_pass_set_halo_exchange(svgf, hook, &hookMain);
+        if (s == ZR_OK && ae) s = zr_auto_exposure_pass_set_rows(ae, y0, y1);
+        if (s == ZR_OK && ae) s = zr_auto_exposure_pass_set_reduce(ae, sharded ? ReduceHook : nullptr, this);
+        if (s == ZR_OK && display) s = zr_display_pass_set_rows(display, y0, y1);
+        return s;
+    }
+    // an error a hook met during the stage that just ran; reported once
+    zr_status TakeHookStatus()
+    {
+        const zr_status s = hookStatus;
+        hookStatus = ZR_OK;
         return s;
     }
     void ReleaseDisplay()
@@ -202,7 +204,8 @@ extern "C"
             ZR_CUDA(cudaEventRecord(r->evDirect, r->side));
             ZR_CUDA(cudaStreamWaitEvent(stream, r->evDirect, 0));
         }
-        if (r->hookStatus != ZR_OK) { s = r->hookStatus; r->hookStatus = ZR_OK; return s; }
+        s = r->TakeHookStatus();
+        if (s != ZR_OK) return s;
         zr_image2d di, ind, comp;
         s = zr_direct_pass_get_output(r->direct, ZR_DIRECT_FINAL, &di);
         if (s != ZR_OK) return s;
@@ -226,7 +229,8 @@ extern "C"
         {
             s = zr_svgf_pass_render(r->svgf, &in, comp.d_ptr, stream);
             if (s != ZR_OK) return s;
-            if (r->hookStatus != ZR_OK) { s = r->hookStatus; r->hookStatus = ZR_OK; return s; }
+            s = r->TakeHookStatus();
+            if (s != ZR_OK) return s;
             s = zr_svgf_pass_get_output(r->svgf, ZR_SVGF_DENOISED, &comp);
             if (s != ZR_OK) return s;
         }
@@ -235,7 +239,8 @@ extern "C"
         {
             s = zr_auto_exposure_pass_render(r->ae, &in, comp.d_ptr, stream);
             if (s != ZR_OK) return s;
-            if (r->hookStatus != ZR_OK) { s = r->hookStatus; r->hookStatus = ZR_OK; return s; }
+            s = r->TakeHookStatus();
+            if (s != ZR_OK) return s;
             s = zr_auto_exposure_pass_get_output(r->ae, &exposure);
             if (s != ZR_OK) return s;
         }
@@ -281,7 +286,7 @@ extern "C"
             if (!r->gi) s = zr_gi_pass_create(r->width, r->height, &r->gi);
             else s = zr_gi_pass_reset_temporal(r->gi);
             if (s == ZR_OK) s = zr_gi_pass_set_method(r->gi, method);
-            if (s == ZR_OK) s = r->ApplyShardToGI();
+            if (s == ZR_OK) s = r->ApplyShard();
         }
         else
             s = zr_indirect_pass_reset_temporal(r->indirect);
@@ -297,7 +302,7 @@ extern "C"
         if (enable && !r->svgf)
         {
             s = zr_svgf_pass_create(r->width, r->height, &r->svgf);
-            if (s == ZR_OK) s = r->ApplyShardToSVGF();
+            if (s == ZR_OK) s = r->ApplyShard();
             if (s != ZR_OK && r->svgf) { zr_svgf_pass_destroy(r->svgf); r->svgf = nullptr; }
         }
         if (!enable && r->svgf) { zr_svgf_pass_destroy(r->svgf); r->svgf = nullptr; }
@@ -313,7 +318,7 @@ extern "C"
         {
             s = zr_auto_exposure_pass_create(r->width, r->height, &r->ae);
             if (s == ZR_OK) s = zr_display_pass_create(r->width, r->height, &r->display);
-            if (s == ZR_OK) s = r->ApplyShardToDisplay();
+            if (s == ZR_OK) s = r->ApplyShard();
             if (s != ZR_OK) r->ReleaseDisplay();
         }
         if (!enable) r->ReleaseDisplay();
@@ -330,25 +335,14 @@ extern "C"
     zr_status zr_renderer_set_shard(zr_renderer* r, zr_comm* comm, const uint32_t* bounds, int gather_output)
     {
         if (!r) return ZR_ERR_INVALID_ARG;
-        zr_status s = ZR_OK;
         if (!comm)
         {
             r->comm = nullptr; r->world = 1; r->rank = 0; r->bounds.clear();
-            s = zr_gbuffer_pass_set_rows(r->gbufferPass, 0, r->height);
-            if (s == ZR_OK) s = zr_direct_pass_set_rows(r->direct, 0, r->height);
-            if (s == ZR_OK) s = zr_indirect_pass_set_rows(r->indirect, 0, r->height);
-            if (s == ZR_OK) s = zr_compositing_pass_set_rows(r->compositing, 0, r->height);
-            if (s == ZR_OK) s = zr_taa_pass_set_rows(r->taa, 0, r->height);
-            if (s == ZR_OK) s = zr_direct_pass_set_halo_exchange(r->direct, nullptr, nullptr);
-            if (s == ZR_OK) s = zr_indirect_pass_set_halo_exchange(r->indirect, nullptr, nullptr);
-            if (s == ZR_OK) s = r->ApplyShardToGI();
-            if (s == ZR_OK) s = r->ApplyShardToSVGF();
-            if (s == ZR_OK) s = r->ApplyShardToDisplay();
-            return s;
+            return r->ApplyShard();
         }
         if (!bounds) { zr::set_error("zr_renderer_set_shard: bounds missing"); return ZR_ERR_INVALID_ARG; }
         int rank = 0, world = 1;
-        s = zr_comm_rank(comm, &rank, &world);
+        zr_status s = zr_comm_rank(comm, &rank, &world);
         if (s != ZR_OK) return s;
         if (bounds[0] != 0 || bounds[world] != r->height) { zr::set_error("zr_renderer_set_shard: bounds must cover [0, height)"); return ZR_ERR_INVALID_ARG; }
         for (int q = 0; q < world; q++)
@@ -359,20 +353,7 @@ extern "C"
             }
         r->comm = comm; r->rank = rank; r->world = world; r->gatherOutput = gather_output != 0;
         r->bounds.assign(bounds, bounds + world + 1);
-        const uint32_t y0 = bounds[rank], y1 = bounds[rank + 1], H = r->height;
-        const uint32_t g0 = y0 > zr_renderer::HALO ? y0 - zr_renderer::HALO : 0, g1 = y1 + zr_renderer::HALO < H ? y1 + zr_renderer::HALO : H;
-        s = zr_gbuffer_pass_set_rows(r->gbufferPass, g0, g1);            // the G-buffer halo is re-rendered locally
-        if (s == ZR_OK) s = zr_direct_pass_set_rows(r->direct, y0, y1);
-        if (s == ZR_OK) s = zr_indirect_pass_set_rows(r->indirect, y0, y1);
-        // the TAA neighbourhood reads the composited signal one row beyond the strip
-        if (s == ZR_OK) s = zr_compositing_pass_set_rows(r->compositing, y0 > 0 ? y0 - 1 : 0, y1 + 1 < H ? y1 + 1 : H);
-        if (s == ZR_OK) s = zr_taa_pass_set_rows(r->taa, y0, y1);
-        if (s == ZR_OK) s = zr_direct_pass_set_halo_exchange(r->direct, world > 1 ? zr_renderer::HaloHook : nullptr, &r->hookSide);
-        if (s == ZR_OK) s = zr_indirect_pass_set_halo_exchange(r->indirect, world > 1 ? zr_renderer::HaloHook : nullptr, &r->hookMain);
-        if (s == ZR_OK) s = r->ApplyShardToGI();
-        if (s == ZR_OK) s = r->ApplyShardToSVGF();
-        if (s == ZR_OK) s = r->ApplyShardToDisplay();
-        return s;
+        return r->ApplyShard();
     }
     zr_status zr_renderer_get_gi_pass(zr_renderer* r, zr_gi_pass** gi)
     {
