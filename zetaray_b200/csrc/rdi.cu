@@ -18,23 +18,44 @@ namespace zr
 {
 namespace
 {
-// 512 threads at 128 registers: on an H100 SXM (700 W) k_di_temporal + k_di_spatial take 1.30 + 0.73 ms per bench frame, against
-// 1.55 + 1.01 at 1024 x 64 registers, 1.32 + 0.92 at 768 x 80 and 1.44 + 0.93 at 512 x 2 blocks x 64 (DESIGN 4.1). Swept before the plain material build existed; both builds use this shape.
-#ifndef ZR_RDI_THREADS
-#define ZR_RDI_THREADS 512
+// Block sizes: k_di_temporal 768 threads at 80 registers with its reservoir parked in shared memory (below), k_di_spatial 512 at
+// 128. Measured on an H100 SXM (700 W, 1980 MHz), ms per bench frame: k_di_temporal 1.013 at 768 x 80 parked, 1.078 at 512 x 128
+// parked, 1.099 at 512 x 128 unparked (the previous shape); k_di_spatial 0.632 at 512 x 128, 0.644 with its reservoirs and
+// neighbour list parked, 0.763 parked at 768 x 80, so it is not parked (DESIGN 4.1, item 2). Both material builds use these
+// shapes. A block is always whole 8x8 groups (threads / 64 of them), the unit of the group RNG and the disocclusion vote.
+#ifndef ZR_RDI_TEMPORAL_THREADS
+#define ZR_RDI_TEMPORAL_THREADS 768
 #endif
-    // ReSTIR_DI_Temporal.hlsl main + EstimateDirectLighting. A block is ZR_RDI_THREADS/64 consecutive 8x8 groups of the
+#ifndef ZR_RDI_SPATIAL_THREADS
+#define ZR_RDI_SPATIAL_THREADS 512
+#endif
+    static_assert(ZR_RDI_TEMPORAL_THREADS % 64 == 0 && ZR_RDI_SPATIAL_THREADS % 64 == 0, "a DI block is whole 8x8 groups");
+    // k_di_temporal's RIS reservoir: only reservoir updates and the MIS tails touch it, yet it crosses the roughly 20 barriers of
+    // RIS_InitialCandidates_Sync and TemporalResample1_Sync. It lives in dynamic shared memory, one record per thread, as
+    // k_pathtrace's PtParked does. Reservoir's float2 makes the record a multiple of 8 bytes, so its stride cannot be an odd number
+    // of words; 2 mod 4 words is the next best: the 32 lanes of a warp fall in 16 different banks, two per bank.
+    struct DiTemporalParked
+    {
+        Reservoir r;
+        uint32_t pad[2];
+    };
+    static_assert(sizeof(DiTemporalParked) % 16 == 8, "DiTemporalParked must be 2 mod 4 words");
+    constexpr size_t DI_TEMPORAL_SMEM_BYTES = (size_t)ZR_RDI_TEMPORAL_THREADS * sizeof(DiTemporalParked);
+
+    // ReSTIR_DI_Temporal.hlsl main + EstimateDirectLighting. A block is ZR_RDI_TEMPORAL_THREADS/64 consecutive 8x8 groups of the
     // reference's swizzled dispatch, walking the resampling phases together (no thread leaves before the last barrier).
     // MF: the material features the kernel is compiled for (BSDF::ShadingDataT); the scene's materials must use no others.
+    // Dynamic shared memory: DI_TEMPORAL_SMEM_BYTES.
     template<uint32_t MF>
-    __global__ void ZR_LB(ZR_RDI_THREADS) k_di_temporal(SceneDev sc, FrameView f, DIParams prm, zr_rdi_reservoir* __restrict__ resCurr,
+    __global__ void ZR_LB(ZR_RDI_TEMPORAL_THREADS) k_di_temporal(SceneDev sc, FrameView f, DIParams prm, zr_rdi_reservoir* __restrict__ resCurr,
         const zr_rdi_reservoir* __restrict__ resPrev, uint2* __restrict__ target, float4* __restrict__ finalImg, uint32_t dispX, uint32_t dispY,
         const uint32_t* __restrict__ order)
     {
         using SD = BSDF::ShadingDataT<MF>;
+        extern __shared__ DiTemporalParked s_diTemporalParked[];
         const zr_frame_constants& fc = f.fc;
         uint2 sg = make_uint2(0, 0);
-        const uint32_t groupFlat = order[blockIdx.x] * (ZR_RDI_THREADS / 64) + (threadIdx.x >> 6);
+        const uint32_t groupFlat = order[blockIdx.x] * (ZR_RDI_TEMPORAL_THREADS / 64) + (threadIdx.x >> 6);
         const uint32_t tInGroup = threadIdx.x & 63;
         uint2 px = make_uint2(0xffffffffu, 0xffffffffu);
         if (groupFlat < dispX * dispY)
@@ -72,7 +93,8 @@ namespace
         // group-uniform index so that every thread of an 8x8 group uses the same presampled set (ReSTIR_DI_Temporal.hlsl:368-370)
         RNG rng_group = RNG::Init(groupFlat % dispX, groupFlat / dispX, fc.FrameNum);
         const uint32_t sampleSetIdx = rng_group.UniformUintBounded_Faster(sc.numSampleSets);
-        Reservoir r = RIS_InitialCandidates_Sync(act, sc, p.pos, p.normal, p.roughness, p.surface, sampleSetIdx, numBsdfSamples, rng_thread);
+        Reservoir& r = s_diTemporalParked[threadIdx.x].r;
+        RIS_InitialCandidates_Sync(r, act, sc, p.pos, p.normal, p.roughness, p.surface, sampleSetIdx, numBsdfSamples, rng_thread);
         if (prm.temporal)
         {
             float2 motionVec = f2(0, 0);
@@ -110,14 +132,14 @@ namespace
 
     // ReSTIR_DI_Spatial.hlsl main + SpatialResample
     template<uint32_t MF>
-    __global__ void ZR_LB(ZR_RDI_THREADS) k_di_spatial(SceneDev sc, FrameView f, DIParams prm, const zr_rdi_reservoir* __restrict__ resCurr,
+    __global__ void ZR_LB(ZR_RDI_SPATIAL_THREADS) k_di_spatial(SceneDev sc, FrameView f, DIParams prm, const zr_rdi_reservoir* __restrict__ resCurr,
         const uint2* __restrict__ target, float4* __restrict__ finalImg, uint32_t dispX, uint32_t dispY,
         const uint32_t* __restrict__ order)
     {
         using SD = BSDF::ShadingDataT<MF>;
         const zr_frame_constants& fc = f.fc;
         uint2 sg = make_uint2(0, 0);
-        const uint32_t groupFlat = order[blockIdx.x] * (ZR_RDI_THREADS / 64) + (threadIdx.x >> 6);
+        const uint32_t groupFlat = order[blockIdx.x] * (ZR_RDI_SPATIAL_THREADS / 64) + (threadIdx.x >> 6);
         const uint32_t tInGroup = threadIdx.x & 63;
         uint2 px = make_uint2(0xffffffffu, 0xffffffffu);
         if (groupFlat < dispX * dispY)
@@ -258,7 +280,7 @@ struct zr_direct_pass
     bool resetTemporalTextures = true;
     bool patternLoaded = false;
     zr_direct_params params = Defaults();
-    zr::LightingStrip strip{ "zr_direct_pass" };     // both kernels share the 8x8-group block schedule
+    zr::LightingStrip strip{ "zr_direct_pass" };     // sched[0]: k_di_temporal, sched[1]: k_di_spatial (8x8-group blocks)
 
     static zr_direct_params Defaults()
     {
@@ -268,7 +290,14 @@ struct zr_direct_pass
         p.M_max = 20; p.alpha_min = 0.05f * 0.05f;
         return p;
     }
-    zr_status Setup() { return ZR_OK; }
+    zr_status Setup()
+    {
+        // both material-feature builds, whichever scenes the pass will render
+        using zr::BSDF::MF_NONE; using zr::BSDF::MF_ALL;
+        ZR_TRY(zr::ReserveParkedSmem(zr::k_di_temporal<MF_NONE>, ZR_RDI_TEMPORAL_THREADS, zr::DI_TEMPORAL_SMEM_BYTES, "zr_direct_pass: k_di_temporal"));
+        ZR_TRY(zr::ReserveParkedSmem(zr::k_di_temporal<MF_ALL>, ZR_RDI_TEMPORAL_THREADS, zr::DI_TEMPORAL_SMEM_BYTES, "zr_direct_pass: k_di_temporal"));
+        return ZR_OK;
+    }
     zr_status OnWindowResized(uint32_t w, uint32_t h)
     {
         const size_t n = (size_t)w * h;
@@ -319,19 +348,23 @@ struct zr_direct_pass
             params.alpha_min, resetTemporalTextures, strip.rowBegin, strip.ClampedRowEnd(height), strip.d_costMap };
         const uint32_t dispX = (width + 7) / 8, dispY = (height + 7) / 8;
         const int cur = currTemporalIdx;
-        st = strip.Schedule(width, height, 8, 8, ZR_RDI_THREADS / 64);
+        // the two kernels have different block sizes, so each has its own block table
+        st = strip.Schedule(width, height, 8, 8, ZR_RDI_TEMPORAL_THREADS / 64, 0);
         if (st != ZR_OK) return st;
-        const BlockSchedule& sched = strip.sched;
+        st = strip.Schedule(width, height, 8, 8, ZR_RDI_SPATIAL_THREADS / 64, 1);
+        if (st != ZR_OK) return st;
+        const BlockSchedule& schedT = strip.sched[0];
+        const BlockSchedule& schedS = strip.sched[1];
         const bool plain = (in->scene->materialFeatures & BSDF::MF_ALL) == 0;
         ZR_PROF("k_di_temporal", stream);
-        (plain ? k_di_temporal<BSDF::MF_NONE> : k_di_temporal<BSDF::MF_ALL>)<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, dispX, dispY, sched.d_order);
+        (plain ? k_di_temporal<BSDF::MF_NONE> : k_di_temporal<BSDF::MF_ALL>)<<<schedT.count, ZR_RDI_TEMPORAL_THREADS, DI_TEMPORAL_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, dispX, dispY, schedT.d_order);
         ZR_LAUNCH_CHECK();
         // the temporal output is what neighbours read in the spatial pass and what the next frame reprojects into
         strip.Exchange(sz.d_res[cur], width, height, 32u, stream);
         if (doSpatial)
         {
             ZR_PROF("k_di_spatial", stream);
-            (plain ? k_di_spatial<BSDF::MF_NONE> : k_di_spatial<BSDF::MF_ALL>)<<<sched.count, ZR_RDI_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY, sched.d_order);
+            (plain ? k_di_spatial<BSDF::MF_NONE> : k_di_spatial<BSDF::MF_ALL>)<<<schedS.count, ZR_RDI_SPATIAL_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY, schedS.d_order);
             ZR_LAUNCH_CHECK();
         }
         isTemporalReservoirValid = true;

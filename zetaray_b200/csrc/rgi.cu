@@ -352,7 +352,7 @@ struct zr_gi_pass
         const uint32_t dispX = (width + 7) / 8, dispY = (height + 7) / 8;
         st = strip.Schedule(width, height, 8, 8, ZR_RGI_THREADS / 64);
         if (st != ZR_OK) return st;
-        const BlockSchedule& sched = strip.sched;
+        const BlockSchedule& sched = strip.sched[0];
         const int cur = currTemporalIdx;
         if (plainPathTracer)
         {

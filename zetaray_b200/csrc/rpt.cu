@@ -558,25 +558,11 @@ struct zr_indirect_pass
 
     zr_status Setup()
     {
-        // k_pathtrace's parked state needs more than the 48 KB of static shared memory. The carveout asks for just the shared
-        // memory its resident blocks use (plus the 1 KB the system reserves per block); the rest of the 256 KB stays L1 for
-        // what still spills.
-        // Both material-feature builds are set up, whichever scenes the pass will render.
+        // k_pathtrace's parked state needs more than the 48 KB of static shared memory. Both material-feature builds are set up,
+        // whichever scenes the pass will render.
         decltype(&zr::k_pathtrace<zr::BSDF::MF_ALL>) const kernels[2] = { zr::k_pathtrace<zr::BSDF::MF_NONE>, zr::k_pathtrace<zr::BSDF::MF_ALL> };
         for (const auto kernel : kernels)
-        {
-            ZR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zr::PT_SMEM_BYTES));
-            int ptBlocks = 0;
-            ZR_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ptBlocks, kernel, ZR_PT_THREADS, zr::PT_SMEM_BYTES));
-            if (ptBlocks < 1)
-            {
-                zr::set_error("zr_indirect_pass: k_pathtrace (%d threads, %zu B shared) cannot be resident", ZR_PT_THREADS, zr::PT_SMEM_BYTES);
-                return ZR_ERR_UNSUPPORTED;
-            }
-            const size_t ptSmem = (size_t)ptBlocks * (zr::PT_SMEM_BYTES + 1024);
-            ZR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                (int)((ptSmem * 100 + 228 * 1024 - 1) / (228 * 1024))));
-        }
+            ZR_TRY(zr::ReserveParkedSmem(kernel, ZR_PT_THREADS, zr::PT_SMEM_BYTES, "zr_indirect_pass: k_pathtrace"));
         return shiftStreams.Init();
     }
 
@@ -648,8 +634,8 @@ struct zr_indirect_pass
         const uint32_t dispX = (width + 15) / 16, dispY = (height + 7) / 8;
         const bool plain = (in->scene->materialFeatures & BSDF::MF_ALL) == 0;
         ZR_PROF("k_pathtrace", stream);
-        (plain ? k_pathtrace<BSDF::MF_NONE> : k_pathtrace<BSDF::MF_ALL>)<<<strip.sched.count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY,
-            strip.sched.d_order);
+        (plain ? k_pathtrace<BSDF::MF_NONE> : k_pathtrace<BSDF::MF_ALL>)<<<strip.sched[0].count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY,
+            strip.sched[0].d_order);
         ZR_LAUNCH_CHECK();
         if (doTemporal)
         {

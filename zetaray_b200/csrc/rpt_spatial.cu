@@ -327,6 +327,8 @@ zr_status ShiftStreams::Init()
     ZR_CUDA(cudaGetDevice(&dev));
     ZR_CUDA(cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev));
     ZR_CUDA(cudaFuncSetAttribute(k_spatial_merge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MergeSmem)));
+    ZR_TRY(SetupShifts<false>());
+    ZR_TRY(SetupTemporalShifts());
     for (int i = 0; i < 2; i++)
     {
         ZR_CUDA(cudaStreamCreateWithFlags(&aux[i], cudaStreamNonBlocking));

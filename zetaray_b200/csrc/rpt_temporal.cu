@@ -185,6 +185,11 @@ namespace
     }
 }
 
+zr_status SetupTemporalShifts()
+{
+    return SetupShifts<true>();
+}
+
 zr_status SpatialQueued::RunTemporal(const ShiftStreams& ss, const SceneDev& sc, const FrameView& f, const RptParams& prm, zr_rpt_reservoir* resCurr,
     const zr_rpt_reservoir* resPrev, float4* target, float4* finalImg, bool plain, cudaStream_t stream)
 {

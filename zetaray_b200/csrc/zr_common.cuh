@@ -52,6 +52,24 @@ void count_launch(uint64_t n = 1);
 // right after the call can neither be overwritten by a late memset nor overwrite an early one. These are rare host calls.
 #define ZR_CLEAR_BEGIN() ZR_CUDA(cudaDeviceSynchronize())
 #define ZR_CLEAR_END() ZR_CUDA(cudaStreamSynchronize(cudaStreamLegacy))
+// For a kernel that parks per-thread state in `bytes` of dynamic shared memory per block: raises its limit to `bytes` and asks for a
+// carveout of just the shared memory its resident blocks use (plus the 1 KB the system reserves per block), so that the rest of
+// the 256 KB stays L1 for what still spills. `what` names the kernel in the error of a shape that cannot be resident.
+template<class Kernel>
+zr_status ReserveParkedSmem(Kernel kernel, int threads, size_t bytes, const char* what)
+{
+    ZR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    int blocks = 0;
+    ZR_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kernel, threads, bytes));
+    if (blocks < 1)
+    {
+        set_error("%s (%d threads, %zu B shared) cannot be resident", what, threads, bytes);
+        return ZR_ERR_UNSUPPORTED;
+    }
+    const size_t smem = (size_t)blocks * (bytes + 1024);
+    ZR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)((smem * 100 + 228 * 1024 - 1) / (228 * 1024))));
+    return ZR_OK;
+}
 void prof_before(const char* name, cudaStream_t stream);
 void prof_after();
 #define ZR_PROF(name, stream) zr::prof_before(name, (cudaStream_t)(stream))

@@ -148,11 +148,12 @@ struct EmissiveData
 // RIS over BSDF and light samples (Resampling.hlsli:116-331) as block-synchronous phases (zr_rpt.cuh): every
 // thread of the block walks the same 2 + 3 sample slots, `act` / the per-pixel sample counts predicate the work.
 #define ZR_PHASE() __syncthreads()
+// The result is built in `r`, which may live in shared memory (k_di_temporal parks it there).
 template<class SD>
-ZR_D Reservoir RIS_InitialCandidates_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, float roughness, SD surface,
+ZR_D void RIS_InitialCandidates_Sync(Reservoir& r, bool act, const SceneDev& sc, float3 pos, float3 normal, float roughness, SD surface,
     uint32_t sampleSetIdx, int numBsdfSamples, RNG& rng)
 {
-    Reservoir r = Reservoir::Init();
+    r = Reservoir::Init();
     const bool specular = surface.GlossSpecular() && (surface.metallic || surface.specTr) && (!surface.Coated() || surface.CoatSpecular());
     const int numLightSamples = !specular ? 3 : 0;
     for (int s_b = 0; s_b < 2; s_b++)
@@ -253,6 +254,14 @@ ZR_D Reservoir RIS_InitialCandidates_Sync(bool act, const SceneDev& sc, float3 p
     }
     float targetLum = Math::Luminance(r.target);
     r.W = targetLum > 0.0f ? r.w_sum / targetLum : 0.0f;
+}
+// The same, returning the reservoir (the host build of the device source in tests/hostsim calls this form).
+template<class SD>
+ZR_D Reservoir RIS_InitialCandidates_Sync(bool act, const SceneDev& sc, float3 pos, float3 normal, float roughness, SD surface,
+    uint32_t sampleSetIdx, int numBsdfSamples, RNG& rng)
+{
+    Reservoir r;
+    RIS_InitialCandidates_Sync(r, act, sc, pos, normal, roughness, surface, sampleSetIdx, numBsdfSamples, rng);
     return r;
 }
 

@@ -3,10 +3,12 @@
 // (zr_rpt.cuh Replay_kGt2_Sync / Shift2_Sync<CASE>) on real work. Used by the spatial pass (rpt_spatial.cu: current <-> neighbour
 // pixel of the same frame) and by the temporal pass (rpt_temporal.cu: current <-> reprojected pixel of the previous frame).
 //
-// Block size: 512 threads x 1 block per SM (128 registers). At 64 registers the replay classes spill ~1 KB per thread, more
-// than L1 holds at a full SM. Measured on an H100 SXM (700 W), spatial + temporal shift per bench frame: 0.88 + 0.78 ms at
-// 512 x 1, 0.87 + 0.85 at 768 x 1 (80 registers), 0.96 + 0.83 at 512 x 2 (64 registers), 0.99 + 0.87 at 1024 x 1 (DESIGN 4.1).
-// Swept before the plain material build existed; both builds use this shape.
+// Block size: 768 threads x 1 block per SM (80 registers), with the reconnection parked in shared memory (ShiftParked, 69 KB per
+// block). Measured on an H100 SXM (700 W, 1980 MHz), spatial + temporal shift per bench frame (plain material build), all shapes
+// parked: 0.676 + 0.661 ms at 768 x 1, 0.660 + 0.640 at 384 x 2 (80 registers), 0.651 + 0.683 at 512 x 2 (64 registers), 0.755 +
+// 0.685 at 512 x 1 (128 registers); the previous shape, 512 x 1 unparked, 0.744 + 0.678. The two-block shapes are no faster than
+// 768 x 1 on the bench frame beyond its run-to-run spread, and slower on the full material build (tunnel 4K), so both builds use
+// 768 x 1 (DESIGN 4.1, item 2).
 #pragma once
 #include "zr_rpt_spatial.h"
 
@@ -16,13 +18,24 @@ namespace
 {
     using namespace RPT;
 #ifndef ZR_SHIFT_THREADS
-#define ZR_SHIFT_THREADS 512
+#define ZR_SHIFT_THREADS 768
 #endif
 #ifndef ZR_SHIFT_MINBLOCKS
 #define ZR_SHIFT_MINBLOCKS 1
 #endif
     constexpr int SHIFT_THREADS = ZR_SHIFT_THREADS, SHIFT_MINBLOCKS = ZR_SHIFT_MINBLOCKS;
     constexpr uint32_t NO_ITEM = 0xffffffffu;
+
+    // The sample's reconnection: every phase of the shift reads it, nothing after the claim writes it. Held in registers it crossed
+    // every phase barrier and spilled; it lives in dynamic shared memory instead, one record per thread, as k_pathtrace's PtParked
+    // does. The record's odd number of 32-bit words puts the 32 lanes of a warp in 32 different banks.
+    struct ShiftParked
+    {
+        Reconnection rc;
+        uint32_t pad;
+    };
+    static_assert(sizeof(ShiftParked) % 4 == 0 && (sizeof(ShiftParked) / 4) % 2 == 1, "ShiftParked must be an odd number of words");
+    constexpr size_t SHIFT_SMEM_BYTES = (size_t)SHIFT_THREADS * sizeof(ShiftParked);
 
     // queue class of a reservoir's sample from its metadata word: (case 1, 2, 3) x (k == 2, k > 2)
     ZR_D uint32_t ShiftClass(uint32_t meta)
@@ -36,6 +49,7 @@ namespace
 
     // item = x | y << 16 | flag << 30 | direction << 31 (x < 65536, y < 16384); flag: temporal pass only, "the tighter plane test
     // of the replay passed" (ReSTIR_PT_Replay.hlsl:404). MF: the material features the kernel is compiled for (BSDF::ShadingDataT).
+    // Dynamic shared memory: SHIFT_SMEM_BYTES (ShiftParked per thread).
     template<int CASE, bool REPLAY, bool TEMPORAL, uint32_t MF>
     __global__ void __launch_bounds__(SHIFT_THREADS, SHIFT_MINBLOCKS) k_shift(SceneDev sc, FrameView f, RptParams prm,
         const zr_rpt_reservoir* __restrict__ resIn, const zr_rpt_reservoir* __restrict__ resPrev, const uint16_t* __restrict__ neighbor,
@@ -43,6 +57,8 @@ namespace
     {
         using SD = BSDF::ShadingDataT<MF>;
         __shared__ uint32_t s_base;
+        extern __shared__ ShiftParked s_shiftParked[];
+        Reconnection& rc = s_shiftParked[threadIdx.x].rc;
         const uint32_t total = counters[cls];
         for (;;)
         {
@@ -55,7 +71,6 @@ namespace
             int x = 0, y = 0;
             uint32_t dir = 0;
             bool replayOk = act;
-            Reservoir r = Reservoir::Init();
             PixelT<SD> p, pr;
             if (act)
             {
@@ -69,9 +84,10 @@ namespace
                     int nx = 0, ny = 0;
                     NeighborOf(f, neighbor, x, y, nx, ny);
                     LoadRecord(dir == 0 ? &resIn[(size_t)y * f.W + x] : &resIn[(size_t)ny * f.W + nx], rec);
-                    r = Reservoir::Load_NonReconnection(rec);
+                    Reservoir r = Reservoir::Load_NonReconnection(rec);
                     r.rc.x_k_in_motion = false;
                     r.Load_Reconnection(rec);
+                    rc = r.rc;
                     if (dir == 0) p = LoadPixel<SD>(f, sc, f.core, f.coat, nx, ny, false, x, y);
                     else p = LoadPixel<SD>(f, sc, f.core, f.coat, x, y, false, x, y);
                     if (REPLAY)
@@ -88,27 +104,30 @@ namespace
                     int ppx = 0, ppy = 0;
                     PrevPixel(f, x, y, ppx, ppy);
                     LoadRecord(dir == 0 ? &resIn[(size_t)y * f.W + x] : &resPrev[(size_t)ppy * f.W + ppx], rec);
-                    r = Reservoir::Load_NonReconnection(rec);
+                    Reservoir r = Reservoir::Load_NonReconnection(rec);
                     r.Load_Reconnection(rec);
                     if (r.rc.IsCase1() || r.rc.IsCase2())
                     {
                         if (dir == 0) XkToPrev(sc, r.rc);
                         else XkToCurr(sc, r.rc);
                     }
+                    rc = r.rc;
                     if (dir == 0) p = LoadPixel<SD>(f, sc, f.pcore, f.pcoat, ppx, ppy, true, x, y);
                     else p = LoadPixel<SD>(f, sc, f.core, f.coat, x, y, false, x, y);
                     if (REPLAY) pr = p;
                 }
             }
+            else
+                rc = Reconnection::Init();
             OffsetPathContextT<SD> ctx = OffsetPathContextT<SD>::Init();
             if (REPLAY)
             {
                 ZR_PHASE();
-                ctx = Replay_kGt2_Sync(act && replayOk, sc, pr.pos, pr.normal, pr.eta_next, pr.surface, r.rc, prm.alpha_min);
+                ctx = Replay_kGt2_Sync(act && replayOk, sc, pr.pos, pr.normal, pr.eta_next, pr.surface, rc, prm.alpha_min);
                 if (act && replayOk)
                     ctx = ctx.Quantize();
             }
-            const OffsetPath shift = Shift2_Sync<CASE>(act, sc, p.pos, p.normal, p.eta_next, p.surface, r.rc, &ctx, prm.alpha_min);
+            const OffsetPath shift = Shift2_Sync<CASE>(act, sc, p.pos, p.normal, p.eta_next, p.surface, rc, &ctx, prm.alpha_min);
             if (act)
             {
                 ShiftResult* o = &out[(size_t)y * f.W + x];
@@ -143,7 +162,7 @@ namespace
         ZR_CUDA(cudaStreamWaitEvent(s1, ss.evFork, 0));
         ZR_CUDA(cudaStreamWaitEvent(s2, ss.evFork, 0));
 #define ZR_LAUNCH_SHIFT(CASE, REPLAY, CLS, STREAM) \
-        (plain ? k_shift<CASE, REPLAY, TEMPORAL, BSDF::MF_NONE> : k_shift<CASE, REPLAY, TEMPORAL, BSDF::MF_ALL>)<<<grid, SHIFT_THREADS, 0, STREAM>>>(sc, f, prm, resIn, resPrev, neighbor, q.d_queue + (size_t)(CLS) * q.capacity, \
+        (plain ? k_shift<CASE, REPLAY, TEMPORAL, BSDF::MF_NONE> : k_shift<CASE, REPLAY, TEMPORAL, BSDF::MF_ALL>)<<<grid, SHIFT_THREADS, SHIFT_SMEM_BYTES, STREAM>>>(sc, f, prm, resIn, resPrev, neighbor, q.d_queue + (size_t)(CLS) * q.capacity, \
             q.d_counters, CLS, q.d_shift); \
         zr::count_launch()
         ZR_LAUNCH_SHIFT(1, false, 0, stream);
@@ -157,6 +176,22 @@ namespace
         ZR_CUDA(cudaEventRecord(ss.evJoin[1], s2));
         ZR_CUDA(cudaStreamWaitEvent(stream, ss.evJoin[0], 0));
         ZR_CUDA(cudaStreamWaitEvent(stream, ss.evJoin[1], 0));
+        return ZR_OK;
+    }
+
+    // Sets the shared-memory limit and carveout of the pass's twelve shift kernels (six classes x two material builds); once, from
+    // ShiftStreams::Init.
+    template<bool TEMPORAL>
+    zr_status SetupShifts()
+    {
+        using BSDF::MF_NONE; using BSDF::MF_ALL;
+        decltype(&k_shift<1, false, TEMPORAL, MF_ALL>) const kernels[12] = {
+            k_shift<1, false, TEMPORAL, MF_NONE>, k_shift<2, false, TEMPORAL, MF_NONE>, k_shift<3, false, TEMPORAL, MF_NONE>,
+            k_shift<1, true, TEMPORAL, MF_NONE>, k_shift<2, true, TEMPORAL, MF_NONE>, k_shift<3, true, TEMPORAL, MF_NONE>,
+            k_shift<1, false, TEMPORAL, MF_ALL>, k_shift<2, false, TEMPORAL, MF_ALL>, k_shift<3, false, TEMPORAL, MF_ALL>,
+            k_shift<1, true, TEMPORAL, MF_ALL>, k_shift<2, true, TEMPORAL, MF_ALL>, k_shift<3, true, TEMPORAL, MF_ALL> };
+        for (const auto kernel : kernels)
+            ZR_TRY(ReserveParkedSmem(kernel, SHIFT_THREADS, SHIFT_SMEM_BYTES, "zr_indirect_pass: k_shift"));
         return ZR_OK;
     }
 

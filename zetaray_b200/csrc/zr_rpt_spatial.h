@@ -39,8 +39,10 @@ struct ShiftStreams
     ShiftStreams(const ShiftStreams&) = delete;
     ShiftStreams& operator=(const ShiftStreams&) = delete;
     ~ShiftStreams();
-    zr_status Init();
+    zr_status Init();       // also sets up the shift kernels of both passes (SetupShifts in zr_rpt_shift.cuh)
 };
+// SetupShifts<true>: the temporal pass's shift kernels are instantiated in rpt_temporal.cu
+zr_status SetupTemporalShifts();
 
 // The queues, shift results and tensor maps of one frame size. Temporal reuse runs through the same queues, counters and shift-result
 // plane (the two passes never overlap in a frame).

@@ -155,7 +155,7 @@ struct LightingStrip : StripRows
 {
     unsigned long long* d_costMap = nullptr;
     TileCosts tileCosts;
-    BlockSchedule sched;
+    BlockSchedule sched[2];     // one block table per block shape; a pass whose kernels have two shapes uses both
 
     explicit LightingStrip(const char* passName) : StripRows(passName) {}
     // after a resize: the rows, cost map, tile costs and block table described the old frame; the halo hook stays
@@ -164,7 +164,8 @@ struct LightingStrip : StripRows
         ForgetRows();
         d_costMap = nullptr;
         tileCosts = TileCosts{};
-        sched.Release();
+        sched[0].Release();
+        sched[1].Release();
     }
     zr_status SetCostMap(void* d_cycles)
     {
@@ -184,13 +185,14 @@ struct LightingStrip : StripRows
         tileCosts.version++;
         return ZR_OK;
     }
-    // sched for a kernel whose blocks are groupsPerBlock swizzled groups of groupW x groupH pixels; the table is rebuilt and
+    // sched[shape] for a kernel whose blocks are groupsPerBlock swizzled groups of groupW x groupH pixels; the table is rebuilt and
     // uploaded only when the rows or the tile costs changed
-    zr_status Schedule(uint32_t width, uint32_t height, uint32_t groupW, uint32_t groupH, uint32_t groupsPerBlock)
+    zr_status Schedule(uint32_t width, uint32_t height, uint32_t groupW, uint32_t groupH, uint32_t groupsPerBlock, int shape = 0)
     {
         const uint32_t y0 = rowBegin, y1 = ClampedRowEnd(height), v = tileCosts.version;
-        if (!sched.UpToDate(y0, y1, v))
-            ZR_CUDA(sched.Upload(ScheduleSwizzled((width + groupW - 1) / groupW, (height + groupH - 1) / groupH, groupW, groupH, groupsPerBlock,
+        BlockSchedule& s = sched[shape];
+        if (!s.UpToDate(y0, y1, v))
+            ZR_CUDA(s.Upload(ScheduleSwizzled((width + groupW - 1) / groupW, (height + groupH - 1) / groupH, groupW, groupH, groupsPerBlock,
                 y0, y1, tileCosts), y0, y1, v));
         return ZR_OK;
     }
