@@ -52,7 +52,8 @@ ZR_API const char* zr_last_error(void);
  * measurement and test hooks: the ReSTIR PT execution-model switch and the two-dispatch compositing entry point. 1.4 removed
  * the stage-limited ReSTIR PT render and its stage enum, which nothing called. 1.6 added the AutoExposure and Display passes,
  * zr_renderer_set_display / get_display_output and zr_comm_allreduce_u32. 1.7 added zr_comm_create_transport (zr_comm_transport). 1.8
- * added zr_svgf_pass_set_rows / set_halo_exchange, and zr_renderer_set_shard runs the SVGF stage sharded instead of refusing it. */
+ * added zr_svgf_pass_set_rows / set_halo_exchange, and zr_renderer_set_shard runs the SVGF stage sharded instead of refusing it. 1.9
+ * added zr_scene_update_materials and zr_scene_get_tables. */
 ZR_API uint32_t zr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -309,12 +310,41 @@ ZR_API zr_status zr_scene_create(const zr_scene_desc* desc, zr_scene** out);
 ZR_API void zr_scene_destroy(zr_scene* scene);
 /* BVH statistics for tests: {num_nodes, num_tris, max_depth, bytes}. */
 ZR_API zr_status zr_scene_bvh_stats(const zr_scene* scene, uint32_t out[4]);
-/* The optional BSDF features the scene's materials use: the OR over its material table, fixed at zr_scene_create. The
- * lighting passes run kernels built without clear coat, specular transmission and thin-walled transmission when none is set. */
+/* The optional BSDF features the scene's materials use: the OR over its material table as zr_scene_create or the last
+ * zr_scene_update_materials left it. The lighting passes read it on every render and run kernels built without clear coat,
+ * specular transmission and thin-walled transmission when none is set. */
 #define ZR_MATERIAL_COAT         0x1u   /* coat weight > 0 */
 #define ZR_MATERIAL_TRANSMISSION 0x2u   /* transmissive flag (bit 26 of CoatColor_Flags) */
 #define ZR_MATERIAL_THIN_WALLED  0x4u   /* thin-walled flag (bit 29 of CoatColor_Flags) with subsurface weight > 0 */
 ZR_API zr_status zr_scene_material_features(const zr_scene* scene, uint32_t* out);
+
+/* Scene edit between frames (SceneCore::UpdateMaterial / UpdateEmissiveMaterial, SceneCore.cpp:436, 711-715): replaces materials
+ * [first, first + count) of the scene's table. The scene's geometry, instances, BVH and its set of emissive triangles are unchanged.
+ *  - Refusals (ZR_ERR_INVALID_ARG, zr_last_error names the rule) are decided on the host before any work, and leave the material
+ *    table, the emissive triangles, the power estimate, the alias table and zr_scene_material_features as they were: a NULL scene or
+ *    h_materials, count == 0, first + count > the number of materials; an edit that gives a material a non-zero emissive factor
+ *    where it had none while an instance using it has no emissive triangles (BaseEmissiveTriOffset == 0xffffffff); and, in a scene
+ *    with emissive triangles, an edit after which every instance with emissive triangles uses a material of zero emissive factor
+ *    or zero strength (the light distribution cannot be normalised over zero power). A light whose factor goes to zero keeps its
+ *    triangles in the emissive set, with zero power.
+ *  - Ordering: the material copy waits for the frames in flight (like every host-side replacement of data a frame reads), the
+ *    rest is enqueued on `stream`: the next render on `stream` sees the edited scene, and no earlier frame does.
+ *  - The emissive triangles of the instances whose material's emissive factor, double-sided flag or strength changed take the new
+ *    bits on the device (k_refresh_emissives: PackedA's factor, double-sided and strength bits, PackedB's strength); positions,
+ *    UVs, IDs and the id-patched bit stay. When any did and zr_prelighting_render has run before, the call runs it again on
+ *    `stream` (power estimate + alias build), so the next frame samples the new distribution; an edit that changes no emissive
+ *    bits launches no kernel. Presampled sets and the light voxel grid are redrawn every frame and need nothing.
+ *  - The material features are recomputed over the whole table; the next render picks its kernel build from them.
+ *  - History is left alone, as the reference leaves it: ReSTIR DI / PT / GI reservoirs that cached the old radiance age out through
+ *    their M caps. To restart accumulation, render the next frame with CameraStatic = 0 and NumFramesCameraStatic = 0
+ *    (DefaultRenderer.cpp:96-102 after SceneModified), or reset a pass's temporal history.
+ *  - Strip-sharded frames: every rank makes the same call with the same materials; the work is deterministic, so every rank's
+ *    tables end identical. */
+ZR_API zr_status zr_scene_update_materials(zr_scene* scene, uint32_t first, uint32_t count, const zr_material* h_materials,
+    void* stream);
+/* The scene's device material table and emissive triangles (read-only; valid until zr_scene_destroy). */
+ZR_API zr_status zr_scene_get_tables(const zr_scene* scene, const zr_material** d_materials, uint32_t* num_materials,
+    const zr_emissive_tri** d_emissives, uint32_t* num_emissives);
 
 /* The BVH builder alone, on host memory (no GPU needed): world-space triangles as 9 floats {v0, e1, e2} in, 80-byte
  * nodes and the leaf-order permutation out (either may be NULL to query sizes). out_info = {num_nodes, num_tris,

@@ -57,6 +57,7 @@ class FrameSequence:
         self.cam_path, self.accumulate = cam_path, accumulate
         self.prev_cam = None
         self.static_frames = 0
+        self.scene_changed_pending = False
 
     def next(self):
         self.frame += 1
@@ -72,7 +73,18 @@ class FrameSequence:
                                                prev_cam=self.prev_cam or cam)
             self.prev_cam = cam
         if self.accumulate:
-            self.static_frames += 1
-            fc.Accumulate, fc.CameraStatic, fc.NumFramesCameraStatic = 1, 1, self.static_frames
+            if self.scene_changed_pending:
+                self.static_frames = 0
+                fc.Accumulate, fc.CameraStatic, fc.NumFramesCameraStatic = 1, 0, 0
+            else:
+                self.static_frames += 1
+                fc.Accumulate, fc.CameraStatic, fc.NumFramesCameraStatic = 1, 1, self.static_frames
+        self.scene_changed_pending = False
         self.prev_jitter = j
         return fc
+
+    def scene_changed(self):
+        """DefaultRenderer::SceneModified (DefaultRenderer.cpp:96-102, 553-556): the next frame says CameraStatic = 0 and
+        NumFramesCameraStatic = 0, so accumulation starts over from the frame after it. Call it after an edit such as
+        Scene.update_materials."""
+        self.scene_changed_pending = True

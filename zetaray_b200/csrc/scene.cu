@@ -41,6 +41,37 @@ namespace
         o[6] = e2.x; o[7] = e2.y; o[8] = e2.z;
     }
 
+    // The emissive triangles [first[r], first[r] + start[r + 1] - start[r]) of range r take the material-derived bits packedA[r] /
+    // packedB[r] (emissive_bits). One job holds up to EDIT_RANGES ranges; it travels as a kernel parameter, so an edit needs no device
+    // allocation.
+    constexpr uint32_t EDIT_RANGES = 96;
+    struct EmissiveRefresh
+    {
+        uint32_t numRanges;
+        uint32_t start[EDIT_RANGES + 1];    // exclusive prefix sum of the range lengths: thread t belongs to the r with start[r] <= t < start[r + 1]
+        uint32_t first[EDIT_RANGES];
+        uint32_t packedA[EDIT_RANGES];
+        uint32_t packedB[EDIT_RANGES];
+    };
+    // PackedA bits the material sets: the emissive factor [0, 24), double sided (25) and the strength's low 4 bits [28, 32). The
+    // id-patched bit (24) and bits 26-27 are the triangle's own; PackedB keeps its texture index [0, 16).
+    constexpr uint32_t EMISSIVE_A_MATERIAL_BITS = 0xffffffu | (1u << 25) | (0xfu << 28);
+
+    __global__ void k_refresh_emissives(const __grid_constant__ EmissiveRefresh job, zr_emissive_tri* __restrict__ emissives)
+    {
+        const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+        if (t >= job.start[job.numRanges]) return;
+        uint32_t lo = 0, hi = job.numRanges - 1;
+        while (lo < hi)
+        {
+            const uint32_t mid = (lo + hi + 1) >> 1;
+            if (job.start[mid] <= t) lo = mid; else hi = mid - 1;
+        }
+        zr_emissive_tri& e = emissives[job.first[lo] + (t - job.start[lo])];
+        e.PackedA = (e.PackedA & ~EMISSIVE_A_MATERIAL_BITS) | job.packedA[lo];
+        e.PackedB = (e.PackedB & 0xffffu) | job.packedB[lo];
+    }
+
     __global__ void k_trace_closest(SceneDev sc, const float* __restrict__ rays, uint32_t n, float* __restrict__ hits)
     {
         const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -58,6 +89,34 @@ namespace
         const float* r = rays + (size_t)i * 8;
         flags[i] = TraceAnyExcept(sc, f3(r[0], r[1], r[2]), f3(r[4], r[5], r[6]), r[3], r[7], 0xffffffffu) ? 1u : 0u;
     }
+}
+
+// The optional BSDF features a material table uses. The per-pixel coat / transmissive / subsurface bits of the G-buffer and the
+// surfaces built at path vertices come from these material fields alone (no textures or instance overrides in this build), read as
+// Mat::GetCoatWeight, Mat::Transmissive and Mat::ThinWalled ? Mat::GetSubsurface : 0 do.
+static uint32_t material_features(const zr_material* mats, size_t n)
+{
+    uint32_t f = 0;
+    for (size_t i = 0; i < n; i++)
+    {
+        const zr_material& m = mats[i];
+        if ((m.BaseColorTex_Subsurf_CoatWeight >> 24) & 0xff) f |= ZR_MATERIAL_COAT;
+        if (m.CoatColor_Flags & (1u << 26)) f |= ZR_MATERIAL_TRANSMISSION;
+        if ((m.CoatColor_Flags & (1u << 29)) && ((m.BaseColorTex_Subsurf_CoatWeight >> 16) & 0xff)) f |= ZR_MATERIAL_THIN_WALLED;
+    }
+    return f;
+}
+
+static uint32_t emissive_factor(const zr_material& m) { return m.EmissiveFactor_NormalScale & 0xffffffu; }
+static uint32_t emissive_strength(const zr_material& m) { return m.EmissiveStrength_IOR & 0xffffu; }      // half bits
+
+// The bits an emissive triangle takes from its instance's material, as RT::EmissiveTriangle's constructor stores them (the factor,
+// the double-sided flag and the strength, whose low 4 bits also go to PackedA[28, 32)).
+static void emissive_bits(const zr_material& m, uint32_t& packedA, uint32_t& packedB)
+{
+    const uint32_t strength = emissive_strength(m);
+    packedA = emissive_factor(m) | (m.CoatColor_Flags & (1u << 25)) | ((strength & 0xfu) << 28);
+    packedB = strength << 16;
 }
 
 template<typename T>
@@ -125,17 +184,12 @@ zr_status scene_create(const zr_scene_desc* desc, zr_scene** out)
     UP(emissives, desc->h_emissives, desc->num_emissives);
     sc->dev.numInstances = desc->num_instances;
     sc->dev.numEmissives = desc->num_emissives;
-    // The per-pixel coat / transmissive / subsurface bits of the G-buffer and the surfaces built at path vertices come from these
-    // material fields alone (no textures or instance overrides in this build), read as Mat::GetCoatWeight, Mat::Transmissive and
-    // Mat::ThinWalled ? Mat::GetSubsurface : 0 do.
-    for (uint32_t i = 0; i < desc->num_materials; i++)
-    {
-        const zr_material& m = desc->h_materials[i];
-        if ((m.BaseColorTex_Subsurf_CoatWeight >> 24) & 0xff) sc->materialFeatures |= ZR_MATERIAL_COAT;
-        if (m.CoatColor_Flags & (1u << 26)) sc->materialFeatures |= ZR_MATERIAL_TRANSMISSION;
-        if ((m.CoatColor_Flags & (1u << 29)) && ((m.BaseColorTex_Subsurf_CoatWeight >> 16) & 0xff))
-            sc->materialFeatures |= ZR_MATERIAL_THIN_WALLED;
-    }
+    sc->materialFeatures = material_features(desc->h_materials, desc->num_materials);
+    sc->hostMaterials.assign(desc->h_materials, desc->h_materials + desc->num_materials);
+    sc->hostInstances.resize(desc->num_instances);
+    for (uint32_t m = 0; m < desc->num_instances; m++)
+        sc->hostInstances[m] = SceneHostInstance{ desc->h_instances[m].MatIdx, desc->h_instances[m].BaseEmissiveTriOffset,
+            desc->h_instance_num_tris[m] };
 
     // triangle -> mesh maps
     std::vector<uint32_t> triMesh, meshFirst(desc->num_instances);
@@ -220,6 +274,94 @@ zr_status scene_create(const zr_scene_desc* desc, zr_scene** out)
     *out = sc;
     return ZR_OK;
 }
+
+zr_status scene_update_materials(zr_scene* sc, uint32_t first, uint32_t count, const zr_material* h, cudaStream_t stream)
+{
+    // Every refusal happens here, before anything on the host or the device changes.
+    if (!sc || !h || count == 0)
+    {
+        set_error("zr_scene_update_materials: null scene or materials, or count == 0");
+        return ZR_ERR_INVALID_ARG;
+    }
+    const uint32_t numMaterials = (uint32_t)sc->hostMaterials.size();
+    if ((uint64_t)first + count > numMaterials)
+    {
+        set_error("zr_scene_update_materials: materials [%u, %llu) lie past the %u materials of the scene", first,
+            (unsigned long long)first + count, numMaterials);
+        return ZR_ERR_INVALID_ARG;
+    }
+    std::vector<zr_material> next(sc->hostMaterials);
+    std::copy(h, h + count, next.begin() + first);
+    bool anyPower = false, anyEmissiveInstance = false;
+    for (uint32_t m = 0; m < (uint32_t)sc->hostInstances.size(); m++)
+    {
+        const SceneHostInstance& in = sc->hostInstances[m];
+        const zr_material& mat = next[in.matIdx];
+        const bool hasEmissives = in.baseEmissiveTri != 0xffffffffu && in.numTris != 0;
+        if (!hasEmissives && emissive_factor(mat) != 0 && emissive_factor(sc->hostMaterials[in.matIdx]) == 0)
+        {
+            set_error("zr_scene_update_materials: material %u becomes emissive, but instance %u, which uses it, has no emissive "
+                "triangles (the emissive set is fixed at zr_scene_create)", (unsigned)in.matIdx, m);
+            return ZR_ERR_INVALID_ARG;
+        }
+        if (hasEmissives)
+        {
+            anyEmissiveInstance = true;
+            anyPower |= emissive_factor(mat) != 0 && (emissive_strength(mat) & 0x7fffu) != 0;
+        }
+    }
+    if (sc->dev.numEmissives && anyEmissiveInstance && !anyPower)
+    {
+        set_error("zr_scene_update_materials: the edit leaves every emissive triangle with a zero emissive factor or strength; the "
+            "light distribution cannot be normalised over zero power");
+        return ZR_ERR_INVALID_ARG;
+    }
+
+    // The emissive triangles whose bits change: those of the instances whose material's factor, double-sided flag or strength the
+    // edit changes. Consecutive triangles that take the same bits form one range.
+    std::vector<uint32_t> rFirst, rCount, rA, rB;
+    for (const SceneHostInstance& in : sc->hostInstances)
+    {
+        if (in.baseEmissiveTri == 0xffffffffu || in.numTris == 0 || in.matIdx < first || in.matIdx >= first + count) continue;
+        uint32_t a, b, a0, b0;
+        emissive_bits(next[in.matIdx], a, b);
+        emissive_bits(sc->hostMaterials[in.matIdx], a0, b0);
+        if (a == a0 && b == b0) continue;
+        if (!rFirst.empty() && rFirst.back() + rCount.back() == in.baseEmissiveTri && rA.back() == a && rB.back() == b)
+            rCount.back() += in.numTris;
+        else
+        {
+            rFirst.push_back(in.baseEmissiveTri); rCount.push_back(in.numTris); rA.push_back(a); rB.push_back(b);
+        }
+    }
+
+    ZR_CLEAR_BEGIN();       // a frame still in flight may read the old materials
+    ZR_CUDA(cudaMemcpy(const_cast<zr_material*>(sc->dev.materials) + first, h, (size_t)count * sizeof(zr_material), cudaMemcpyHostToDevice));
+    ZR_CLEAR_END();
+    sc->hostMaterials.swap(next);
+    sc->materialFeatures = material_features(sc->hostMaterials.data(), sc->hostMaterials.size());
+
+    zr_emissive_tri* emissives = const_cast<zr_emissive_tri*>(sc->dev.emissives);
+    for (size_t r0 = 0; r0 < rFirst.size(); r0 += EDIT_RANGES)
+    {
+        EmissiveRefresh job;
+        job.numRanges = (uint32_t)std::min<size_t>(EDIT_RANGES, rFirst.size() - r0);
+        job.start[0] = 0;
+        for (uint32_t r = 0; r < job.numRanges; r++)
+        {
+            job.first[r] = rFirst[r0 + r]; job.packedA[r] = rA[r0 + r]; job.packedB[r] = rB[r0 + r];
+            job.start[r + 1] = job.start[r] + rCount[r0 + r];       // <= numEmissives < 2^32 (checked at create)
+        }
+        const uint32_t n = job.start[job.numRanges];
+        ZR_PROF("k_refresh_emissives", stream);
+        k_refresh_emissives<<<(n + 255) / 256, 256, 0, stream>>>(job, emissives);
+        ZR_LAUNCH_CHECK();
+    }
+    // The next frame samples the new light distribution. Before the first zr_prelighting_render there is none to rebuild.
+    if (!rFirst.empty() && sc->aliasBuilt)
+        return zr_prelighting_render(sc, stream);
+    return ZR_OK;
+}
 } // namespace zr
 
 extern "C"
@@ -249,6 +391,18 @@ extern "C"
             memcpy(h_nodes, w.nodes.data(), w.nodes.size() * sizeof(zr::BVH8Node));
         }
         if (h_leaf_order) memcpy(h_leaf_order, w.leafOrder.data(), (size_t)num_tris * sizeof(uint32_t));
+        return ZR_OK;
+    }
+    zr_status zr_scene_update_materials(zr_scene* sc, uint32_t first, uint32_t count, const zr_material* h_materials, void* stream)
+    {
+        return zr::scene_update_materials(sc, first, count, h_materials, (cudaStream_t)stream);
+    }
+    zr_status zr_scene_get_tables(const zr_scene* sc, const zr_material** d_materials, uint32_t* num_materials,
+        const zr_emissive_tri** d_emissives, uint32_t* num_emissives)
+    {
+        if (!sc || !d_materials || !num_materials || !d_emissives || !num_emissives) return ZR_ERR_INVALID_ARG;
+        *d_materials = sc->dev.materials; *num_materials = (uint32_t)sc->hostMaterials.size();
+        *d_emissives = sc->dev.emissives; *num_emissives = sc->dev.numEmissives;
         return ZR_OK;
     }
     zr_status zr_scene_bvh_stats(const zr_scene* sc, uint32_t out[4])

@@ -12,6 +12,7 @@
 #pragma once
 #include "zr_common.cuh"
 #include "zr_bvh.h"
+#include <vector>
 
 namespace zr
 {
@@ -299,6 +300,8 @@ ZR_D VertexD LoadVertex(const SceneDev& sc, uint32_t idx)
 
 // host side (scene.cu)
 struct SceneHostInfo { uint32_t numNodes, numTris, maxDepth, bytes, maxStack; };
+// What zr_scene_update_materials needs of an instance to refuse an edit and to find the emissive triangles it refreshes
+struct SceneHostInstance { uint32_t matIdx, baseEmissiveTri, numTris; };
 } // namespace zr
 
 struct zr_scene
@@ -315,5 +318,7 @@ struct zr_scene
     bool samplesValid = false;      // zr_presample_emissives ran since the sets were (re)configured
     zr_voxel_sample* d_lvg = nullptr;
     bool lvgValid = false;          // zr_build_light_voxel_grid ran since the grid was (re)configured
-    uint32_t materialFeatures = 0;  // ZR_MATERIAL_* over the material table (zr_scene_create); materials never change afterwards
+    uint32_t materialFeatures = 0;  // ZR_MATERIAL_* over the material table (zr_scene_create, zr_scene_update_materials)
+    std::vector<zr_material> hostMaterials;                 // the device material table as last uploaded
+    std::vector<zr::SceneHostInstance> hostInstances;       // fixed at zr_scene_create
 };

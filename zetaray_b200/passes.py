@@ -7,6 +7,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import lib, check
+from .scene import EMISSIVE_TRI, MATERIAL
 
 
 def _vp(a):
@@ -45,6 +46,25 @@ class Scene:
         out = (C.c_uint32 * 4)()
         check(lib.zr_scene_bvh_stats(self.handle, out))
         return dict(nodes=out[0], tris=out[1], max_depth=out[2], bytes=out[3])
+
+    def material_features(self):
+        """ZR_MATERIAL_* bits of the current material table."""
+        out = C.c_uint32()
+        check(lib.zr_scene_material_features(self.handle, C.byref(out)))
+        return out.value
+
+    def update_materials(self, first, materials, stream=None):
+        """Replaces materials [first, first + len(materials)) between frames (zr_scene_update_materials): the emissive triangles
+        of changed lights take the new factor / strength on the device and the alias table is rebuilt on `stream`. Geometry,
+        instances and the emissive set stay; scene.update_materials applies the same edit to a FlatScene."""
+        m = np.ascontiguousarray(np.asarray(materials, dtype=MATERIAL).reshape(-1))
+        check(lib.zr_scene_update_materials(self.handle, int(first), len(m), _vp(m), stream))
+
+    def tables(self):
+        """(materials, emissive triangles) as the device holds them."""
+        dm, nm, de, ne = C.c_void_p(), C.c_uint32(), C.c_void_p(), C.c_uint32()
+        check(lib.zr_scene_get_tables(self.handle, C.byref(dm), C.byref(nm), C.byref(de), C.byref(ne)))
+        return _d2h((np.zeros(nm.value, dtype=MATERIAL), dm), (np.zeros(ne.value, dtype=EMISSIVE_TRI), de))
 
     def prelighting(self, stream=None):
         check(lib.zr_prelighting_render(self.handle, stream))

@@ -211,6 +211,46 @@ class FlatScene:
         return int(self.instance_num_tris.sum())
 
 
+EMISSIVE_A_MATERIAL_BITS = 0xffffff | (1 << 25) | (0xf << 28)     # the PackedA bits emissive_triangle takes from the material
+
+
+def update_materials(flat, first, materials):
+    """zr_scene_update_materials on host arrays: a copy of `flat` whose materials [first, first + len(materials)) are replaced
+    and whose emissive triangles of the instances using them carry the re-derived factor, double-sided flag and strength, as
+    emissive_triangle stores them. Geometry, instances and the emissive set stay. Raises ValueError where the library refuses
+    the edit: a material that becomes emissive while an instance using it has no emissive triangles, or an edit that leaves
+    every emissive triangle with zero factor or strength."""
+    materials = np.asarray(materials, dtype=MATERIAL).reshape(-1)
+    if len(materials) == 0 or first < 0 or first + len(materials) > len(flat.materials):
+        raise ValueError("materials [%d, %d) of %d" % (first, first + len(materials), len(flat.materials)))
+    out = FlatScene()
+    out.vertices, out.indices, out.instances, out.instance_num_tris = flat.vertices, flat.indices, flat.instances, flat.instance_num_tris
+    out.materials = flat.materials.copy()
+    out.materials[first:first + len(materials)] = materials
+    out.emissives = flat.emissives.copy()
+    factor = lambda m: int(m["EmissiveFactor_NormalScale"]) & 0xffffff
+    strength = lambda m: int(m["EmissiveStrength_IOR"]) & 0xffff
+    bits = lambda m: (factor(m) | (int(m["CoatColor_Flags"]) & (1 << 25)) | ((strength(m) & 0xf) << 28), strength(m) << 16)
+    powered = lit = False
+    for m, (inst, nt) in enumerate(zip(flat.instances, flat.instance_num_tris)):
+        mi, base = int(inst["MatIdx"]), int(inst["BaseEmissiveTriOffset"])
+        old, new = flat.materials[mi], out.materials[mi]
+        if base == 0xffffffff or nt == 0:
+            if factor(new) and not factor(old):
+                raise ValueError("material %d becomes emissive, but instance %d, which uses it, has no emissive triangles" % (mi, m))
+            continue
+        lit = True
+        powered |= bool(factor(new)) and (strength(new) & 0x7fff) != 0
+        if bits(new) != bits(old):      # the library rewrites the triangles of changed lights only
+            e = out.emissives[base:base + nt]
+            a, b = bits(new)
+            e["PackedA"] = (e["PackedA"] & np.uint32(~EMISSIVE_A_MATERIAL_BITS & 0xffffffff)) | np.uint32(a)
+            e["PackedB"] = (e["PackedB"] & np.uint32(0xffff)) | np.uint32(b)
+    if len(flat.emissives) and lit and not powered:
+        raise ValueError("the edit leaves every emissive triangle with zero emissive factor or strength")
+    return out
+
+
 class SceneBuilder:
     """Programmatic scene assembly (also used for the synthetic 'Sponza-class' / 'Subway-class' scenes)."""
 
