@@ -741,8 +741,9 @@ ZR_API zr_status zr_comm_allreduce_u32(zr_comm* c, int which_comm, uint32_t* d_v
 /* ---- The frame (ZetaRenderer/Default: DefaultRenderer.cpp:304-520, PathTracer.cpp:149-563) ----
  * Owns the double-buffered G-buffers and one object of every pass and runs a frame in the reference's order:
  * (frame 1: emissive power + alias table) -> presampling if enabled -> GBufferRT -> DirectLighting || IndirectLighting
- * -> Compositing + firefly filter -> TAA. DirectLighting is recorded on an internal second stream when two_streams != 0
- * (the two lighting passes are independent render-graph nodes in the reference). Parameters are set on the pass handles. */
+ * -> Compositing + firefly filter -> TAA. When two_streams != 0, GBufferRT and IndirectLighting run on an internal stream of the
+ * greatest priority and DirectLighting on an internal second stream of the least (the two lighting passes are independent
+ * render-graph nodes in the reference); both join the caller's stream before Compositing. Parameters are set on the pass handles. */
 typedef struct zr_renderer zr_renderer;
 typedef struct zr_renderer_desc { uint32_t width, height; int with_tridiff; int two_streams; } zr_renderer_desc;
 ZR_API zr_status zr_renderer_create(const zr_renderer_desc* desc, zr_scene* scene, zr_renderer** out);

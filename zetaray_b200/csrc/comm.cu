@@ -62,7 +62,7 @@ namespace
 struct zr_comm
 {
     int rank = 0, world = 1;
-    NcclComm comm[2] = { nullptr, nullptr };       // [0] main stream, [1] second stream (DirectLighting): never shared between streams
+    NcclComm comm[2] = { nullptr, nullptr };       // [0] main streams, [1] second stream (DirectLighting): never used by two streams at once
     zr_comm_transport transport{};                  // set (and comm[] unused) for a comm made by zr_comm_create_transport
     void* user = nullptr;
     uint64_t bytesSent = 0, calls = 0;

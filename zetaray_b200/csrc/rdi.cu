@@ -18,18 +18,40 @@ namespace zr
 {
 namespace
 {
-// Block sizes: k_di_temporal 768 threads at 80 registers with its reservoir parked in shared memory (below), k_di_spatial 512 at
-// 128. Measured on an H100 SXM (700 W, 1980 MHz), ms per bench frame: k_di_temporal 1.013 at 768 x 80 parked, 1.078 at 512 x 128
-// parked, 1.099 at 512 x 128 unparked (the previous shape); k_di_spatial 0.632 at 512 x 128, 0.644 with its reservoirs and
-// neighbour list parked, 0.763 parked at 768 x 80, so it is not parked (DESIGN 4.1, item 2). Both material builds use these
-// shapes. A block is always whole 8x8 groups (threads / 64 of them), the unit of the group RNG and the disocclusion vote.
+// Block sizes and register bounds: k_di_temporal 384 threads at 80 registers with its reservoir parked in shared memory (below),
+// k_di_spatial 256 at 128; two blocks per SM each. Measured on an H100 SXM (700 W, 1980 MHz), ms per bench frame, at one block per SM:
+// k_di_temporal 1.013 at 768 x 80 parked, 1.078 at 512 x 128 parked, 1.099 at 512 x 128 unparked; k_di_spatial 0.632 at 512 x 128,
+// 0.644 with its reservoirs and neighbour list parked, 0.763 parked at 768 x 80, so it is not parked (DESIGN 4.1, item 2).
+// In the renderer's frame DirectLighting runs at the least stream priority in the SM time that IndirectLighting leaves idle
+// (renderer.cu). A DI block that takes an SM there holds it to its end while the chain's next kernel waits, so smaller blocks were
+// measured at the same register bounds and the same threads per SM: bench.py's ms per frame, and the kernels' ms from its single-stream
+// pass, medians of three runs in each of three sessions (A, B, C), builds alternating within a session:
+//
+//   temporal x spatial threads   frame   k_di_temporal   k_di_spatial   session
+//   768 x 512 (previous)         6.394   1.020           0.636          A
+//   384 x 512                    6.350   0.973           0.636          A
+//   256 x 512                    6.345   1.072           0.634          A
+//   768 x 256                    6.329   1.015           0.594          A
+//   768 x 512 (previous)         6.367   1.015           0.634          B
+//   384 x 256                    6.291   0.979           0.595          B
+//   384 x 256                    6.286   0.971           0.596          C
+//   384 x 128                    6.375   0.976           0.650          C
+//   192 x 256                    6.348   1.134           0.597          C
+//   128 x 256                    6.394   1.283           0.597          C
+//
+// 384 x 256 is the fastest frame, and each kernel is also faster on its own at its new size. Both material builds use these shapes. A
+// block is always whole 8x8 groups (threads / 64 of them), the unit of the group RNG and the disocclusion vote.
 #ifndef ZR_RDI_TEMPORAL_THREADS
-#define ZR_RDI_TEMPORAL_THREADS 768
+#define ZR_RDI_TEMPORAL_THREADS 384
 #endif
 #ifndef ZR_RDI_SPATIAL_THREADS
-#define ZR_RDI_SPATIAL_THREADS 512
+#define ZR_RDI_SPATIAL_THREADS 256
 #endif
     static_assert(ZR_RDI_TEMPORAL_THREADS % 64 == 0 && ZR_RDI_SPATIAL_THREADS % 64 == 0, "a DI block is whole 8x8 groups");
+    // the register bound through __launch_bounds__'s blocks-per-SM argument, whatever the block size
+    constexpr int DI_TEMPORAL_REGS = 80, DI_SPATIAL_REGS = 128;
+    static_assert(ZR_RDI_TEMPORAL_THREADS * DI_TEMPORAL_REGS <= 65536 && ZR_RDI_SPATIAL_THREADS * DI_SPATIAL_REGS <= 65536,
+        "a DI block must fit the register file at its bound");
     // k_di_temporal's RIS reservoir: only reservoir updates and the MIS tails touch it, yet it crosses the roughly 20 barriers of
     // RIS_InitialCandidates_Sync and TemporalResample1_Sync. It lives in dynamic shared memory, one record per thread, as
     // k_pathtrace's PtParked does. Reservoir's float2 makes the record a multiple of 8 bytes, so its stride cannot be an odd number
@@ -47,7 +69,7 @@ namespace
     // MF: the material features the kernel is compiled for (BSDF::ShadingDataT); the scene's materials must use no others.
     // Dynamic shared memory: DI_TEMPORAL_SMEM_BYTES.
     template<uint32_t MF>
-    __global__ void ZR_LB(ZR_RDI_TEMPORAL_THREADS) k_di_temporal(SceneDev sc, FrameView f, DIParams prm, zr_rdi_reservoir* __restrict__ resCurr,
+    __global__ void __launch_bounds__(ZR_RDI_TEMPORAL_THREADS, 65536 / (ZR_RDI_TEMPORAL_THREADS * DI_TEMPORAL_REGS)) k_di_temporal(SceneDev sc, FrameView f, DIParams prm, zr_rdi_reservoir* __restrict__ resCurr,
         const zr_rdi_reservoir* __restrict__ resPrev, uint2* __restrict__ target, float4* __restrict__ finalImg, uint32_t dispX, uint32_t dispY,
         const uint32_t* __restrict__ order)
     {
@@ -132,7 +154,7 @@ namespace
 
     // ReSTIR_DI_Spatial.hlsl main + SpatialResample
     template<uint32_t MF>
-    __global__ void ZR_LB(ZR_RDI_SPATIAL_THREADS) k_di_spatial(SceneDev sc, FrameView f, DIParams prm, const zr_rdi_reservoir* __restrict__ resCurr,
+    __global__ void __launch_bounds__(ZR_RDI_SPATIAL_THREADS, 65536 / (ZR_RDI_SPATIAL_THREADS * DI_SPATIAL_REGS)) k_di_spatial(SceneDev sc, FrameView f, DIParams prm, const zr_rdi_reservoir* __restrict__ resCurr,
         const uint2* __restrict__ target, float4* __restrict__ finalImg, uint32_t dispX, uint32_t dispY,
         const uint32_t* __restrict__ order)
     {

@@ -7,10 +7,21 @@
 //
 //   frame 1 only      zr_prelighting_render        power estimate + alias table (on device, so no one-frame read-back delay)
 //   every frame       zr_presample_emissives       when presampling is on (the reference: >= 13107 emissive triangles)
-//                     GBufferRT
-//                     DirectLighting  ||  IndirectLighting      second stream, joined before Compositing
+//                     GBufferRT -> IndirectLighting               `chain` stream, the greatest priority
+//                     DirectLighting                              `side` stream, the least priority, after GBufferRT
 //                     Compositing (+ firefly filter) -> [SVGF denoise, zr_renderer_set_denoiser] -> TAA
 //                     with zr_renderer_set_display: AutoExposure on the TAA input before TAA, Display on its output after it
+//
+// Streams (two_streams != 0; otherwise every pass runs on the caller's stream in the order above). `chain` is forked from the caller's
+// stream by an event and holds the frame's critical path: GBufferRT and IndirectLighting, whose shift stages fork two more streams of
+// the same priority (ShiftStreams, rpt_spatial.cu). DirectLighting is the shorter of the two lighting passes and needs only the
+// G-buffer, so it runs at the least priority: the block scheduler hands an SM to a pending DirectLighting block only when no chain
+// kernel has a block waiting, and DirectLighting fills the SM time the chain leaves idle (the last wave of k_pathtrace, the drain of the
+// persistent shift launches, the ramps and gaps of the short kernels) instead of delaying the chain. Both streams join the caller's
+// stream before Compositing, and everything from Compositing on -- SVGF, AutoExposure, TAA, Display, the post-lighting halo exchange and
+// the gathers -- runs on the caller's stream, so the caller's stream is ordered after the whole frame. Strip-sharded, DirectLighting's
+// halo exchange uses communicator 1 on `side`; IndirectLighting's use communicator 0 on `chain`, and the caller's stream uses
+// communicator 0 after the join, which orders the two.
 //
 // The renderer owns the double-buffered G-buffers (DefaultRendererImpl.h:111-121) and the pass objects; callers reach
 // the passes through zr_renderer_get_*_pass to set parameters, exactly like the reference's UI callbacks do.
@@ -36,8 +47,9 @@ struct zr_renderer
     zr_svgf_pass* svgf = nullptr;                   // optional denoise stage between Compositing and TAA (BASELINE config 3)
     zr_auto_exposure_pass* ae = nullptr;            // optional post-processing (PostProcessor.cpp): both or neither
     zr_display_pass* display = nullptr;
-    cudaStream_t side = nullptr;            // DirectLighting runs here when twoStreams
-    cudaEvent_t evGBuffer = nullptr, evDirect = nullptr;
+    cudaStream_t chain = nullptr;           // GBufferRT + IndirectLighting when twoStreams, the greatest priority
+    cudaStream_t side = nullptr;            // DirectLighting when twoStreams, the least priority
+    cudaEvent_t evFork = nullptr, evGBuffer = nullptr, evChain = nullptr, evDirect = nullptr;
     bool twoStreams = true;
     // strip-sharded frames
     zr_comm* comm = nullptr;                // not owned
@@ -51,7 +63,7 @@ struct zr_renderer
     {
         HookCtx* h = (HookCtx*)user;
         zr_renderer* r = h->r;
-        // DirectLighting runs on the second stream when twoStreams: it gets its own communicator
+        // DirectLighting runs on `side` when twoStreams, concurrently with the chain's exchanges: it gets its own communicator
         const int which = (r->twoStreams && stream == (void*)r->side) ? 1 : 0;
         const zr_status s = zr_comm_exchange_halos(r->comm, which, r->bounds.data(), HALO, planes, n, stream);
         if (s != ZR_OK) r->hookStatus = s;
@@ -117,10 +129,11 @@ struct zr_renderer
         ReleaseDisplay();
         gbufferPass = nullptr; direct = nullptr; indirect = nullptr; compositing = nullptr; taa = nullptr;
         for (int i = 0; i < 2; i++) zr_gbuffer_free(&gbuffer[i]);
+        if (chain) cudaStreamDestroy(chain);
         if (side) cudaStreamDestroy(side);
-        if (evGBuffer) cudaEventDestroy(evGBuffer);
-        if (evDirect) cudaEventDestroy(evDirect);
-        side = nullptr; evGBuffer = evDirect = nullptr;
+        for (cudaEvent_t e : { evFork, evGBuffer, evChain, evDirect })
+            if (e) cudaEventDestroy(e);
+        chain = side = nullptr; evFork = evGBuffer = evChain = evDirect = nullptr;
     }
 };
 
@@ -142,9 +155,12 @@ extern "C"
         if (s == ZR_OK) s = zr_indirect_pass_create(desc->width, desc->height, &r->indirect);
         if (s == ZR_OK) s = zr_compositing_pass_create(desc->width, desc->height, &r->compositing);
         if (s == ZR_OK) s = zr_taa_pass_create(desc->width, desc->height, &r->taa);
-        if (s == ZR_OK && cudaStreamCreateWithFlags(&r->side, cudaStreamNonBlocking) != cudaSuccess) s = ZR_ERR_CUDA;
-        if (s == ZR_OK && cudaEventCreateWithFlags(&r->evGBuffer, cudaEventDisableTiming) != cudaSuccess) s = ZR_ERR_CUDA;
-        if (s == ZR_OK && cudaEventCreateWithFlags(&r->evDirect, cudaEventDisableTiming) != cudaSuccess) s = ZR_ERR_CUDA;
+        int leastPriority = 0, greatestPriority = 0;
+        if (s == ZR_OK && cudaDeviceGetStreamPriorityRange(&leastPriority, &greatestPriority) != cudaSuccess) s = ZR_ERR_CUDA;
+        if (s == ZR_OK && cudaStreamCreateWithPriority(&r->chain, cudaStreamNonBlocking, greatestPriority) != cudaSuccess) s = ZR_ERR_CUDA;
+        if (s == ZR_OK && cudaStreamCreateWithPriority(&r->side, cudaStreamNonBlocking, leastPriority) != cudaSuccess) s = ZR_ERR_CUDA;
+        for (cudaEvent_t* e : { &r->evFork, &r->evGBuffer, &r->evChain, &r->evDirect })
+            if (s == ZR_OK && cudaEventCreateWithFlags(e, cudaEventDisableTiming) != cudaSuccess) s = ZR_ERR_CUDA;
         if (s != ZR_OK) { r->Release(); delete r; return s; }
         *out = r;
         return ZR_OK;
@@ -186,22 +202,33 @@ extern "C"
         in.prev = r->gbuffer[r->curr ^ 1];
         in.scene = r->scene;
 
-        s = zr_gbuffer_pass_render(r->gbufferPass, &in, stream);
-        if (s != ZR_OK) return s;
-        cudaStream_t directStream = stream;
+        cudaStream_t chainStream = stream, directStream = stream;
         if (r->twoStreams)
         {
-            ZR_CUDA(cudaEventRecord(r->evGBuffer, stream));
-            ZR_CUDA(cudaStreamWaitEvent(r->side, r->evGBuffer, 0));
+            ZR_CUDA(cudaEventRecord(r->evFork, stream));
+            ZR_CUDA(cudaStreamWaitEvent(r->chain, r->evFork, 0));
+            chainStream = r->chain;
             directStream = r->side;
         }
-        s = zr_direct_pass_render(r->direct, &in, directStream);
-        if (s != ZR_OK) return s;
-        s = r->integrator != ZR_INTEGRATOR_RESTIR_PT ? zr_gi_pass_render(r->gi, &in, stream) : zr_indirect_pass_render(r->indirect, &in, stream);
+        s = zr_gbuffer_pass_render(r->gbufferPass, &in, chainStream);
         if (s != ZR_OK) return s;
         if (r->twoStreams)
         {
-            ZR_CUDA(cudaEventRecord(r->evDirect, r->side));
+            ZR_CUDA(cudaEventRecord(r->evGBuffer, chainStream));
+            ZR_CUDA(cudaStreamWaitEvent(r->side, r->evGBuffer, 0));
+        }
+        // the chain is enqueued first: were DirectLighting first, a device that has caught up with the host would start its blocks
+        // before the chain's kernels exist, and no priority could give those SMs back
+        s = r->integrator != ZR_INTEGRATOR_RESTIR_PT ? zr_gi_pass_render(r->gi, &in, chainStream)
+                                                     : zr_indirect_pass_render(r->indirect, &in, chainStream);
+        if (s != ZR_OK) return s;
+        s = zr_direct_pass_render(r->direct, &in, directStream);
+        if (s != ZR_OK) return s;
+        if (r->twoStreams)
+        {
+            ZR_CUDA(cudaEventRecord(r->evChain, chainStream));
+            ZR_CUDA(cudaEventRecord(r->evDirect, directStream));
+            ZR_CUDA(cudaStreamWaitEvent(stream, r->evChain, 0));
             ZR_CUDA(cudaStreamWaitEvent(stream, r->evDirect, 0));
         }
         s = r->TakeHookStatus();

@@ -329,9 +329,13 @@ zr_status ShiftStreams::Init()
     ZR_CUDA(cudaFuncSetAttribute(k_spatial_merge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MergeSmem)));
     ZR_TRY(SetupShifts<false>());
     ZR_TRY(SetupTemporalShifts());
+    // the greatest priority: in the renderer's frame the shift stages are on the critical path, and DirectLighting runs beside them at
+    // the least (renderer.cu); a pass driven on a stream of the default priority loses nothing by it
+    int leastPriority = 0, greatestPriority = 0;
+    ZR_CUDA(cudaDeviceGetStreamPriorityRange(&leastPriority, &greatestPriority));
     for (int i = 0; i < 2; i++)
     {
-        ZR_CUDA(cudaStreamCreateWithFlags(&aux[i], cudaStreamNonBlocking));
+        ZR_CUDA(cudaStreamCreateWithPriority(&aux[i], cudaStreamNonBlocking, greatestPriority));
         ZR_CUDA(cudaEventCreateWithFlags(&evJoin[i], cudaEventDisableTiming));
     }
     ZR_CUDA(cudaEventCreateWithFlags(&evFork, cudaEventDisableTiming));

@@ -28,8 +28,8 @@ static_assert(sizeof(ShiftResult) == 32, "ShiftResult is two 128-bit words");
 
 // What the shift launches need whatever the frame size: created once with the pass (Init, which also sets k_spatial_merge's shared
 // memory limit), released with it. The six class launches of a shift stage are independent (own queue, own claim cursor, disjoint result
-// bytes): they are spread over the caller's stream and two forked ones, so that short queues -- small classes, strip-sharded frames --
-// run side by side.
+// bytes): they are spread over the caller's stream and two forked ones of the greatest priority, so that short queues -- small classes,
+// strip-sharded frames -- run side by side.
 struct ShiftStreams
 {
     int numSMs = 0;
