@@ -53,7 +53,8 @@ ZR_API const char* zr_last_error(void);
  * the stage-limited ReSTIR PT render and its stage enum, which nothing called. 1.6 added the AutoExposure and Display passes,
  * zr_renderer_set_display / get_display_output and zr_comm_allreduce_u32. 1.7 added zr_comm_create_transport (zr_comm_transport). 1.8
  * added zr_svgf_pass_set_rows / set_halo_exchange, and zr_renderer_set_shard runs the SVGF stage sharded instead of refusing it. 1.9
- * added zr_scene_update_materials and zr_scene_get_tables. */
+ * added zr_scene_update_materials and zr_scene_get_tables. 1.10 added pixel picking (zr_gbuffer_pass_pick / get_pick), the Display
+ * pass's G-buffer debug views (zr_display_pass_set_view) and the outline of picked instances (zr_display_pass_set_picked). */
 ZR_API uint32_t zr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -462,6 +463,13 @@ ZR_API zr_status zr_gbuffer_pass_render(zr_gbuffer_pass* p, const zr_frame_input
 ZR_API zr_status zr_gbuffer_pass_set_rows(zr_gbuffer_pass* p, uint32_t y0, uint32_t y1);
 ZR_API zr_status zr_gbuffer_pass_describe_io(zr_gbuffer_pass* p, zr_resource_use* uses, int* n);
 ZR_API void zr_gbuffer_pass_destroy(zr_gbuffer_pass* p);
+/* Pixel picking (DefaultRenderer::Pick -> GBufferRT::PickPixel, DefaultRenderer.cpp:558-568; GBufferRT_Inline.hlsl:241-242). A pick
+ * is one-shot: the next zr_gbuffer_pass_render writes into the pass's pick word the index of the instance under pixel (x, y) (its
+ * position in zr_scene_desc.h_instances), or 0xffffffff when the primary ray misses, (x, y) lies outside the frame or row y
+ * outside the rows this pass renders; later renders leave the word alone. The word holds 0xffffffff from create on. Copy it to
+ * the host after that render on its stream (Display.cpp:210-229, ReadbackPickIdx). */
+ZR_API zr_status zr_gbuffer_pass_pick(zr_gbuffer_pass* p, uint32_t x, uint32_t y);
+ZR_API zr_status zr_gbuffer_pass_get_pick(zr_gbuffer_pass* p, zr_image2d* out);        /* 1 x 1 uint32, device */
 
 /* ---- DirectLighting (ReSTIR DI, DirectLighting/Emissive/DirectLighting.h:36-57) ---- */
 typedef struct zr_direct_pass zr_direct_pass;
@@ -692,6 +700,24 @@ ZR_API zr_status zr_display_pass_render(zr_display_pass* p, const zr_frame_input
 ZR_API zr_status zr_display_pass_set_rows(zr_display_pass* p, uint32_t y0, uint32_t y1);
 ZR_API zr_status zr_display_pass_get_output(zr_display_pass* p, zr_image2d* out);      /* RGBA8, 4 B/px */
 ZR_API void zr_display_pass_destroy(zr_display_pass* p);
+/* Debug views (DisplayOption, Display_Common.h:6-19, same order; Display.hlsl:53-170). A view other than DEFAULT shows one
+ * channel of the current G-buffer in place of the tone-mapped signal: render then reads no signal, exposure or LUT (d_signal and
+ * d_exposure may be NULL) and writes (0, 0, 0, 0) where the primary ray missed. ROUGHNESS_TH marks roughness >= roughness_th.
+ * Default DEFAULT, 1.0 (Display.cpp:73); a view > DEPTH or a non-finite threshold is ZR_ERR_INVALID_ARG. */
+typedef enum zr_display_view
+{
+    ZR_DISPLAY_VIEW_DEFAULT = 0, ZR_DISPLAY_VIEW_BASE_COLOR, ZR_DISPLAY_VIEW_NORMAL, ZR_DISPLAY_VIEW_METALNESS_ROUGHNESS,
+    ZR_DISPLAY_VIEW_COAT_WEIGHT, ZR_DISPLAY_VIEW_COAT_COLOR, ZR_DISPLAY_VIEW_ROUGHNESS_TH, ZR_DISPLAY_VIEW_EMISSIVE,
+    ZR_DISPLAY_VIEW_TRANSMISSION, ZR_DISPLAY_VIEW_DEPTH
+} zr_display_view;
+ZR_API zr_status zr_display_pass_set_view(zr_display_pass* p, uint32_t view, float roughness_th);
+/* Outline of picked instances (SetPickedInstance / GetPickedInstances; Display.cpp:293-400, DrawPicked.hlsl, Sobel.hlsl). Each
+ * frame with picks, render rasterises picked instance k into bit k of a mask (placed by its TRS, clipped at CameraNear, no culling
+ * and no depth test) and draws the mask's Sobel outline over the image. h_instances holds instance indices as in
+ * zr_gbuffer_pass_pick; n == 0 clears the picks. More than ZR_DISPLAY_MAX_PICKED, or NULL with n > 0, is ZR_ERR_INVALID_ARG; render
+ * refuses, before it launches anything, an index that is not in the frame's scene. Picks and the view survive a resize. */
+#define ZR_DISPLAY_MAX_PICKED 32u
+ZR_API zr_status zr_display_pass_set_picked(zr_display_pass* p, const uint32_t* h_instances, uint32_t n);
 
 /* ---- host <-> device helpers so callers need no CUDA runtime of their own ---- */
 ZR_API zr_status zr_device_malloc(void** d_ptr, size_t bytes);

@@ -10,8 +10,12 @@
 //   k_exposure        one block: weighted mean of bins 1..255 in a fixed pairwise order, inverse mapping, temporal adaptation,
 //                     EV100 exposure -> float2 {exposure, adapted luminance}; clears the bins for the next frame
 //   k_display         TAA output (8 B/px) x exposure -> tone mapper -> saturate -> sRGB OETF -> RGBA8 (4 B/px)
+//   k_display_view    a G-buffer debug view (Display.hlsl:79-170) in place of k_display
+//   k_pick_mask       picked instance k's triangles -> bit k of a per-pixel mask (DrawPicked.hlsl), a warp per triangle
+//   k_outline         the mask's Sobel outline over the displayed image (Sobel.hlsl:27-105)
 #include <cmath>
 #include "zr_common.cuh"
+#include "zr_pixel.cuh"
 #include "zr_planes.h"
 #include "zr_schedule.h"
 
@@ -192,6 +196,12 @@ namespace
 
     ZR_D float SrgbOetf(float v) { return v <= 0.0031308f ? 12.92f * v : 1.055f * zr_powf(v, 1.0f / 2.4f) - 0.055f; }
 
+    // saturated linear RGB -> the R8G8B8A8_UNORM_SRGB store's RGB bytes
+    ZR_D uint32_t EncodeSrgb8(float3 c)
+    {
+        return Math::FloatToUNorm8(SrgbOetf(c.x)) | Math::FloatToUNorm8(SrgbOetf(c.y)) << 8 | Math::FloatToUNorm8(SrgbOetf(c.z)) << 16;
+    }
+
     struct DisplayArgs { uint32_t tonemapper, autoExposure; float saturation, agxExp; };
 
     ZR_D float3 Tonemap(float3 c, const DisplayArgs& a, const uint32_t* __restrict__ lut)
@@ -223,8 +233,197 @@ namespace
         if (a.autoExposure)
             c = c * __ldg(&exposure->x);
         c = saturate(Tonemap(c, a, lut));
-        out[i] = Math::FloatToUNorm8(SrgbOetf(c.x)) | Math::FloatToUNorm8(SrgbOetf(c.y)) << 8 |
-            Math::FloatToUNorm8(SrgbOetf(c.z)) << 16 | 0xff000000u;
+        out[i] = EncodeSrgb8(c) | 0xff000000u;
+    }
+
+    // Display.hlsl:53-54, 79-170: one G-buffer channel in place of the tone-mapped signal, pixels [begin, end). The reference
+    // tone-maps first and then overwrites the result, so a view reads no signal, exposure or LUT.
+    __global__ void __launch_bounds__(256) k_display_view(const uint4* __restrict__ core, const uint2* __restrict__ me,
+        const uint2* __restrict__ coat, uint32_t* __restrict__ out, size_t begin, size_t end, uint32_t view, float roughnessTh,
+        float cameraNear)
+    {
+        const size_t i = begin + (size_t)blockIdx.x * 256 + threadIdx.x;
+        if (i >= end)
+            return;
+        const uint4 c = ld128(&core[i]);
+        const float z = asfloat(c.x);
+        if (z == FLT_MAX_)
+        {
+            out[i] = 0u;        // background: (0, 0, 0, 0), alpha included
+            return;
+        }
+        const GFlags fl = DecodeFlags(c.w & 0xff);
+        const float roughness = Math::UNorm8ToFloat((c.w >> 8) & 0xff);
+        const float3 baseColor = Math::UnpackRGB8(c.z & 0xffffff);
+        float3 d = f3(0.0f);
+        switch (view)
+        {
+        case ZR_DISPLAY_VIEW_BASE_COLOR: d = baseColor; break;
+        case ZR_DISPLAY_VIEW_NORMAL: d = Math::DecodeUnitVector(Math::DecodeUNorm2(c.y)) * 0.5f + 0.5f; break;
+        case ZR_DISPLAY_VIEW_METALNESS_ROUGHNESS: d = f3(fl.metallic ? 1.0f : 0.0f, roughness, 0.0f); break;
+        case ZR_DISPLAY_VIEW_COAT_WEIGHT:
+        case ZR_DISPLAY_VIEW_COAT_COLOR:
+            if (fl.coated)
+            {
+                // GBuffer::UnpackCoat, as LoadPixel (zr_pixel.cuh) reads the coat plane
+                const uint2 cc = __ldg(&coat[i]);
+                const uint32_t px = cc.x & 0xffff, py = cc.x >> 16;
+                d = view == ZR_DISPLAY_VIEW_COAT_WEIGHT ? f3(Math::UNorm8ToFloat((py >> 8) & 0xff)) : Math::UnpackRGB8(px | ((py & 0xff) << 16));
+            }
+            break;
+        case ZR_DISPLAY_VIEW_ROUGHNESS_TH: d = roughness >= roughnessTh ? f3(0.26f, 0.014f, 0.021f) : f3(0.0f); break;
+        case ZR_DISPLAY_VIEW_EMISSIVE: d = fl.emissive ? unpack_r11g11b10(__ldg(&me[i].y)) : baseColor * 0.005f; break;
+        case ZR_DISPLAY_VIEW_TRANSMISSION: d = f3(fl.transmissive ? 1.0f : 0.0f, fl.transmissive ? 0.0f : 1.0f, 0.0f); break;
+        case ZR_DISPLAY_VIEW_DEPTH: d = f3(cameraNear / z); break;
+        default: break;
+        }
+        out[i] = EncodeSrgb8(saturate(d)) | 0xff000000u;
+    }
+
+    // ---- picked-instance outline (Display.cpp:293-400, DrawPicked.hlsl, Sobel.hlsl); DESIGN 6b states the rasteriser's rules ----
+    // The picked instances and the running sum of their triangle counts: warp w rasterises triangle w - triEnd[k - 1] of inst[k].
+    struct PickList { uint32_t n; uint32_t inst[ZR_DISPLAY_MAX_PICKED]; uint32_t triEnd[ZR_DISPLAY_MAX_PICKED]; };
+
+    // Clips a view-space triangle to z >= near, the one clip plane of a reverse-Z projection with an infinite far plane: 0, 3 or 4
+    // vertices of a convex polygon, in order. A crossing point is computed from the edge's inside vertex, so the two triangles
+    // that share an edge clip it to the same point.
+    ZR_D int ClipNear(const float3 (&v)[3], float nearZ, float3 (&out)[4])
+    {
+        int n = 0;
+        for (int e = 0; e < 3; e++)
+        {
+            const float3 a = v[e], b = v[e == 2 ? 0 : e + 1];
+            const bool ina = a.z >= nearZ, inb = b.z >= nearZ;
+            if (ina)
+                out[n++] = a;
+            if (ina != inb)
+            {
+                const float3 p = ina ? a : b, q = ina ? b : a;
+                const float t = (nearZ - p.z) / (q.z - p.z);
+                out[n++] = f3(p.x + t * (q.x - p.x), p.y + t * (q.y - p.y), nearZ);
+            }
+        }
+        return n;
+    }
+
+    // The inverse of k_gbuffer's camera-ray mapping (Math::NDCFromUV, jitter included): a view-space point on the ray of pixel
+    // (x, y) lands on (x + 0.5, y + 0.5).
+    ZR_D float2 ProjectToPixel(float3 p, const zr_frame_constants& fc)
+    {
+        const float2 ndc = f2(p.x / p.z / fc.TanHalfFOV / fc.AspectRatio, p.y / p.z / fc.TanHalfFOV);
+        const float2 uv = Math::UVFromNDC(ndc);
+        return f2(uv.x * (float)fc.RenderWidth - fc.CurrCameraJitter[0], uv.y * (float)fc.RenderHeight - fc.CurrCameraJitter[1]);
+    }
+
+    // Edge function of a -> b at p, evaluated with the endpoints in one fixed order, so the two triangles that share an edge get
+    // exactly opposite values
+    ZR_D float EdgeFn(float2 a, float2 b, float2 p)
+    {
+        const bool swap = b.y < a.y || (b.y == a.y && b.x < a.x);
+        const float2 s = swap ? b : a, t = swap ? a : b;
+        const float e = (t.x - s.x) * (p.y - s.y) - (t.y - s.y) * (p.x - s.x);
+        return swap ? -e : e;
+    }
+    // Inside is E > 0 on every edge of an oriented triangle (rows grow downwards). A centre on an edge is inside when the edge is
+    // a left edge (b.y < a.y) or a top edge (horizontal, b.x > a.x): the D3D top-left rule.
+    ZR_D bool EdgeIn(float2 a, float2 b, float2 p)
+    {
+        const float e = EdgeFn(a, b, p);
+        return e > 0.0f || (e == 0.0f && (b.y < a.y || (b.y == a.y && b.x > a.x)));
+    }
+    // Either winding: no back-face culling (the DrawPicked PSO, Display.cpp:452-470). A degenerate triangle covers nothing.
+    ZR_D bool InTriangle(float2 a, float2 b, float2 c, float2 p)
+    {
+        const float area = EdgeFn(a, b, c);
+        if (area == 0.0f)
+            return false;
+        if (area < 0.0f) { const float2 t = b; b = c; c = t; }
+        return EdgeIn(a, b, p) && EdgeIn(b, c, p) && EdgeIn(c, a, p);
+    }
+
+    // Rows [y0, y1) of the mask; no depth test, so hidden parts of an instance are marked too
+    __global__ void __launch_bounds__(256) k_pick_mask(SceneDev sc, zr_frame_constants fc, PickList pl, uint32_t* __restrict__ mask,
+        uint32_t y0, uint32_t y1)
+    {
+        const uint32_t w = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+        if (w >= pl.triEnd[pl.n - 1])
+            return;
+        uint32_t k = 0;
+        while (w >= pl.triEnd[k])
+            k++;
+        const uint32_t prim = w - (k ? pl.triEnd[k - 1] : 0u);
+        const zr_mesh_instance md = LoadInstance(sc, pl.inst[k]);
+        const float4 q = normalize(Math::DecodeNormalized4(md.Rotation));
+        const float3 scale = h3(md.Scale);
+        const float3 translation = f3(md.Translation[0], md.Translation[1], md.Translation[2]);
+        float3 v[3];
+        for (int j = 0; j < 3; j++)
+        {
+            const VertexD V = LoadVertex(sc, __ldg(&sc.indices[prim * 3 + md.BaseIdxOffset + j]) + md.BaseVtxOffset);
+            v[j] = Math::mul3x4(fc.CurrView, Math::TransformTRS(V.pos, translation, q, scale));
+        }
+        float3 c[4];
+        const int n = ClipNear(v, fc.CameraNear, c);
+        if (n < 3)
+            return;
+        float2 s[4];
+        float x0 = FLT_MAX_, x1 = -FLT_MAX_, ya = FLT_MAX_, yb = -FLT_MAX_;
+        for (int j = 0; j < n; j++)
+        {
+            s[j] = ProjectToPixel(c[j], fc);
+            x0 = fminf(x0, s[j].x); x1 = fmaxf(x1, s[j].x); ya = fminf(ya, s[j].y); yb = fmaxf(yb, s[j].y);
+        }
+        // pixels whose centre can lie inside, clamped to the frame's columns and the rows asked for
+        const float xs = fmaxf(ceilf(x0 - 0.5f), 0.0f), xe = fminf(floorf(x1 - 0.5f), (float)fc.RenderWidth - 1.0f);
+        const float ys = fmaxf(ceilf(ya - 0.5f), (float)y0), ye = fminf(floorf(yb - 0.5f), (float)y1 - 1.0f);
+        if (!(xs <= xe && ys <= ye))
+            return;
+        const uint32_t bx = (uint32_t)xs, by = (uint32_t)ys, bw = (uint32_t)xe - bx + 1, bh = (uint32_t)ye - by + 1;
+        const uint32_t bit = 1u << k;
+        for (uint32_t j = lane; j < bw * bh; j += 32)
+        {
+            const uint32_t x = bx + j % bw, y = by + j / bw;
+            const float2 p = f2((float)x + 0.5f, (float)y + 0.5f);
+            if (InTriangle(s[0], s[1], s[2], p) || (n == 4 && InTriangle(s[0], s[2], s[3], p)))
+                atomicOr(&mask[(size_t)y * fc.RenderWidth + x], bit);
+        }
+    }
+
+    // Sobel.hlsl, for each bit k of the mask: a pixel with bit k somewhere in its in-frame 3 x 3 neighbourhood (CheckNeighborHood)
+    // and a non-zero Sobel gradient of bit k (taps outside the frame read 0) takes the outline colour. The gradients are small
+    // integers, exact in float, and Luminance(sqrt(gx^2 + gy^2)) > 0 exactly when one of them is non-zero. Pixels [begin, end).
+    __global__ void __launch_bounds__(256) k_outline(const uint32_t* __restrict__ mask, uint32_t* __restrict__ out, uint32_t W,
+        uint32_t H, size_t begin, size_t end)
+    {
+        const size_t i = begin + (size_t)blockIdx.x * 256 + threadIdx.x;
+        if (i >= end)
+            return;
+        const int x = (int)(i % W), y = (int)(i / W);
+        uint32_t m[3][3];
+        uint32_t any = 0;
+        for (int r = 0; r < 3; r++)
+            for (int c = 0; c < 3; c++)
+            {
+                const int xx = x - 1 + c, yy = y - 1 + r;
+                m[r][c] = xx >= 0 && xx < (int)W && yy >= 0 && yy < (int)H ? __ldg(&mask[(size_t)yy * W + xx]) : 0u;
+                any |= m[r][c];
+            }
+        for (uint32_t b = any; b; b &= b - 1)
+        {
+            const uint32_t bit = b & (0u - b);
+            int t[3][3];
+            for (int r = 0; r < 3; r++)
+                for (int c = 0; c < 3; c++)
+                    t[r][c] = (m[r][c] & bit) ? 1 : 0;
+            const int gx = -t[0][0] - 2 * t[1][0] - t[2][0] + t[0][2] + 2 * t[1][2] + t[2][2];
+            const int gy = t[0][0] + 2 * t[0][1] + t[0][2] - t[2][0] - 2 * t[2][1] - t[2][2];
+            if (gx != 0 || gy != 0)
+            {
+                // the reference writes this linear colour into its _SRGB back buffer
+                out[i] = EncodeSrgb8(f3(0.913098693f, 0.332451582f, 0.048171822f)) | 0xff000000u;
+                return;
+            }
+        }
     }
 
     bool is_finite(float v) { return std::isfinite(v); }
@@ -318,17 +517,22 @@ struct zr_auto_exposure_pass
 
 struct zr_display_pass
 {
-    // DisplayPass (Display/Display.h), default display option: the R8G8B8A8 image it presents
+    // DisplayPass (Display/Display.h): the R8G8B8A8 image it presents, its debug view and the outline of the picked instances
     uint32_t width = 0, height = 0;
     struct Sized
     {
         zr::Planes planes{ "zr_display_pass" };
         uint32_t* d_out = nullptr;
+        uint32_t* d_mask = nullptr;         // bit k: picked instance k covers the pixel (rows of the frame with picks)
     } sz;
     zr::Planes lutPlanes{ "zr_display_pass" };
     uint32_t* d_lut = nullptr;              // Tony McMapface, packed R9G9B9E5; NULL until set_lut
     zr_display_params params = Defaults();
     zr::StripRows strip{ "zr_display_pass" };
+    uint32_t view = ZR_DISPLAY_VIEW_DEFAULT;
+    float roughnessTh = 1.0f;               // Display.cpp:73
+    uint32_t picked[ZR_DISPLAY_MAX_PICKED] = {};
+    uint32_t numPicked = 0;
 
     static zr_display_params Defaults() { return zr_display_params{ ZR_TONEMAPPER_NEUTRAL, 1u, 1.0f, 1.0f }; }     // Display.cpp:70-74
     zr_status Setup() { return ZR_OK; }
@@ -336,6 +540,7 @@ struct zr_display_pass
     {
         Sized next;
         ZR_TRY(next.planes.Alloc(next.d_out, (size_t)w * h));
+        ZR_TRY(next.planes.Alloc(next.d_mask, (size_t)w * h));
         ZR_TRY(next.planes.Clear());
         sz = std::move(next);
         width = w; height = h;
@@ -365,7 +570,8 @@ struct zr_display_pass
     zr_status Render(const zr_frame_inputs* in, const void* d_signal, const void* d_exposure, cudaStream_t stream)
     {
         using namespace zr;
-        if (!in || !d_signal)
+        const bool defaultView = view == ZR_DISPLAY_VIEW_DEFAULT;
+        if (!in || (defaultView && !d_signal))
         {
             set_error("zr_display_pass_render: missing input");
             return ZR_ERR_INVALID_ARG;
@@ -377,22 +583,82 @@ struct zr_display_pass
                 in->frame.DisplayWidth, in->frame.DisplayHeight, in->frame.RenderWidth, in->frame.RenderHeight);
             return ZR_ERR_INVALID_ARG;
         }
-        if (params.auto_exposure && !d_exposure)
+        if (defaultView && params.auto_exposure && !d_exposure)
         {
             set_error("zr_display_pass_render: auto exposure is on but no exposure state was given");
             return ZR_ERR_INVALID_ARG;
         }
-        if (params.tonemapper == ZR_TONEMAPPER_NEUTRAL && !d_lut)
+        if (defaultView && params.tonemapper == ZR_TONEMAPPER_NEUTRAL && !d_lut)
         {
             set_error("zr_display_pass_render: the NEUTRAL tone mapper needs the Tony McMapface LUT (zr_display_pass_set_lut)");
             return ZR_ERR_INVALID_ARG;
         }
-        const DisplayArgs a{ params.tonemapper, params.auto_exposure ? 1u : 0u, params.saturation, params.agx_exp };
-        const size_t begin = (size_t)strip.rowBegin * width, end = (size_t)strip.ClampedRowEnd(height) * width;
-        ZR_PROF("k_display", stream);
-        k_display<<<(uint32_t)((end - begin + 255) / 256), 256, 0, stream>>>((const uint2*)d_signal, (const float2*)d_exposure, d_lut,
-            sz.d_out, begin, end, a);
-        ZR_LAUNCH_CHECK();
+        if (!defaultView && (!in->curr.d_core || !in->curr.d_motion_emissive || !in->curr.d_coat))
+        {
+            set_error("zr_display_pass_render: debug view %u reads the current G-buffer, which is missing", view);
+            return ZR_ERR_INVALID_ARG;
+        }
+        PickList pl{};
+        if (numPicked)
+        {
+            if (!in->scene)
+            {
+                set_error("zr_display_pass_render: picked instances need the scene");
+                return ZR_ERR_INVALID_ARG;
+            }
+            if (!(in->frame.CameraNear > 0.0f))
+            {
+                set_error("zr_display_pass_render: picked instances need CameraNear > 0 (got %g)", (double)in->frame.CameraNear);
+                return ZR_ERR_INVALID_ARG;
+            }
+            uint32_t total = 0;
+            for (uint32_t k = 0; k < numPicked; k++)
+            {
+                if (picked[k] >= in->scene->dev.numInstances)
+                {
+                    set_error("zr_display_pass_render: picked instance %u is not in the scene (%u instances)", picked[k],
+                        in->scene->dev.numInstances);
+                    return ZR_ERR_INVALID_ARG;
+                }
+                pl.inst[k] = picked[k];
+                total += in->scene->hostInstances[picked[k]].numTris;
+                pl.triEnd[k] = total;
+            }
+            pl.n = numPicked;
+        }
+        const uint32_t y0 = strip.rowBegin, y1 = strip.ClampedRowEnd(height);
+        const size_t begin = (size_t)y0 * width, end = (size_t)y1 * width;
+        const uint32_t blocks = (uint32_t)((end - begin + 255) / 256);
+        if (defaultView)
+        {
+            const DisplayArgs a{ params.tonemapper, params.auto_exposure ? 1u : 0u, params.saturation, params.agx_exp };
+            ZR_PROF("k_display", stream);
+            k_display<<<blocks, 256, 0, stream>>>((const uint2*)d_signal, (const float2*)d_exposure, d_lut, sz.d_out, begin, end, a);
+            ZR_LAUNCH_CHECK();
+        }
+        else
+        {
+            ZR_PROF("k_display_view", stream);
+            k_display_view<<<blocks, 256, 0, stream>>>((const uint4*)in->curr.d_core, (const uint2*)in->curr.d_motion_emissive,
+                (const uint2*)in->curr.d_coat, sz.d_out, begin, end, view, roughnessTh, in->frame.CameraNear);
+            ZR_LAUNCH_CHECK();
+        }
+        if (numPicked)
+        {
+            // the outline of row y reads the mask rows y - 1 .. y + 1: each strip rasterises its rows and one on either side
+            const uint32_t m0 = y0 ? y0 - 1 : 0u, m1 = y1 < height ? y1 + 1 : height;
+            ZR_CUDA(cudaMemsetAsync(sz.d_mask + (size_t)m0 * width, 0, (size_t)(m1 - m0) * width * sizeof(uint32_t), stream));
+            const uint32_t tris = pl.triEnd[numPicked - 1];
+            if (tris)
+            {
+                ZR_PROF("k_pick_mask", stream);
+                k_pick_mask<<<(uint32_t)(((uint64_t)tris * 32 + 255) / 256), 256, 0, stream>>>(in->scene->dev, in->frame, pl, sz.d_mask, m0, m1);
+                ZR_LAUNCH_CHECK();
+            }
+            ZR_PROF("k_outline", stream);
+            k_outline<<<blocks, 256, 0, stream>>>(sz.d_mask, sz.d_out, width, height, begin, end);
+            ZR_LAUNCH_CHECK();
+        }
         return ZR_OK;
     }
 };
@@ -461,6 +727,31 @@ extern "C"
         return p->Render(in, d_signal, d_exposure, (cudaStream_t)stream);
     }
     zr_status zr_display_pass_set_rows(zr_display_pass* p, uint32_t y0, uint32_t y1) { return p ? p->strip.SetRows(y0, y1, p->height) : ZR_ERR_INVALID_ARG; }
+    zr_status zr_display_pass_set_view(zr_display_pass* p, uint32_t view, float roughness_th)
+    {
+        if (!p) return ZR_ERR_INVALID_ARG;
+        if (view > ZR_DISPLAY_VIEW_DEPTH || !zr::is_finite(roughness_th))
+        {
+            zr::set_error("zr_display_pass_set_view: view must be 0..%d and roughness_th finite (got %u, %g)", (int)ZR_DISPLAY_VIEW_DEPTH,
+                view, (double)roughness_th);
+            return ZR_ERR_INVALID_ARG;
+        }
+        p->view = view; p->roughnessTh = roughness_th;
+        return ZR_OK;
+    }
+    zr_status zr_display_pass_set_picked(zr_display_pass* p, const uint32_t* h_instances, uint32_t n)
+    {
+        if (!p) return ZR_ERR_INVALID_ARG;
+        if (n > ZR_DISPLAY_MAX_PICKED || (n && !h_instances))
+        {
+            zr::set_error("zr_display_pass_set_picked: need n <= %u instance indices (got n = %u, %s)", ZR_DISPLAY_MAX_PICKED, n,
+                h_instances ? "data" : "NULL");
+            return ZR_ERR_INVALID_ARG;
+        }
+        for (uint32_t k = 0; k < n; k++) p->picked[k] = h_instances[k];
+        p->numPicked = n;
+        return ZR_OK;
+    }
     zr_status zr_display_pass_get_output(zr_display_pass* p, zr_image2d* out)
     {
         if (!p || !out) return ZR_ERR_INVALID_ARG;

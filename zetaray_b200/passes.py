@@ -248,9 +248,20 @@ class _Pass:
 
 class GBufferRT(_Pass):
     prefix = "zr_gbuffer_pass"
+    NO_PICK = 0xffffffff
 
     def __init__(self):
         self._create()
+
+    def Pick(self, x, y):
+        """GBufferRT::PickPixel: the next Render writes the instance index under pixel (x, y) (NO_PICK for none) into the pick word."""
+        self._call("pick", int(x), int(y))
+
+    def GetPick(self):
+        """The pick word (waits for the default stream): the instance index the last picking Render found, or NO_PICK."""
+        img = _lib.Image2D()
+        self._call("get_pick", C.byref(img))
+        return int(_d2h((np.zeros(1, dtype=np.uint32), img.d_ptr))[0][0])
 
 
 class DirectLighting(_Pass):
@@ -320,6 +331,19 @@ class Display(_Pass):
     prefix = "zr_display_pass"
     Params = _lib.DisplayParams
     NONE, NEUTRAL, AGX_DEFAULT, AGX_GOLDEN, AGX_PUNCHY, AGX_CUSTOM = range(6)
+    # zr_display_view (DisplayOption)
+    (VIEW_DEFAULT, VIEW_BASE_COLOR, VIEW_NORMAL, VIEW_METALNESS_ROUGHNESS, VIEW_COAT_WEIGHT, VIEW_COAT_COLOR, VIEW_ROUGHNESS_TH,
+     VIEW_EMISSIVE, VIEW_TRANSMISSION, VIEW_DEPTH) = range(10)
+    MAX_PICKED = 32
+
+    def SetView(self, view, roughness_th=1.0):
+        """DisplayOptionCallback: a G-buffer debug view in place of the tone-mapped image (VIEW_DEFAULT returns to it)."""
+        self._call("set_view", int(view), float(roughness_th))
+
+    def SetPicked(self, instances):
+        """SetPickedInstance / GetPickedInstances: outline these instance indices (at most MAX_PICKED; empty clears)."""
+        a = np.ascontiguousarray(np.asarray(instances, dtype=np.int64).reshape(-1)).astype(np.uint32)
+        self._call("set_picked", _vp(a) if len(a) else None, len(a))
 
     def SetLUT(self, lut):
         """lut: the Tony McMapface LUT as packed R9G9B9E5 texels, uint32[48][48][48] (x fastest)."""
@@ -448,6 +472,15 @@ class Renderer:
         self.display = self._wrapper(self.display, Display, disp)
         if enable and lut is not None:
             self.display.SetLUT(lut)
+
+    def Pick(self, x, y):
+        """DefaultRenderer::Pick: the next Render reports the instance under pixel (x, y) (GBufferRT.Pick)."""
+        self.gbuffer.Pick(x, y)
+
+    def GetPick(self):
+        """The instance the last picking Render found under its pixel, GBufferRT.NO_PICK for none. In a strip-sharded frame it is
+        what this rank's rows show: NO_PICK on a rank whose rows do not hold the pixel."""
+        return self.gbuffer.GetPick()
 
     def GetDisplayOutput(self):
         img = _lib.Image2D()
