@@ -11,6 +11,7 @@
 //   Math::Halton                ZetaCore/Math/Sampling.cpp:160-174
 // Pinned against the reference itself (oracle/_ref/libref_alias.so) and the golden vector of
 // SURVEY 8c by tests/test_alias_oracle.py.
+#include "orc_api.h"
 #include "orc_math.h"
 #include <vector>
 #include <cstdlib>

@@ -6,8 +6,8 @@
 //   display                Display/Display.hlsl:42-77 (DisplayOption::DEFAULT), Tonemap.hlsli, R8G8B8A8_UNORM_SRGB store
 // Defined here (DESIGN 6): the bin values are summed in one pairwise tree (h = 128, 64, ..., 1), the LUT is filtered with
 // float weights, the sRGB OETF is the exact IEC 61966-2-1 curve. Transcendentals are zr_fpmath.h's, as on the device.
+#include "orc_api.h"
 #include "orc_math.h"
-#include "../include/zr_abi.h"
 
 using namespace orc;
 

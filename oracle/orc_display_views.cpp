@@ -7,6 +7,7 @@
 //                  the inverse of the G-buffer's camera-ray mapping, pixel centres inside under the D3D top-left rule
 //   outline        Sobel.hlsl:27-105, for each bit of the mask
 // DESIGN 6b states the rasteriser's rules; the device kernels are csrc/display.cu and csrc/gbuffer.cu.
+#include "orc_api.h"
 #include "orc_scene.h"
 
 using namespace orc;
@@ -142,9 +143,12 @@ extern "C"
     }
 
     // Display.hlsl:53-170 over rows [y0, y1) of a W-wide G-buffer (core uint4, me uint2, coat uint2) -> RGBA8
-    void orc_display_view(const uint4* core, const uint2* me, const uint2* coat, uint32_t W, uint32_t y0, uint32_t y1, uint32_t view,
+    void orc_display_view(const uint32_t* core_, const uint32_t* me_, const uint32_t* coat_, uint32_t W, uint32_t y0, uint32_t y1, uint32_t view,
         float roughnessTh, float cameraNear, uint32_t* out)
     {
+        const uint4* core = (const uint4*)core_;
+        const uint2* me = (const uint2*)me_;
+        const uint2* coat = (const uint2*)coat_;
         for (size_t i = (size_t)y0 * W; i < (size_t)y1 * W; i++)
         {
             const uint4 c = core[i];

@@ -5,6 +5,7 @@
 //   ZetaRenderPass/GBuffer/GBufferRT.hlsli        ApplyTextureMaps :178-282, WriteToGBuffers :102-176
 //   ZetaRenderPass/Common/GBuffers.hlsli          EncodeMetallic :52-68
 // Parity unpinned (no reference tests). No textures / alpha test (DESIGN.md scope).
+#include "orc_api.h"
 #include "orc_scene.h"
 #include <thread>
 #include <functional>
@@ -80,9 +81,12 @@ extern "C"
     }
 
     // core: uint4[w*h], depth: float[w*h], me: uint2[w*h], coat: uint2[w*h], tridiff: 6 x u32 [w*h] or null
-    void orc_gbuffer(void* scene_, const zr_frame_constants* fc, uint4* core, float* depthPlane, uint2* me, uint2* coat,
+    void orc_gbuffer(void* scene_, const zr_frame_constants* fc, uint32_t* core_, float* depthPlane, uint32_t* me_, uint32_t* coat_,
         uint32_t* tridiff, int nthreads)
     {
+        uint4* core = (uint4*)core_;
+        uint2* me = (uint2*)me_;
+        uint2* coat = (uint2*)coat_;
         const Scene& sc = *(Scene*)scene_;
         const uint32_t W = fc->RenderWidth, H = fc->RenderHeight;
         auto rows = [&](uint32_t y0, uint32_t y1)

@@ -9,6 +9,7 @@
 // Documented deviations (DESIGN.md): sky/sun-disk background for invalid pixels is out of scope
 // (writes 0); the firefly filter reads an input image and writes a separate output (the reference
 // filters in place and races with itself); bilinear history taps use exact float weights.
+#include "orc_api.h"
 #include "orc_gbuffer.h"
 
 using namespace orc;
@@ -16,9 +17,13 @@ using namespace orc;
 extern "C"
 {
     // direct / indirect: float4[w*h] or null; out: float4[w*h]
-    void orc_compositing(const zr_frame_constants* fc, const uint4* core, const float4* direct,
-        const float4* indirect, float4* out)
+    void orc_compositing(const zr_frame_constants* fc, const uint32_t* core_, const float* direct_,
+        const float* indirect_, float* out_)
     {
+        const uint4* core = (const uint4*)core_;
+        const float4* direct = (const float4*)direct_;
+        const float4* indirect = (const float4*)indirect_;
+        float4* out = (float4*)out_;
         const uint32_t W = fc->RenderWidth, H = fc->RenderHeight;
         const bool accumulate = fc->Accumulate && fc->CameraStatic;
         const uint32_t numFramesAccumulated = accumulate ? fc->NumFramesCameraStatic : 1;
@@ -42,8 +47,11 @@ extern "C"
             }
     }
 
-    void orc_firefly(const zr_frame_constants* fc, const uint4* core, const float4* in, float4* out)
+    void orc_firefly(const zr_frame_constants* fc, const uint32_t* core_, const float* in_, float* out_)
     {
+        const uint4* core = (const uint4*)core_;
+        const float4* in = (const float4*)in_;
+        float4* out = (float4*)out_;
         const int W = (int)fc->RenderWidth, H = (int)fc->RenderHeight;
         for (int y = 0; y < H; y++)
             for (int x = 0; x < W; x++)
@@ -155,9 +163,14 @@ extern "C"
     }
 
     // signal: float4[w*h]; prevOut / out: half4 as uint2[w*h]
-    void orc_taa(const zr_frame_constants* fc, const uint4* core, const uint2* motionEmissive,
-        const float4* signal, const uint2* prevOut, uint2* out, float blendWeight, int temporalIsValid)
+    void orc_taa(const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* motionEmissive_,
+        const float* signal_, const uint32_t* prevOut_, uint32_t* out_, float blendWeight, int temporalIsValid)
     {
+        const uint4* core = (const uint4*)core_;
+        const uint2* motionEmissive = (const uint2*)motionEmissive_;
+        const float4* signal = (const float4*)signal_;
+        const uint2* prevOut = (const uint2*)prevOut_;
+        uint2* out = (uint2*)out_;
         const int W = (int)fc->RenderWidth, H = (int)fc->RenderHeight;
         for (int y = 0; y < H; y++)
             for (int x = 0; x < W; x++)

@@ -11,6 +11,7 @@
 //   DirectLighting/Emissive/DirectLighting.cpp:166-284 host sequencing
 // Compiled configuration: USE_HALF_VECTOR_COPY_SHIFT 0, no presampled sets (Params.hlsli:4-17).
 // Parity unpinned: the reference has no tests for this code.
+#include "orc_api.h"
 #include "orc_pixel.h"
 
 using namespace orc;
@@ -619,11 +620,16 @@ extern "C"
 {
     // Probe for the CPU-tier device-source parity test: ReSTIR DI at one pixel as the temporal kernel does it (mirrored by
     // tests/hostsim/hostsim_di.cpp). out (14 words): the 32-byte reservoir record, target (3), rng state, candidate valid, #BSDF samples
-    void orc_probe_rdi_pixel(void* scene, const zr_frame_constants* fc, const orc::uint4* core, const orc::uint2* me, const orc::uint2* coat,
-        const orc::uint4* pcore, const orc::uint2* pcoat, const zr_rdi_reservoir* prevRes, int x, int y, uint32_t sampleSetIdx, int temporal,
+    void orc_probe_rdi_pixel(void* scene, const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* me_, const uint32_t* coat_,
+        const uint32_t* pcore_, const uint32_t* pcoat_, const zr_rdi_reservoir* prevRes, int x, int y, uint32_t sampleSetIdx, int temporal,
         uint32_t M_max, uint32_t* out)
     {
         using namespace orc;
+        const uint4* core = (const uint4*)core_;
+        const uint2* me = (const uint2*)me_;
+        const uint2* coat = (const uint2*)coat_;
+        const uint4* pcore = (const uint4*)pcore_;
+        const uint2* pcoat = (const uint2*)pcoat_;
         Frame f;
         f.sc = (const Scene*)scene; f.fc = fc; f.core = core; f.me = me; f.coat = coat; f.pcore = pcore; f.pcoat = pcoat;
         f.W = fc->RenderWidth; f.H = fc->RenderHeight;
@@ -655,13 +661,18 @@ extern "C"
 
     void orc_rdi_set_sample_pattern(const float* p) { g_disk32 = p; }
 
-    struct orc_rdi_params { uint32_t temporal_resample, spatial_resample, stochastic_spatial, extra_disocclusion_sampling, M_max; float alpha_min; };
-
     // state[0] = currTemporalIdx, state[1] = isTemporalReservoirValid, state[2] = reset flag
-    void orc_rdi_render(void* scene_, const zr_frame_constants* fc, const uint4* core, const uint2* me, const uint2* coat,
-        const uint4* pcore, const uint2* pcoat, const orc_rdi_params* p, zr_rdi_reservoir* res0, zr_rdi_reservoir* res1,
-        uint2* target, float4* finalImg, uint32_t* state, int nthreads)
+    void orc_rdi_render(void* scene_, const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* me_, const uint32_t* coat_,
+        const uint32_t* pcore_, const uint32_t* pcoat_, const zr_direct_params* p, zr_rdi_reservoir* res0, zr_rdi_reservoir* res1,
+        uint32_t* target_, float* finalImg_, uint32_t* state, int nthreads)
     {
+        const uint4* core = (const uint4*)core_;
+        const uint2* me = (const uint2*)me_;
+        const uint2* coat = (const uint2*)coat_;
+        const uint4* pcore = (const uint4*)pcore_;
+        const uint2* pcoat = (const uint2*)pcoat_;
+        uint2* target = (uint2*)target_;
+        float4* finalImg = (float4*)finalImg_;
         Frame f;
         f.sc = (Scene*)scene_; f.fc = fc; f.core = core; f.me = me; f.coat = coat; f.pcore = pcore; f.pcoat = pcoat;
         f.W = fc->RenderWidth; f.H = fc->RenderHeight;
@@ -684,10 +695,12 @@ extern "C"
     // Pairwise-MIS spatial reuse (PairwiseMIS.hlsli) of the centre pixel (x, y) with neighbours (nx[i], ny[i]): the centre reservoir is
     // completed from the emissive buffer + target plane as k_di_spatial does it; neighbours enter with their own LoadPixel surface.
     // out (14 words): the resulting 32-byte record (Write with M_max 0 = no clamp), target (3), W, m_c, rng state
-    void orc_probe_rdi_pairwise(void* scene, const zr_frame_constants* fc, const orc::uint4* core, const orc::uint2* coat,
+    void orc_probe_rdi_pairwise(void* scene, const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* coat_,
         const zr_rdi_reservoir* res, const void* target, int x, int y, const int* nx, const int* ny, int numNeighbors, uint32_t seed, uint32_t* out)
     {
         using namespace orc;
+        const uint4* core = (const uint4*)core_;
+        const uint2* coat = (const uint2*)coat_;
         Frame f;
         f.sc = (const Scene*)scene; f.fc = fc; f.core = core; f.me = nullptr; f.coat = coat; f.pcore = core; f.pcoat = coat;
         f.W = fc->RenderWidth; f.H = fc->RenderHeight;

@@ -18,6 +18,7 @@
 // are at the same iteration (lock-step, like the ReSTIR PT restatement); SuppressOutlierReservoirs sums over the lanes
 // that reached it, in the xor-butterfly order.
 // D3D semantics kept: texture reads outside the image return 0 (FindTemporalCandidate does not reject negative taps).
+#include "orc_api.h"
 #include "orc_pixel.h"
 
 namespace orc
@@ -743,11 +744,16 @@ extern "C"
     // Probe for the CPU-tier device-source parity test (tests/test_device_source_vs_oracle.py): ReSTIR GI's temporal reuse at one pixel,
     // starting from a given initial reservoir record. Mirrors EstimateIndirectLighting :564-596 (candidate search, one- or
     // two-candidate resampling). out: the resulting 48-byte record, then target_z (3 words), rng state, #valid candidates.
-    void orc_probe_rgi_temporal(void* scene, const zr_frame_constants* fc, const orc::uint4* core, const orc::uint2* me, const orc::uint2* coat,
-        const orc::uint4* pcore, const orc::uint2* pcoat, const zr_rgi_reservoir* prevRes, const zr_rgi_reservoir* initial, int x, int y,
+    void orc_probe_rgi_temporal(void* scene, const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* me_, const uint32_t* coat_,
+        const uint32_t* pcore_, const uint32_t* pcoat_, const zr_rgi_reservoir* prevRes, const zr_rgi_reservoir* initial, int x, int y,
         uint32_t seed, uint32_t M_max, uint32_t* out)
     {
         using namespace orc;
+        const uint4* core = (const uint4*)core_;
+        const uint2* me = (const uint2*)me_;
+        const uint2* coat = (const uint2*)coat_;
+        const uint4* pcore = (const uint4*)pcore_;
+        const uint2* pcoat = (const uint2*)pcoat_;
         Frame f;
         f.sc = (const Scene*)scene; f.fc = fc; f.core = core; f.me = me; f.coat = coat; f.pcore = pcore; f.pcoat = pcoat;
         f.W = fc->RenderWidth; f.H = fc->RenderHeight;
@@ -792,30 +798,40 @@ extern "C"
     }
 
     // IndirectLighting with INTEGRATOR::PATH_TRACING (IndirectLighting.cpp: RenderPathTracer; PathTracer/PathTracer.hlsl), emissive NEE.
-    // params: the same GIParams words (only the bounce budgets and the Russian-roulette flag are read).
-    void orc_pt_render(void* scene, const zr_frame_constants* fc, const orc::uint4* core, const orc::uint2* me, const orc::uint2* coat,
-        const uint32_t* params, orc::float4* finalImg, int nthreads)
+    // Of the parameters only the bounce budgets and the Russian-roulette flag are read.
+    void orc_pt_render(void* scene, const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* me_, const uint32_t* coat_,
+        const zr_gi_params* p, float* finalImg_, int nthreads)
     {
         using namespace orc;
+        const uint4* core = (const uint4*)core_;
+        const uint2* me = (const uint2*)me_;
+        const uint2* coat = (const uint2*)coat_;
+        float4* finalImg = (float4*)finalImg_;
         Frame f;
         f.sc = (const Scene*)scene; f.fc = fc; f.core = core; f.me = me; f.coat = coat; f.pcore = core; f.pcoat = coat;
         f.W = fc->RenderWidth; f.H = fc->RenderHeight;
-        GIParams prm;
-        memcpy(&prm, params, sizeof(prm));
+        const GIParams prm{ p->max_non_tr_bounces, p->max_glossy_tr_bounces, p->russian_roulette, p->stochastic_multi_bounce,
+            p->boiling_suppression, p->M_max, p->temporal_resample };
         RenderPass(f, prm, false, false, nullptr, nullptr, finalImg, nthreads, true);
     }
 
     // state[0] = currTemporalIdx, state[1] = isTemporalReservoirValid, state[2] = reset flag (IndirectLighting.cpp:277-368, :1021-1024)
-    void orc_rgi_render(void* scene, const zr_frame_constants* fc, const orc::uint4* core, const orc::uint2* me, const orc::uint2* coat,
-        const orc::uint4* pcore, const orc::uint2* pcoat, const uint32_t* params /* GIParams */, zr_rgi_reservoir* res0, zr_rgi_reservoir* res1,
-        orc::float4* finalImg, uint32_t* state, int nthreads)
+    void orc_rgi_render(void* scene, const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* me_, const uint32_t* coat_,
+        const uint32_t* pcore_, const uint32_t* pcoat_, const zr_gi_params* p, zr_rgi_reservoir* res0, zr_rgi_reservoir* res1,
+        float* finalImg_, uint32_t* state, int nthreads)
     {
         using namespace orc;
+        const uint4* core = (const uint4*)core_;
+        const uint2* me = (const uint2*)me_;
+        const uint2* coat = (const uint2*)coat_;
+        const uint4* pcore = (const uint4*)pcore_;
+        const uint2* pcoat = (const uint2*)pcoat_;
+        float4* finalImg = (float4*)finalImg_;
         Frame f;
         f.sc = (const Scene*)scene; f.fc = fc; f.core = core; f.me = me; f.coat = coat; f.pcore = pcore; f.pcoat = pcoat;
         f.W = fc->RenderWidth; f.H = fc->RenderHeight;
-        GIParams prm;
-        memcpy(&prm, params, sizeof(prm));
+        const GIParams prm{ p->max_non_tr_bounces, p->max_glossy_tr_bounces, p->russian_roulette, p->stochastic_multi_bounce,
+            p->boiling_suppression, p->M_max, p->temporal_resample };
         zr_rgi_reservoir* res[2] = { res0, res1 };
         const int cur = (int)state[0];
         const bool doTemporal = prm.temporalResample && state[1];

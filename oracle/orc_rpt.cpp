@@ -11,6 +11,7 @@
 // with the reference's lane -> pixel maps (16x8 / 8x8 / 16x16 groups, row-major lanes, group swizzle).
 // Deterministic choices where the reference is racy or unspecified (DESIGN.md): waves of a sort
 // group take their offsets in wave order; wave sums use the xor-butterfly order.
+#include "orc_api.h"
 #include "orc_rpt.h"
 #include "orc_pixel.h"
 #include <functional>
@@ -965,29 +966,19 @@ extern "C"
 {
     void orc_rpt_set_sample_pattern(const float* pattern512x2) { g_samplePattern = pattern512x2; }
 
-    struct orc_rpt_params
-    {
-        uint32_t max_non_tr_bounces, max_glossy_tr_bounces, russian_roulette, temporal_resample, num_spatial_passes;
-        uint32_t M_max_temporal, M_max_spatial, boiling_suppression, sort_temporal, sort_spatial;
-        float alpha_min;
-    };
-
-    struct orc_rpt_buffers
-    {
-        zr_rpt_reservoir* res[2];
-        float4* target;
-        float4* finalImg;
-        uint16_t* neighbor;
-        uint16_t* threadMapCtN;
-        uint16_t* threadMapNtC;
-    };
-
     // One IndirectLighting::Render. state[0] = currTemporalIdx, state[1] = isTemporalReservoirValid,
     // state[2] = reset-temporal-textures flag (all updated). last_stage: 0 = whole frame, 1 = stop after
     // PathTrace, 2 = after temporal, 3 = after spatial.
-    void orc_rpt_render(void* scene_, const zr_frame_constants* fc, const uint4* core, const uint2* me, const uint2* coat,
-        const uint4* pcore, const uint2* pcoat, const orc_rpt_params* p, orc_rpt_buffers* b, uint32_t* state, int last_stage, int nthreads)
+    void orc_rpt_render(void* scene_, const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* me_, const uint32_t* coat_,
+        const uint32_t* pcore_, const uint32_t* pcoat_, const zr_indirect_params* p, orc_rpt_buffers* b, uint32_t* state, int last_stage, int nthreads)
     {
+        const uint4* core = (const uint4*)core_;
+        const uint2* me = (const uint2*)me_;
+        const uint2* coat = (const uint2*)coat_;
+        const uint4* pcore = (const uint4*)pcore_;
+        const uint2* pcoat = (const uint2*)pcoat_;
+        float4* target = (float4*)b->target;
+        float4* finalImg = (float4*)b->finalImg;
         Frame f;
         f.sc = (Scene*)scene_; f.fc = fc; f.core = core; f.me = me; f.coat = coat; f.pcore = pcore; f.pcoat = pcoat;
         f.W = fc->RenderWidth; f.H = fc->RenderHeight;
@@ -1003,7 +994,7 @@ extern "C"
         zr_rpt_reservoir* resCurr = b->res[cur];
         zr_rpt_reservoir* resPrev = b->res[1 - cur];
 
-        PathTracePass(f, prm, doTemporal, state[2] != 0, resCurr, b->target, b->finalImg, nthreads);
+        PathTracePass(f, prm, doTemporal, state[2] != 0, resCurr, target, finalImg, nthreads);
         if (doTemporal && last_stage != 1)
         {
             if (prm.sortTemporal)
@@ -1012,7 +1003,7 @@ extern "C"
                 SortPass(f, 0, doSpatial, resCurr, resPrev, nullptr, b->threadMapCtN);
             }
             ReconnectCtT(f, prm, resCurr, resPrev, b->threadMapCtN, nthreads);
-            ReconnectTtC(f, prm, doSpatial, resCurr, resPrev, b->target, b->finalImg, b->threadMapNtC, nthreads);
+            ReconnectTtC(f, prm, doSpatial, resCurr, resPrev, target, finalImg, b->threadMapNtC, nthreads);
         }
         if (doSpatial && last_stage != 1 && last_stage != 2)
         {
@@ -1028,7 +1019,7 @@ extern "C"
                     SortPass(f, 3, true, in, nullptr, b->neighbor, b->threadMapNtC);
                 }
                 ReconnectCtS(f, prm, in, out, b->neighbor, b->threadMapCtN, nthreads);
-                ReconnectStC(f, prm, in, out, b->target, b->finalImg, b->neighbor, b->threadMapNtC, nthreads);
+                ReconnectStC(f, prm, in, out, target, finalImg, b->neighbor, b->threadMapNtC, nthreads);
             }
         }
         state[1] = 1;

@@ -13,6 +13,7 @@
 //                   w = h_i h_j * max(0, 1 - |dz| / (sigma_z z_c step)) * max(0, k_n n.n_c + (1 - k_n)) * max(0, 1 - |dl| / (sigma_l sqrt(var_c) + 1e-4));
 //                   colour' = sum w c / sum w, variance' = sum w^2 var / (sum w)^2, taps in row-major order, centre first
 // Storage: colour + variance as 4 x binary16 (variance in alpha), guide = {view depth f32, oct32 normal}.
+#include "orc_api.h"
 #include "orc_gbuffer.h"
 #include <thread>
 #include <vector>
@@ -47,9 +48,17 @@ extern "C"
 {
     // color: float4[w*h] noisy input; core / me: current G-buffer; prevGuide: uint2[w*h] {z, oct normal} of the previous frame;
     // histPrev / histCurr: uint4[w*h] {half4 colour | half m1, m2, N, 0}; cv: uint2[w*h]; guide: uint2[w*h]
-    void orc_svgf_temporal(const zr_frame_constants* fc, const uint4* core, const uint2* me, const float4* color, const uint2* prevGuide,
-        const uint4* histPrev, int historyValid, uint4* histCurr, uint2* cv, uint2* guide, int nthreads)
+    void orc_svgf_temporal(const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* me_, const float* color_, const uint32_t* prevGuide_,
+        const uint32_t* histPrev_, int historyValid, uint32_t* histCurr_, uint32_t* cv_, uint32_t* guide_, int nthreads)
     {
+        const uint4* core = (const uint4*)core_;
+        const uint2* me = (const uint2*)me_;
+        const float4* color = (const float4*)color_;
+        const uint2* prevGuide = (const uint2*)prevGuide_;
+        const uint4* histPrev = (const uint4*)histPrev_;
+        uint4* histCurr = (uint4*)histCurr_;
+        uint2* cv = (uint2*)cv_;
+        uint2* guide = (uint2*)guide_;
         const int W = (int)fc->RenderWidth, H = (int)fc->RenderHeight;
         rows(H, nthreads, [=](int y)
         {
@@ -125,9 +134,13 @@ extern "C"
     }
 
     // one a-trous iteration: in -> out (both uint2[w*h]); outF (float4[w*h], optional) receives the unquantised result as well
-    void orc_svgf_atrous(uint32_t W_, uint32_t H_, const uint2* guide, const uint2* in, uint2* out, float4* outF, uint32_t step,
+    void orc_svgf_atrous(uint32_t W_, uint32_t H_, const uint32_t* guide_, const uint32_t* in_, uint32_t* out_, float* outF_, uint32_t step,
         const float* params4, int nthreads)
     {
+        const uint2* guide = (const uint2*)guide_;
+        const uint2* in = (const uint2*)in_;
+        uint2* out = (uint2*)out_;
+        float4* outF = (float4*)outF_;
         const int W = (int)W_, H = (int)H_, s = (int)step;
         const SvgfParams prm{ params4[0], params4[1], params4[2], (uint32_t)params4[3] };
         const int R = (int)prm.radius;

@@ -1,5 +1,6 @@
 // ORACLE -- test infrastructure, not product code (see orc_math.h header).
 // Small C entry points so the CPU-only tests can probe codecs and the BSDF restatement directly.
+#include "orc_api.h"
 #include "orc_scene.h"
 #include "orc_rpt.h"
 #include "orc_pixel.h"
@@ -22,11 +23,6 @@ extern "C"
     uint32_t orc_pack_snorm16x2(float x, float y) { return pack_snorm16x2(f2(x, y)); }
     void orc_unpack_snorm16x2(uint32_t p, float* out) { float2 c = unpack_snorm16x2(p); out[0] = c.x; out[1] = c.y; }
 
-    struct orc_surface_desc
-    {
-        float normal[3], wo[3]; uint32_t metallic; float roughness; float baseColor[3]; float eta_curr, eta_next; uint32_t specTr;
-        float trDepth, subsurface, coat_weight; float coat_color[3]; float coat_roughness, coat_ior;
-    };
     static BSDF::ShadingData mk(const orc_surface_desc* d)
     {
         return BSDF::ShadingData::Init(f3(d->normal[0], d->normal[1], d->normal[2]), f3(d->wo[0], d->wo[1], d->wo[2]), d->metallic != 0,
@@ -178,8 +174,10 @@ extern "C"
 
     // LoadPixel (the per-pixel reconstruction every lighting kernel starts with) over a whole G-buffer.
     // out: 16 words per pixel {flags byte, roughness, z, pos(3), normal(3), origin(3), eta_next, then a BSDF sample's wi.x, pdf, bsdfOverPdf.x}
-    void orc_probe_load_pixels(void* scene_, const zr_frame_constants* fc, const orc::uint4* core, const orc::uint2* coat, int prev, uint32_t* out)
+    void orc_probe_load_pixels(void* scene_, const zr_frame_constants* fc, const uint32_t* core_, const uint32_t* coat_, int prev, uint32_t* out)
     {
+        const uint4* core = (const uint4*)core_;
+        const uint2* coat = (const uint2*)coat_;
         Frame f;
         f.sc = (const Scene*)scene_; f.fc = fc; f.core = core; f.me = nullptr; f.coat = coat; f.pcore = core; f.pcoat = coat;
         f.W = fc->RenderWidth; f.H = fc->RenderHeight;

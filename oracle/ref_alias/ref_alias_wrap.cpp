@@ -4,6 +4,7 @@
 //
 // Wraps: ZetaCore/Math/Sampling.cpp:13-158 (AliasTable_Normalize/Build/SampleAliasTable),
 //        ZetaCore/Math/Common.cpp:72-140 (KahanSum), ZetaCore/Utility/RNG.h:33-90.
+#include "ref_alias_api.h"
 #include <Math/Sampling.h>
 #include <Math/Common.h>
 #include <Utility/RNG.h>

@@ -9,6 +9,7 @@
 //   ZetaRenderPass/Common/FrameConstants.h   cbFrameConstants (field offsets: the per-frame constant block the passes receive)
 //   the RT::MeshInstance / EmissiveTriangle / Material field offsets
 // Nothing here is product code and no reference source is copied.
+#include "ref_scene_api.h"
 #include "ZetaCore/RayTracing/RtCommon.h"
 #include "ZetaCore/Core/Vertex.h"
 #include "ZetaRenderPass/Common/FrameConstants.h"

@@ -3,6 +3,7 @@
 // against brute force on scenes of the benchmark's size (10^5 - 10^6 triangles) in the CPU test tier, where no GPU exists.
 // Nothing here is shipped or used by the product; the product path is the same source compiled by nvcc for sm_90a.
 #include "prelude.h"
+#include "hostsim_api.h"
 struct ZrTraverseStats { unsigned long long nodes, tris; };
 static thread_local ZrTraverseStats g_stats;
 #define ZR_TRAVERSE_STATS g_stats
@@ -178,21 +179,16 @@ extern "C" int hostsim_trace_stats(const void* nodes, const float* leafTris, con
 // CPU tier can hold the two transcriptions of Common/BSDF.hlsli + BSDFSampling.hlsli to each other bit for bit ----
 extern "C"
 {
-    struct hostsim_surface_desc
-    {
-        float normal[3], wo[3]; uint32_t metallic; float roughness; float baseColor[3]; float eta_curr, eta_next; uint32_t specTr;
-        float trDepth, subsurface, coat_weight; float coat_color[3]; float coat_roughness, coat_ior;
-    };
     static const uint16_t* g_rho = nullptr;
     void hostsim_set_rho_lut(const uint16_t* data) { g_rho = data; }
-    static zr::BSDF::ShadingData mk(const hostsim_surface_desc* d)
+    static zr::BSDF::ShadingData mk(const orc_surface_desc* d)
     {
         using namespace zr;
         return BSDF::ShadingData::Init(f3(d->normal[0], d->normal[1], d->normal[2]), f3(d->wo[0], d->wo[1], d->wo[2]), d->metallic != 0,
             d->roughness, f3(d->baseColor[0], d->baseColor[1], d->baseColor[2]), d->eta_curr, d->eta_next, d->specTr != 0, d->trDepth,
             d->subsurface, d->coat_weight, f3(d->coat_color[0], d->coat_color[1], d->coat_color[2]), d->coat_roughness, d->coat_ior, g_rho);
     }
-    void hostsim_bsdf_sample(const hostsim_surface_desc* d, uint32_t seed, float* out)
+    void hostsim_bsdf_sample(const orc_surface_desc* d, uint32_t seed, float* out)
     {
         using namespace zr;
         BSDF::ShadingData s = mk(d);
@@ -202,7 +198,7 @@ extern "C"
         out[5] = b.bsdfOverPdf.x; out[6] = b.bsdfOverPdf.y; out[7] = b.bsdfOverPdf.z; out[8] = b.f.x; out[9] = b.f.y; out[10] = b.f.z;
         out[11] = asfloat(rng.State);
     }
-    void hostsim_bsdf_sample_nodiffuse(const hostsim_surface_desc* d, uint32_t seed, float* out)
+    void hostsim_bsdf_sample_nodiffuse(const orc_surface_desc* d, uint32_t seed, float* out)
     {
         using namespace zr;
         BSDF::ShadingData s = mk(d);
@@ -212,7 +208,7 @@ extern "C"
         out[5] = b.bsdfOverPdf.x; out[6] = b.bsdfOverPdf.y; out[7] = b.bsdfOverPdf.z; out[8] = b.f.x; out[9] = b.f.y; out[10] = b.f.z;
         out[11] = asfloat(rng.State);
     }
-    void hostsim_bsdf_eval_sampler(const hostsim_surface_desc* d, const float* wi, uint32_t lobe, uint32_t seed, float* out)
+    void hostsim_bsdf_eval_sampler(const orc_surface_desc* d, const float* wi, uint32_t lobe, uint32_t seed, float* out)
     {
         using namespace zr;
         BSDF::ShadingData s = mk(d);
@@ -221,20 +217,20 @@ extern "C"
         out[0] = e.pdf; out[1] = e.bsdfOverPdf.x; out[2] = e.bsdfOverPdf.y; out[3] = e.bsdfOverPdf.z; out[4] = e.f.x; out[5] = e.f.y; out[6] = e.f.z;
         out[7] = asfloat(rng.State);
     }
-    float hostsim_bsdf_sampler_pdf(const hostsim_surface_desc* d, const float* wi, uint32_t seed)
+    float hostsim_bsdf_sampler_pdf(const orc_surface_desc* d, const float* wi, uint32_t seed)
     {
         using namespace zr;
         BSDF::ShadingData s = mk(d);
         RNG rng; rng.State = seed;
         return BSDF::BSDFSamplerPdf(f3(d->normal[0], d->normal[1], d->normal[2]), s, f3(wi[0], wi[1], wi[2]), rng);
     }
-    float hostsim_bsdf_sampler_pdf_nodiffuse(const hostsim_surface_desc* d, const float* wi)
+    float hostsim_bsdf_sampler_pdf_nodiffuse(const orc_surface_desc* d, const float* wi)
     {
         using namespace zr;
         BSDF::ShadingData s = mk(d);
         return BSDF::BSDFSamplerPdf_NoDiffuse(f3(d->normal[0], d->normal[1], d->normal[2]), s, f3(wi[0], wi[1], wi[2]));
     }
-    void hostsim_bsdf_unified(const hostsim_surface_desc* d, const float* wi, float* out)
+    void hostsim_bsdf_unified(const orc_surface_desc* d, const float* wi, float* out)
     {
         using namespace zr;
         BSDF::ShadingData s = mk(d);
@@ -267,15 +263,6 @@ extern "C"
 // ---- ray-query / material / light-sampling device source (zr_rt.cuh) on a host-resident scene ----
 extern "C"
 {
-    struct hostsim_scene
-    {
-        const void* vertices; const uint32_t* indices; const void* instances; const void* materials; const void* emissives;
-        const void* aliasTable; const void* nodes; const float* leafTris; const uint32_t* triMesh; const uint32_t* meshFirstTri;
-        const uint16_t* rho; uint32_t numInstances, numEmissives, numTris;
-        // optional: presampled emissive sets and the light voxel grid, as the oracle built them
-        const void* sampleSets; uint32_t numSampleSets, sampleSetSize;
-        const void* lvg; uint32_t lvgDim[3]; float lvgExtents[3]; float lvgOffsetY;
-    };
     static zr::SceneDev dev_of(const hostsim_scene* h)
     {
         zr::SceneDev sc{};

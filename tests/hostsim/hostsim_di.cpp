@@ -2,6 +2,7 @@
 // one thread, behind probe entry points mirrored by the oracle (oracle/orc_rdi.cpp). A translation unit of its own: zr_rdi.cuh and
 // zr_rgi.cuh both live in the library's unnamed namespace and reuse names.
 #include "prelude.h"
+#include "hostsim_api.h"
 #include "../../zetaray_b200/csrc/zr_rdi.cuh"
 
 namespace zr
@@ -11,14 +12,7 @@ void set_error(const char*, ...) {}
 
 extern "C"
 {
-    struct hostsim_di_scene
-    {
-        const void* vertices; const uint32_t* indices; const void* instances; const void* materials; const void* emissives;
-        const void* aliasTable; const void* nodes; const float* leafTris; const uint32_t* triMesh; const uint32_t* meshFirstTri;
-        const uint16_t* rho; uint32_t numInstances, numEmissives, numTris;
-        const void* sampleSets; uint32_t numSampleSets, sampleSetSize;
-    };
-    static zr::SceneDev dev_of(const hostsim_di_scene* h)
+    static zr::SceneDev dev_of(const hostsim_scene* h)
     {
         zr::SceneDev sc{};
         sc.vertices = (const zr_vertex*)h->vertices; sc.indices = h->indices; sc.instances = (const zr_mesh_instance*)h->instances;
@@ -32,7 +26,7 @@ extern "C"
 
     // ReSTIR DI at one pixel as k_di_temporal does it: RIS over BSDF + light candidates, then (temporal != 0) the temporal candidate
     // and its resampling. out (14 words): the 32-byte reservoir record, target (3), rng state, candidate valid, #BSDF samples
-    void hostsim_probe_rdi_pixel(const hostsim_di_scene* hsc, const zr_frame_constants* fc, const void* core, const void* me, const void* coat,
+    void hostsim_probe_rdi_pixel(const hostsim_scene* hsc, const zr_frame_constants* fc, const void* core, const void* me, const void* coat,
         const void* pcore, const void* pcoat, const zr_rdi_reservoir* prevRes, int x, int y, uint32_t sampleSetIdx, int temporal, uint32_t M_max,
         uint32_t* out)
     {
@@ -69,7 +63,7 @@ extern "C"
     // Pairwise-MIS spatial reuse (PairwiseMIS.hlsli) of the centre pixel (x, y) with neighbours (nx[i], ny[i]): the centre reservoir is
     // completed from the emissive buffer + target plane as k_di_spatial does it; neighbours enter with their own LoadPixel surface.
     // out (14 words): the resulting 32-byte record (Write with M_max 0 = no clamp), target (3), W, m_c, rng state
-    void hostsim_probe_rdi_pairwise(const hostsim_di_scene* hsc, const zr_frame_constants* fc, const void* core, const void* coat,
+    void hostsim_probe_rdi_pairwise(const hostsim_scene* hsc, const zr_frame_constants* fc, const void* core, const void* coat,
         const zr_rdi_reservoir* res, const void* target, int x, int y, const int* nx, const int* ny, int numNeighbors, uint32_t seed, uint32_t* out)
     {
         using namespace zr;

@@ -1,6 +1,7 @@
 // hostsim_io.cpp -- TEST INFRASTRUCTURE. Host (g++) build of the ReSTIR PT per-pixel I/O helpers (zetaray_b200/csrc/zr_rpt_io.cuh) and the
 // storage codecs they rely on. A translation unit of its own: zr_rpt_io.cuh and zr_rgi.cuh reuse names in the library's unnamed namespace.
 #include "prelude.h"
+#include "hostsim_api.h"
 #include "../../zetaray_b200/csrc/zr_rpt_io.cuh"
 
 namespace zr

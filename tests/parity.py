@@ -171,7 +171,8 @@ def frame_parity(scene, w, h, nframes, passes, checks=None, di_params=None, rpt_
         setattr(R.di_params, k, v)
     for k, v in (rpt_params or {}).items():
         setattr(R.params, k, v)
-    R.gi_params.update(gi_params or {})
+    for k, v in (gi_params or {}).items():
+        setattr(R.gi_params, k, v)
     f = DeviceFrame(flat, w, h, passes, di_params, rpt_params, gi_params, presample, lvg)
     oracle = [getattr(R, p) for p in ("rdi", "rpt", "rgi", "pt") if p in passes]
     seq = rpt_util.FrameSequence(w, h, cam_path=cam_path, accumulate=accumulate)

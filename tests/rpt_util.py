@@ -5,7 +5,8 @@ import os
 import numpy as np
 
 from tests import scene_util, synth
-from tests.orc import ptr
+from tests.orc import RptBuffers, ptr
+from zetaray_b200 import _lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 RES = np.dtype([("meta", "<u4"), ("w_sum", "<f4"), ("W", "<f4"), ("L_b", "<u4"),
@@ -15,16 +16,9 @@ RES = np.dtype([("meta", "<u4"), ("w_sum", "<f4"), ("W", "<f4"), ("L_b", "<u4"),
 assert RES.itemsize == 64
 
 
-class RptParams(C.Structure):
-    _fields_ = [("max_non_tr_bounces", C.c_uint32), ("max_glossy_tr_bounces", C.c_uint32), ("russian_roulette", C.c_uint32),
-                ("temporal_resample", C.c_uint32), ("num_spatial_passes", C.c_uint32), ("M_max_temporal", C.c_uint32),
-                ("M_max_spatial", C.c_uint32), ("boiling_suppression", C.c_uint32), ("sort_temporal", C.c_uint32),
-                ("sort_spatial", C.c_uint32), ("alpha_min", C.c_float)]
-
-
 def default_rpt_params():
     # IndirectLighting.h:231-244, IndirectLighting.cpp:146-165
-    return RptParams(3, 4, 1, 1, 1, 10, 8, 1, 1, 1, np.float32(0.175) * np.float32(0.175))
+    return _lib.IndirectParams(3, 4, 1, 1, 1, 10, 8, 1, 1, 1, np.float32(0.175) * np.float32(0.175))
 
 
 RDI = np.dtype([("bary", "<u4"), ("le_rg", "<u4"), ("le_b_meta", "<u4"), ("lightIdx", "<u4"), ("w_sum", "<f4"), ("W", "<f4"),
@@ -32,32 +26,20 @@ RDI = np.dtype([("bary", "<u4"), ("le_rg", "<u4"), ("le_b_meta", "<u4"), ("light
 assert RDI.itemsize == 32
 
 
-class RdiParams(C.Structure):
-    _fields_ = [("temporal_resample", C.c_uint32), ("spatial_resample", C.c_uint32), ("stochastic_spatial", C.c_uint32),
-                ("extra_disocclusion_sampling", C.c_uint32), ("M_max", C.c_uint32), ("alpha_min", C.c_float)]
-
-
 def default_rdi_params():
     # DirectLighting.cpp:99-107, DirectLighting.h:93-98
-    return RdiParams(1, 1, 1, 1, 20, np.float32(0.05) * np.float32(0.05))
+    return _lib.DirectParams(1, 1, 1, 1, 20, np.float32(0.05) * np.float32(0.05))
 
 
 RGI = np.dtype([("pos", "<f4", 3), ("ID", "<u4"), ("Lo_rg", "<u4"), ("Lo_b_M", "<u4"), ("w_sum", "<f4"), ("W", "<f4"),
                 ("normal", "<u4"), ("pad", "<u4", 3)])
 assert RGI.itemsize == 48
-GI_PARAM_NAMES = ("max_non_tr_bounces", "max_glossy_tr_bounces", "russian_roulette", "stochastic_multi_bounce", "boiling_suppression",
-                  "M_max", "temporal_resample")
 
 
 def default_gi_params():
     # IndirectLighting.h:231-244
-    return dict(max_non_tr_bounces=3, max_glossy_tr_bounces=4, russian_roulette=1, stochastic_multi_bounce=1, boiling_suppression=1,
-                M_max=10, temporal_resample=1)
-
-
-class RptBuffers(C.Structure):
-    _fields_ = [("res0", C.c_void_p), ("res1", C.c_void_p), ("target", C.c_void_p), ("final", C.c_void_p),
-                ("neighbor", C.c_void_p), ("tmCtN", C.c_void_p), ("tmNtC", C.c_void_p)]
+    return _lib.GIParams(max_non_tr_bounces=3, max_glossy_tr_bounces=4, russian_roulette=1, stochastic_multi_bounce=1,
+                         boiling_suppression=1, M_max=10, temporal_resample=1)
 
 
 from zetaray_b200.camera import halton, FrameSequence  # noqa: E402,F401  (moved into the package)
@@ -110,7 +92,7 @@ class OracleRenderer:
 
     def rpt(self, fc, last_stage=0):
         c = self.gb[self.cur]; p = self.gb[self.cur ^ 1]
-        b = RptBuffers(self.res[0].ctypes.data, self.res[1].ctypes.data, self.target.ctypes.data, self.final.ctypes.data,
+        b = RptBuffers((self.res[0].ctypes.data, self.res[1].ctypes.data), self.target.ctypes.data, self.final.ctypes.data,
                        self.neighbor.ctypes.data, self.tmCtN.ctypes.data, self.tmNtC.ctypes.data)
         self.o.orc_rpt_render(self.osc.h, C.byref(fc), ptr(c[0]), ptr(c[2]), ptr(c[3]), ptr(p[0]), ptr(p[3]),
                               C.byref(self.params), C.byref(b), ptr(self.state), last_stage, self.nthreads)
@@ -124,15 +106,14 @@ class OracleRenderer:
     def rgi(self, fc):
         """IndirectLighting with INTEGRATOR::ReSTIR_GI"""
         c = self.gb[self.cur]; p = self.gb[self.cur ^ 1]
-        prm = np.array([self.gi_params[k] for k in GI_PARAM_NAMES], dtype=np.uint32)
-        self.o.orc_rgi_render(self.osc.h, C.byref(fc), ptr(c[0]), ptr(c[2]), ptr(c[3]), ptr(p[0]), ptr(p[3]), ptr(prm),
+        self.o.orc_rgi_render(self.osc.h, C.byref(fc), ptr(c[0]), ptr(c[2]), ptr(c[3]), ptr(p[0]), ptr(p[3]), C.byref(self.gi_params),
                               ptr(self.gi_res[0]), ptr(self.gi_res[1]), ptr(self.gi_final), ptr(self.gi_state), self.nthreads)
 
     def pt(self, fc):
         """IndirectLighting with INTEGRATOR::PATH_TRACING (the plain path tracer); writes gi_final like rgi()."""
         c = self.gb[self.cur]
-        prm = np.array([self.gi_params[k] for k in GI_PARAM_NAMES], dtype=np.uint32)
-        self.o.orc_pt_render(self.osc.h, C.byref(fc), ptr(c[0]), ptr(c[2]), ptr(c[3]), ptr(prm), ptr(self.gi_final), self.nthreads)
+        self.o.orc_pt_render(self.osc.h, C.byref(fc), ptr(c[0]), ptr(c[2]), ptr(c[3]), C.byref(self.gi_params), ptr(self.gi_final),
+                             self.nthreads)
 
     def gi_curr_reservoirs(self):
         return self.gi_res[1 - int(self.gi_state[0])]
@@ -151,7 +132,7 @@ class OracleRenderer:
             self.o.orc_firefly(C.byref(fc), ptr(c[0]), ptr(comp), ptr(out))
             comp = out
         taa = np.zeros((n, 2), dtype=np.uint32)
-        self.o.orc_taa(C.byref(fc), ptr(c[0]), ptr(c[2]), ptr(comp), ptr(taa_prev), ptr(taa), C.c_float(0.1), int(taa_valid))
+        self.o.orc_taa(C.byref(fc), ptr(c[0]), ptr(c[2]), ptr(comp), ptr(taa_prev), ptr(taa), 0.1, int(taa_valid))
         return comp, taa
 
     def curr_reservoirs(self):

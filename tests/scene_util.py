@@ -153,7 +153,6 @@ class OracleScene:
         self.lut = rho_lut()
         self.o.orc_set_rho_lut(ptr(self.lut))
         self.alias = np.zeros(max(len(flat.emissives), 1), dtype=ALIAS_ENTRY)
-        self.o.orc_scene_create.restype = C.c_void_p
         self.h = C.c_void_p(self.o.orc_scene_create(ptr(flat.vertices), ptr(flat.indices), ptr(flat.instances),
                                                     len(flat.instances), ptr(flat.instance_num_tris), ptr(flat.materials),
                                                     ptr(flat.emissives) if len(flat.emissives) else None, len(flat.emissives),
@@ -162,7 +161,7 @@ class OracleScene:
             self.power = np.zeros(len(flat.emissives), dtype=np.float32)
             self.o.orc_estimate_power(self.h, ptr(self.power))
             w = self.power.copy()
-            self.o.orc_alias_build_emissive(ptr(w), C.c_int64(len(w)), 0, ptr(self.alias))
+            self.o.orc_alias_build_emissive(ptr(w), len(w), 0, ptr(self.alias))
 
     def set_presampling(self, num_sets, set_size):
         """PresampleEmissives: num_sets x set_size records of 40 bytes; 0, 0 switches back to alias-table sampling."""
@@ -172,7 +171,7 @@ class OracleScene:
 
     def presample(self, frame_num):
         if getattr(self, "num_sets", 0):
-            self.o.orc_presample(self.h, C.c_uint32(frame_num), C.c_uint32(self.num_sets * self.set_size), ptr(self.sample_sets))
+            self.o.orc_presample(self.h, frame_num, self.num_sets * self.set_size, ptr(self.sample_sets))
 
     def set_light_voxel_grid(self, grid_dim, extents, offset_y=0.0):
         self.lvg_dim = tuple(grid_dim)
@@ -180,7 +179,7 @@ class OracleScene:
         self.lvg = np.zeros(max(n, 1) * 64 * 8, dtype=np.uint32)            # 32-byte records
         d = (C.c_uint32 * 3)(*grid_dim)
         e = (C.c_float * 3)(*extents)
-        self.o.orc_scene_set_lvg(self.h, ptr(self.lvg) if n else None, d, e, C.c_float(offset_y))
+        self.o.orc_scene_set_lvg(self.h, ptr(self.lvg) if n else None, d, e, offset_y)
 
     def build_light_voxel_grid(self, fc):
         if getattr(self, "lvg_dim", None) and self.lvg_dim[0]:

@@ -24,7 +24,7 @@ def test_alias_build_bit_exact(oracle, n):
     w = np.array([1, 22, 4, 8, 3.5, 10], dtype=np.float32) if n == 6 else make_weights(n, n)
     ref = np.zeros(n, dtype=ALIAS_ENTRY)
     w_ref = w.copy()
-    oracle.orc_alias_build_emissive(ptr(w_ref), C.c_int64(n), 0, ptr(ref))
+    oracle.orc_alias_build_emissive(ptr(w_ref), n, 0, ptr(ref))
 
     d_w = dev(w)
     d_t = torch.zeros(n * 16, dtype=torch.uint8, device="cuda")
@@ -39,7 +39,7 @@ def test_alias_build_bit_exact(oracle, n):
 
     # sampling twin
     idx_ref = np.zeros(256, dtype=np.uint32); pdf_ref = np.zeros(256, dtype=np.float32)
-    oracle.orc_alias_sample_gpu(ptr(ref), C.c_uint32(n), C.c_uint32(0x1234567 + n), C.c_uint32(256), ptr(idx_ref), ptr(pdf_ref))
+    oracle.orc_alias_sample_gpu(ptr(ref), n, 0x1234567 + n, 256, ptr(idx_ref), ptr(pdf_ref))
     d_i = torch.zeros(256, dtype=torch.int32, device="cuda")
     d_p = torch.zeros(256, dtype=torch.float32, device="cuda")
     check(lib.zr_alias_table_sample(dptr(d_t), C.c_uint32(n), C.c_uint32(0x1234567 + n), C.c_uint32(256), dptr(d_i), dptr(d_p), stream()))

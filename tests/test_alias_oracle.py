@@ -3,7 +3,6 @@
 Pins oracle/orc_alias.cpp against (a) the golden vector of SURVEY 8c, (b) the outputs of the reference's own code
 (oracle/_ref/libref_alias.so) stored in tests/golden/reference_alias.npz by tools/make_reference_golden.py (bit-exact,
 including the pointer-alignment dependence of KahanSum), and re-states the reference's three doctest cases with fixed seeds."""
-import ctypes as C
 import hashlib
 import os
 import numpy as np
@@ -34,7 +33,7 @@ def aligned(n, dtype=np.float32, offset_elems=0):
 def orc_build(o, w, prologue=0):
     w = w.astype(np.float32).copy()
     t = np.zeros(len(w), dtype=ENTRY)
-    o.orc_alias_build(ptr(w), C.c_int64(len(w)), C.c_int(prologue), ptr(t))
+    o.orc_alias_build(ptr(w), len(w), prologue, ptr(t))
     return t, w
 
 
@@ -42,7 +41,7 @@ def ref_build(r, w, prologue=0):
     buf = aligned(len(w), np.float32, prologue)
     buf[:] = w
     t = np.zeros(len(w), dtype=ENTRY)
-    r.ref_alias_build(ptr(buf), C.c_int64(len(w)), ptr(t))
+    r.ref_alias_build(ptr(buf), len(w), ptr(t))
     return t, buf.copy()
 
 
@@ -54,14 +53,14 @@ def test_golden_vector(oracle):
         assert abs(t["P_Orig"][i] - po) < 1e-8
     idx = np.zeros(5, dtype=np.uint32)
     pdf = np.zeros(5, dtype=np.float32)
-    oracle.orc_alias_sample(ptr(t), C.c_int64(6), C.c_uint64(12345), 5, ptr(idx), ptr(pdf))
+    oracle.orc_alias_sample(ptr(t), 6, 12345, 5, ptr(idx), ptr(pdf))
     assert idx.tolist() == [1, 1, 5, 5, 5]
 
 
 def test_normalize(oracle):
     # TestAliasTable.cpp:14-28
     w = GOLDEN_W.copy()
-    oracle.orc_alias_normalize(ptr(w), C.c_int64(6), 0)
+    oracle.orc_alias_normalize(ptr(w), 6, 0)
     s = np.float32(0)
     for e in w:
         s = np.float32(s + e)
@@ -72,17 +71,17 @@ def test_normalize(oracle):
 def test_returned_pdf_matches_original(oracle, seed):
     # TestAliasTable.cpp:30-67 with fixed seeds
     n_buf = np.zeros(1, dtype=np.uint32)
-    oracle.orc_rng64_stream(C.c_uint64(seed), 2, 999, 1, ptr(n_buf), None)
+    oracle.orc_rng64_stream(seed, 2, 999, 1, ptr(n_buf), None)
     n = 1 + int(n_buf[0])
     f = np.zeros(n + 1, dtype=np.float32)
-    oracle.orc_rng64_stream(C.c_uint64(seed + 7), 1, 0, n, None, ptr(f))
+    oracle.orc_rng64_stream(seed + 7, 1, 0, n, None, ptr(f))
     vals = (f[:n] * np.float32(100.0)).astype(np.float32)
-    s = oracle.orc_kahan_sum(ptr(vals), C.c_int64(n), 0)
+    s = oracle.orc_kahan_sum(ptr(vals), n, 0)
     normalized = vals / np.float32(s)
     t, _ = orc_build(oracle, vals)
     idx = np.zeros(100, dtype=np.uint32)
     pdf = np.zeros(100, dtype=np.float32)
-    oracle.orc_alias_sample(ptr(t), C.c_int64(n), C.c_uint64(seed), 100, ptr(idx), ptr(pdf))
+    oracle.orc_alias_sample(ptr(t), n, seed, 100, ptr(idx), ptr(pdf))
     assert (idx < n).all()
     assert np.abs(pdf - normalized[idx]).max() < 1e-7
 
@@ -92,14 +91,14 @@ def test_density_chi_squared(oracle, seed):
     # TestAliasTable.cpp:69-121
     n = 50
     u = np.zeros(n, dtype=np.uint32)
-    oracle.orc_rng64_stream(C.c_uint64(seed), 2, 1000, n, ptr(u), None)
+    oracle.orc_rng64_stream(seed, 2, 1000, n, ptr(u), None)
     vals = u.astype(np.float32)
-    s = oracle.orc_kahan_sum(ptr(vals), C.c_int64(n), 0)
+    s = oracle.orc_kahan_sum(ptr(vals), n, 0)
     normalized = vals / np.float32(s)
     t, _ = orc_build(oracle, vals)
     idx = np.zeros(100, dtype=np.uint32)
     pdf = np.zeros(100, dtype=np.float32)
-    oracle.orc_alias_sample(ptr(t), C.c_int64(n), C.c_uint64(seed * 31 + 1), 100, ptr(idx), ptr(pdf))
+    oracle.orc_alias_sample(ptr(t), n, seed * 31 + 1, 100, ptr(idx), ptr(pdf))
     count = np.bincount(idx, minlength=n).astype(np.float64)
     expected = normalized.astype(np.float64) * 100
     chi = np.where(expected == 0, 0, (count - expected) ** 2 / np.where(expected == 0, 1, expected)).sum()
@@ -125,15 +124,15 @@ def reference_alias_outputs(reflib):
             buf = aligned(n, np.float32, prologue)
             buf[:] = w
             key = "n%d_p%d" % (n, prologue)
-            out[key + "_kahan"] = np.float32(reflib.ref_kahan_sum(ptr(buf), C.c_int64(n)))
+            out[key + "_kahan"] = np.float32(reflib.ref_kahan_sum(ptr(buf), n))
             t, _ = ref_build(reflib, w, prologue)
             out[key + "_table"] = t if n <= REF_FULL_TABLE_MAX_N else np.array(hashlib.sha256(t.tobytes()).hexdigest())
             idx = np.zeros(200, dtype=np.uint32); pdf = np.zeros(200, dtype=np.float32)
-            reflib.ref_alias_sample(ptr(t), C.c_int64(n), C.c_uint64(12345), 200, ptr(idx), ptr(pdf))
+            reflib.ref_alias_sample(ptr(t), n, 12345, 200, ptr(idx), ptr(pdf))
             out[key + "_idx"], out[key + "_pdf"] = idx, pdf
     for sid in RNG_STREAMS:
         a = np.zeros(64, dtype=np.uint32)
-        reflib.ref_rng_stream(C.c_uint64(sid), 0, 0, 64, ptr(a), None)
+        reflib.ref_rng_stream(sid, 0, 0, 64, ptr(a), None)
         out["rng_%x" % sid] = a
     out["halton"] = np.array([[reflib.ref_halton(i, base) for base in (2, 3)] for i in range(1, 70)], dtype=np.float32)
     return out
@@ -155,7 +154,7 @@ def test_bit_exact_vs_reference(oracle, golden_ref, n, prologue):
             pytest.skip("reference reads out of bounds for short unaligned spans")
     w = ref_case_weights(n, prologue)
     key = "n%d_p%d" % (n, prologue)
-    ks_orc = oracle.orc_kahan_sum(ptr(w.copy()), C.c_int64(n), prologue)
+    ks_orc = oracle.orc_kahan_sum(ptr(w.copy()), n, prologue)
     assert golden_ref[key + "_kahan"].tobytes() == np.float32(ks_orc).tobytes()
     t_orc, w_orc = orc_build(oracle, w, prologue)
     t_ref = golden_ref[key + "_table"]
@@ -166,14 +165,14 @@ def test_bit_exact_vs_reference(oracle, golden_ref, n, prologue):
         assert t_ref["P_Curr"].tobytes() == t_orc["P_Curr"].tobytes()
         assert t_ref["P_Orig"].tobytes() == t_orc["P_Orig"].tobytes()
     idx_o = np.zeros(200, dtype=np.uint32); pdf_o = np.zeros(200, dtype=np.float32)
-    oracle.orc_alias_sample(ptr(t_orc), C.c_int64(n), C.c_uint64(12345), 200, ptr(idx_o), ptr(pdf_o))
+    oracle.orc_alias_sample(ptr(t_orc), n, 12345, 200, ptr(idx_o), ptr(pdf_o))
     assert (golden_ref[key + "_idx"] == idx_o).all() and golden_ref[key + "_pdf"].tobytes() == pdf_o.tobytes()
 
 
 def test_rng_and_halton_vs_reference(oracle, golden_ref):
     for sid in RNG_STREAMS:
         b = np.zeros(64, dtype=np.uint32)
-        oracle.orc_rng64_stream(C.c_uint64(sid), 0, 0, 64, ptr(b), None)
+        oracle.orc_rng64_stream(sid, 0, 0, 64, ptr(b), None)
         assert (golden_ref["rng_%x" % sid] == b).all()
     for i in range(1, 70):
         for j, base in enumerate((2, 3)):
@@ -187,7 +186,7 @@ def test_emissive_table_consistent_with_twin(oracle):
     t, _ = orc_build(oracle, w)
     e = np.zeros(n, dtype=ALIAS_ENTRY)
     ww = w.copy()
-    oracle.orc_alias_build_emissive(ptr(ww), C.c_int64(n), 0, ptr(e))
+    oracle.orc_alias_build_emissive(ptr(ww), n, 0, ptr(e))
     assert (e["Alias"] == t["Alias"]).all()
     assert e["P_Curr"].tobytes() == t["P_Curr"].tobytes()
     assert e["CachedP_Orig"].tobytes() == t["P_Orig"].tobytes()

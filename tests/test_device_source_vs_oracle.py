@@ -9,12 +9,11 @@ import numpy as np
 import pytest
 
 from tests import hostsim, orc
-from tests.orc import ptr
-from tests.test_oracle_props import Surf
+from tests.orc import SurfaceDesc, ptr
 
 
 def random_surface(rng):
-    s = Surf()
+    s = SurfaceDesc()
     n = rng.normal(size=3); n /= np.linalg.norm(n)
     wo = rng.normal(size=3); wo /= np.linalg.norm(wo)
     if rng.random() < 0.85 and np.dot(wo, n) < 0:
@@ -47,8 +46,6 @@ def test_bsdf_device_source_is_bit_identical_to_the_oracle():
     o = orc.load()
     lut = scene_util.rho_lut()
     o.orc_set_rho_lut(ptr(lut)); hs.hostsim_set_rho_lut(ptr(lut))
-    o.orc_bsdf_sampler_pdf.restype = C.c_float
-    o.orc_bsdf_sampler_pdf_nodiffuse.restype = C.c_float
     rng = np.random.default_rng(42)
     a = (C.c_float * 12)(); b = (C.c_float * 12)()
     lobes_seen = set()
@@ -79,8 +76,6 @@ def test_storage_codecs_device_source_vs_oracle():
     emissive colour, SNORM16 motion vectors, halves."""
     hs = hostsim.load()
     o = orc.load()
-    for f in (o.orc_pack_r11g11b10, o.orc_pack_snorm16x2, hs.hostsim_pack_r11g11b10, hs.hostsim_pack_snorm16x2, hs.hostsim_pack_half2):
-        f.restype = C.c_uint32
     rng = np.random.default_rng(9)
     n = 20000
     v = rng.normal(size=(n, 3)); v /= np.linalg.norm(v, axis=1, keepdims=True)
@@ -91,30 +86,21 @@ def test_storage_codecs_device_source_vs_oracle():
     out_a = (C.c_float * 3)(); out_b = (C.c_float * 3)()
     cols = np.concatenate([rng.random((3000, 3)) * rng.choice([1e-3, 1.0, 50.0, 7e4], (3000, 1)), [[0, 0, 0], [65504, 1e-8, 1.0]]]).astype(np.float32)
     for c in cols:
-        pa = o.orc_pack_r11g11b10(C.c_float(c[0]), C.c_float(c[1]), C.c_float(c[2])); pb = hs.hostsim_pack_r11g11b10(C.c_float(c[0]), C.c_float(c[1]), C.c_float(c[2]))
+        pa = o.orc_pack_r11g11b10(c[0], c[1], c[2]); pb = hs.hostsim_pack_r11g11b10(c[0], c[1], c[2])
         assert pa == pb, (c, hex(pa), hex(pb))
         o.orc_unpack_r11g11b10(pa, out_a); hs.hostsim_unpack_r11g11b10(pa, out_b)
         assert bytes(out_a) == bytes(out_b)
     mv = np.concatenate([rng.normal(size=(3000, 2)) * 0.3, [[0, 0], [1, -1], [2, -2], [1e-6, -1e-6]]]).astype(np.float32)
     for m in mv:
-        pa = o.orc_pack_snorm16x2(C.c_float(m[0]), C.c_float(m[1])); pb = hs.hostsim_pack_snorm16x2(C.c_float(m[0]), C.c_float(m[1]))
+        pa = o.orc_pack_snorm16x2(m[0], m[1]); pb = hs.hostsim_pack_snorm16x2(m[0], m[1])
         assert pa == pb, (m, hex(pa), hex(pb))
         o.orc_unpack_snorm16x2(pa, out_a); hs.hostsim_unpack_snorm16x2(pa, out_b)
         assert bytes(out_a)[:8] == bytes(out_b)[:8]
     h = np.concatenate([rng.normal(size=4000) * rng.choice([1e-6, 1.0, 300.0, 1e5], 4000), [0.0, -0.0, 65504.0, 65520.0, 1e-8, np.inf]]).astype(np.float32)
-    mine = np.array([hs.hostsim_pack_half2(C.c_float(x), C.c_float(-x)) for x in h], dtype=np.uint32)
+    mine = np.array([hs.hostsim_pack_half2(x, -x) for x in h], dtype=np.uint32)
     with np.errstate(over="ignore"):
         want = h.astype(np.float16).view(np.uint16).astype(np.uint32) | ((-h).astype(np.float16).view(np.uint16).astype(np.uint32) << 16)
     assert np.array_equal(mine, want)
-
-
-class HostScene(C.Structure):
-    _fields_ = [("vertices", C.c_void_p), ("indices", C.c_void_p), ("instances", C.c_void_p), ("materials", C.c_void_p),
-                ("emissives", C.c_void_p), ("aliasTable", C.c_void_p), ("nodes", C.c_void_p), ("leafTris", C.c_void_p),
-                ("triMesh", C.c_void_p), ("meshFirstTri", C.c_void_p), ("rho", C.c_void_p),
-                ("numInstances", C.c_uint32), ("numEmissives", C.c_uint32), ("numTris", C.c_uint32),
-                ("sampleSets", C.c_void_p), ("numSampleSets", C.c_uint32), ("sampleSetSize", C.c_uint32),
-                ("lvg", C.c_void_p), ("lvgDim", C.c_uint32 * 3), ("lvgExtents", C.c_float * 3), ("lvgOffsetY", C.c_float)]
 
 
 @pytest.mark.parametrize("which,detail,nq", [("cornell", None, 3000), ("atrium", 0.5, 1200), ("tunnel", 0.35, 600)])
@@ -140,7 +126,7 @@ def test_ray_query_material_and_light_sampling_device_source_vs_oracle(which, de
     wt, tri_mesh, first = world_tris(flat)
     nodes, order, leaf, info = build(wt)
     keep = [np.ascontiguousarray(x) for x in (flat.vertices, flat.indices, flat.instances, flat.materials, flat.emissives, osc.alias)]
-    hsc = HostScene(*[k.ctypes.data for k in keep], nodes.ctypes.data, leaf.ctypes.data, tri_mesh.ctypes.data, first.ctypes.data,
+    hsc = hostsim.Scene(*[k.ctypes.data for k in keep], nodes.ctypes.data, leaf.ctypes.data, tri_mesh.ctypes.data, first.ctypes.data,
                     lut.ctypes.data, len(flat.instances), len(flat.emissives), len(wt))
 
     def closest(rays):
@@ -233,14 +219,14 @@ def test_restir_pt_hybrid_shift(which):
     wt, tri_mesh, first = world_tris(flat)
     nodes, order, leaf, info = build(wt)
     keep = [np.ascontiguousarray(x) for x in (flat.vertices, flat.indices, flat.instances, flat.materials, flat.emissives, osc.alias)]
-    hsc = HostScene(*[k.ctypes.data for k in keep], nodes.ctypes.data, leaf.ctypes.data, tri_mesh.ctypes.data, first.ctypes.data,
+    hsc = hostsim.Scene(*[k.ctypes.data for k in keep], nodes.ctypes.data, leaf.ctypes.data, tri_mesh.ctypes.data, first.ctypes.data,
                     osc.lut.ctypes.data, len(flat.instances), len(flat.emissives), len(wt))
     rays = _camera_rays(np.array(cam, dtype=np.float32), w, h)
     rng = np.random.default_rng(17)
     nonempty = np.nonzero((res["meta"] & 0xf) != 15)[0]
     a = (C.c_uint32 * 8)(); b = (C.c_uint32 * 8)()
     stats = dict(valid=0, kgt2=0, nonzero=0, replay_ok=0)
-    alpha_min = C.c_float(float(np.float32(0.175) * np.float32(0.175)))
+    alpha_min = float(np.float32(0.175) * np.float32(0.175))
     for it in range(2500):
         src = int(nonempty[rng.integers(0, len(nonempty))])
         sx, sy = src % w, src // w
@@ -273,7 +259,7 @@ def test_load_pixel_reconstruction(which, dof):
     hs.hostsim_set_rho_lut(ptr(osc.lut))
     cam = scene_util.CAMERAS.get(which, (0.0, 1.2, -4.043))
     seq = rpt_util.FrameSequence(w, h, cam_path=lambda f: (cam[0] + 0.03 * f, cam[1], cam[2] + 0.02 * f))
-    hsc = HostScene()
+    hsc = hostsim.Scene()
     hsc.rho = osc.lut.ctypes.data
     for fr in range(2):
         fc = seq.next()
@@ -303,7 +289,7 @@ def test_presampled_sets_and_light_voxel_grid_consumers():
     cam = scene_util.CAMERAS["atrium_lights"]
     fc = rpt_util.FrameSequence(w, h, cam_path=lambda f: cam).next()
     core, depth, me, coat, _ = R.gbuffer(fc)          # runs presampling and the grid build for this frame
-    hsc = HostScene()
+    hsc = hostsim.Scene()
     keep = [np.ascontiguousarray(x) for x in (flat.emissives, osc.alias)]
     hsc.emissives, hsc.aliasTable = keep[0].ctypes.data, keep[1].ctypes.data
     hsc.numEmissives = len(flat.emissives)
@@ -346,7 +332,7 @@ def test_restir_gi_temporal_reuse(which, dof):
 
     def frames(temporal_last):
         R = rpt_util.OracleRenderer(flat, w, h)
-        R.gi_params.update(stochastic_multi_bounce=0)
+        R.gi_params.stochastic_multi_bounce = 0
         seq = rpt_util.FrameSequence(w, h, cam_path=path)
         out = []
         for fr in range(3):
@@ -354,7 +340,7 @@ def test_restir_gi_temporal_reuse(which, dof):
             if dof:
                 fc.DoF, fc.FocusDepth, fc.LensRadius = 1, 4.0, 0.02
             if fr == 2:
-                R.gi_params.update(temporal_resample=int(temporal_last))
+                R.gi_params.temporal_resample = int(temporal_last)
             gb = R.gbuffer(fc)
             prev_res = R.gi_curr_reservoirs().copy()
             R.rgi(fc)
@@ -367,7 +353,7 @@ def test_restir_gi_temporal_reuse(which, dof):
     wt, tri_mesh, first = world_tris(flat)
     nodes, order, leaf, info = build(wt)
     keep = [np.ascontiguousarray(x) for x in (flat.vertices, flat.indices, flat.instances, flat.materials, flat.emissives, osc.alias)]
-    hsc = HostScene()
+    hsc = hostsim.Scene()
     (hsc.vertices, hsc.indices, hsc.instances, hsc.materials, hsc.emissives, hsc.aliasTable) = [k.ctypes.data for k in keep]
     hsc.nodes, hsc.leafTris, hsc.triMesh, hsc.meshFirstTri, hsc.rho = nodes.ctypes.data, leaf.ctypes.data, tri_mesh.ctypes.data, first.ctypes.data, osc.lut.ctypes.data
     hsc.numInstances, hsc.numEmissives, hsc.numTris = len(flat.instances), len(flat.emissives), len(wt)
@@ -389,14 +375,6 @@ def test_restir_gi_temporal_reuse(which, dof):
         changed += bytes(a)[:16] != ini.tobytes()[:16]      # the resampled reservoir picked the temporal sample
     print(which, "candidates 0/1/2:", ncand, "sample replaced:", changed)
     assert ncand[1] + ncand[2] > 1000 and changed > 50, (ncand, changed)
-
-
-class HostSceneDI(C.Structure):
-    _fields_ = [("vertices", C.c_void_p), ("indices", C.c_void_p), ("instances", C.c_void_p), ("materials", C.c_void_p),
-                ("emissives", C.c_void_p), ("aliasTable", C.c_void_p), ("nodes", C.c_void_p), ("leafTris", C.c_void_p),
-                ("triMesh", C.c_void_p), ("meshFirstTri", C.c_void_p), ("rho", C.c_void_p),
-                ("numInstances", C.c_uint32), ("numEmissives", C.c_uint32), ("numTris", C.c_uint32),
-                ("sampleSets", C.c_void_p), ("numSampleSets", C.c_uint32), ("sampleSetSize", C.c_uint32)]
 
 
 @pytest.mark.parametrize("which,presample", [("cornell", None), ("glossy", None), ("glass", (16, 64)), ("atrium", None)])
@@ -427,7 +405,7 @@ def test_restir_di_candidates_and_temporal_reuse(which, presample):
         osc.set_presampling(*presample)        # world_tris() created a second oracle scene; keep this one's configuration in force
     nodes, order, leaf, info = build(wt)
     keep = [np.ascontiguousarray(x) for x in (flat.vertices, flat.indices, flat.instances, flat.materials, flat.emissives, osc.alias)]
-    hsc = HostSceneDI()
+    hsc = hostsim.Scene()
     (hsc.vertices, hsc.indices, hsc.instances, hsc.materials, hsc.emissives, hsc.aliasTable) = [k.ctypes.data for k in keep]
     hsc.nodes, hsc.leafTris, hsc.triMesh, hsc.meshFirstTri, hsc.rho = nodes.ctypes.data, leaf.ctypes.data, tri_mesh.ctypes.data, first.ctypes.data, osc.lut.ctypes.data
     hsc.numInstances, hsc.numEmissives, hsc.numTris = len(flat.instances), len(flat.emissives), len(wt)
@@ -474,7 +452,7 @@ def test_restir_di_pairwise_mis(which):
     wt, tri_mesh, first = world_tris(flat)
     nodes, order, leaf, info = build(wt)
     keep = [np.ascontiguousarray(x) for x in (flat.vertices, flat.indices, flat.instances, flat.materials, flat.emissives, osc.alias)]
-    hsc = HostSceneDI()
+    hsc = hostsim.Scene()
     (hsc.vertices, hsc.indices, hsc.instances, hsc.materials, hsc.emissives, hsc.aliasTable) = [k.ctypes.data for k in keep]
     hsc.nodes, hsc.leafTris, hsc.triMesh, hsc.meshFirstTri, hsc.rho = nodes.ctypes.data, leaf.ctypes.data, tri_mesh.ctypes.data, first.ctypes.data, osc.lut.ctypes.data
     hsc.numInstances, hsc.numEmissives, hsc.numTris = len(flat.instances), len(flat.emissives), len(wt)

@@ -85,11 +85,11 @@ def test_histogram_and_exposure_match_oracle(oracle, w, h):
     ae.Render(_fi(w, h), d_sig.data_ptr(), stream())
     got = _download(ae.GetOutput().d_ptr, np.zeros(2, dtype=np.float32))
     hist = np.zeros(256, dtype=np.uint32)
-    oracle.orc_lum_histogram(ptr(sig), C.c_uint32(w), C.c_uint32(0), C.c_uint32(h), C.byref(p), ptr(hist))
+    oracle.orc_lum_histogram(ptr(sig), w, 0, h, C.byref(p), ptr(hist))
     assert hist.sum() == w * h and hist[0] > 0 and hist[1] > 0
     assert np.array_equal(tap.bins, hist)
     state = np.zeros(2, dtype=np.float32)
-    oracle.orc_exposure(ptr(hist), C.c_uint32(w * h), C.byref(p), C.c_float(1 / 60), ptr(state))
+    oracle.orc_exposure(ptr(hist), w * h, C.byref(p), 1 / 60, ptr(state))
     assert got.tobytes() == state.tobytes(), (got, state)
     assert np.isfinite(state).all() and state[0] > 0
 
@@ -110,9 +110,9 @@ def test_exposure_sequence_and_reset(oracle, w, h):
         ae.Render(_fi(w, h, dt), dev(sig).data_ptr(), stream())
         got = _download(ae.GetOutput().d_ptr, np.zeros(2, dtype=np.float32))
         hist = np.zeros(256, dtype=np.uint32)
-        oracle.orc_lum_histogram(ptr(sig), C.c_uint32(w), C.c_uint32(0), C.c_uint32(h), C.byref(ae.params), ptr(hist))
+        oracle.orc_lum_histogram(ptr(sig), w, 0, h, C.byref(ae.params), ptr(hist))
         assert np.array_equal(tap.bins, hist), "frame %d" % f
-        oracle.orc_exposure(ptr(hist), C.c_uint32(w * h), C.byref(ae.params), C.c_float(dt), ptr(state))
+        oracle.orc_exposure(ptr(hist), w * h, C.byref(ae.params), dt, ptr(state))
         assert got.tobytes() == state.tobytes(), "frame %d: %s vs %s" % (f, got, state)
     ae.ResetTemporal()
     assert not _download(ae.GetOutput().d_ptr, np.zeros(2, dtype=np.float32)).any()
@@ -122,8 +122,8 @@ def test_exposure_sequence_and_reset(oracle, w, h):
     ae.Render(_fi(w, h, 0.5), d_sig.data_ptr(), stream())
     state = np.zeros(2, dtype=np.float32)
     hist = np.zeros(256, dtype=np.uint32)
-    oracle.orc_lum_histogram(ptr(sig), C.c_uint32(w), C.c_uint32(0), C.c_uint32(h), C.byref(ae.params), ptr(hist))
-    oracle.orc_exposure(ptr(hist), C.c_uint32(w * h), C.byref(ae.params), C.c_float(0.5), ptr(state))
+    oracle.orc_lum_histogram(ptr(sig), w, 0, h, C.byref(ae.params), ptr(hist))
+    oracle.orc_exposure(ptr(hist), w * h, C.byref(ae.params), 0.5, ptr(state))
     assert _download(ae.GetOutput().d_ptr, np.zeros(2, dtype=np.float32)).tobytes() == state.tobytes()
 
 
@@ -148,7 +148,7 @@ def test_display_matches_oracle_every_tonemapper(oracle, w, h):
             img = disp.GetOutput()
             assert (img.width, img.height, img.pitch_bytes, img.texel_bytes) == (w, h, 4 * w, 4)
             _download(img.d_ptr, out)
-            oracle.orc_display(ptr(taa), C.c_uint32(w), C.c_uint32(0), C.c_uint32(h), C.byref(disp.params), ptr(exposure), ptr(lut), ptr(ref))
+            oracle.orc_display(ptr(taa), w, 0, h, C.byref(disp.params), ptr(exposure), ptr(lut), ptr(ref))
             bad = np.flatnonzero(out != ref)
             assert bad.size == 0, "tonemapper %d auto %d: pixel %d is %08x, oracle %08x" % (tm, auto, bad[0], out[bad[0]], ref[bad[0]])
             assert (out >> 24 == 255).all()
@@ -180,12 +180,12 @@ def test_renderer_display_stage_on_cornell(oracle):
         assert taa.tobytes() == host_rows(plain.GetOutput()).tobytes(), "frame %d: TAA output changed" % fr
         comp = host_rows(R.compositing.GetOutput())
         hist = np.zeros(256, dtype=np.uint32)
-        oracle.orc_lum_histogram(ptr(comp), C.c_uint32(w), C.c_uint32(0), C.c_uint32(h), C.byref(R.auto_exposure.params), ptr(hist))
-        oracle.orc_exposure(ptr(hist), C.c_uint32(w * h), C.byref(R.auto_exposure.params), C.c_float(fc.dt), ptr(state))
+        oracle.orc_lum_histogram(ptr(comp), w, 0, h, C.byref(R.auto_exposure.params), ptr(hist))
+        oracle.orc_exposure(ptr(hist), w * h, C.byref(R.auto_exposure.params), fc.dt, ptr(state))
         got_state = _download(R.auto_exposure.GetOutput().d_ptr, np.zeros(2, dtype=np.float32))
         assert got_state.tobytes() == state.tobytes(), "frame %d: %s vs %s" % (fr, got_state, state)
         ref = np.zeros(w * h, dtype=np.uint32)
-        oracle.orc_display(ptr(taa), C.c_uint32(w), C.c_uint32(0), C.c_uint32(h), C.byref(R.display.params), ptr(state), ptr(lut), ptr(ref))
+        oracle.orc_display(ptr(taa), w, 0, h, C.byref(R.display.params), ptr(state), ptr(lut), ptr(ref))
         got = host_rows(R.GetDisplayOutput()).view(np.uint32).reshape(-1)
         assert got.tobytes() == ref.tobytes(), "frame %d: display image differs from the oracle" % fr
     assert len(np.unique(got & 0xffffff)) > 100

@@ -139,7 +139,7 @@ def test_rgb9e5_decode_every_exponent_and_mantissa_edge(oracle):
                 v.append((e << 27) | (int(mant[-1] - r if g else r) << 18) | (g << 9) | int(r))
     v = np.array(v, dtype=np.uint32)
     got = np.zeros((len(v), 3), dtype=np.float32)
-    oracle.orc_rgb9e5_decode(ptr(v), C.c_int64(len(v)), ptr(got))
+    oracle.orc_rgb9e5_decode(ptr(v), len(v), ptr(got))
     assert np.array_equal(got.astype(np.float64), decode_rgb9e5(v))      # exact: a 9-bit integer times a power of two
 
 
@@ -147,7 +147,7 @@ def test_srgb_oetf_all_binary16_inputs(oracle):
     h = np.arange(1 << 16, dtype=np.uint32).astype(np.uint16).view(np.float16)
     x = h[np.isfinite(h)].astype(np.float32)
     got = np.zeros_like(x)
-    oracle.orc_srgb_oetf(ptr(x), C.c_int64(len(x)), ptr(got))
+    oracle.orc_srgb_oetf(ptr(x), len(x), ptr(got))
     want = srgb_oetf(x.astype(np.float64))
     big = np.abs(want) > 1e30
     assert np.all(np.isinf(got[big]) | (np.abs(got[big] / want[big] - 1) < 1e-5))
@@ -155,7 +155,7 @@ def test_srgb_oetf_all_binary16_inputs(oracle):
     # the 8-bit codes the display writes
     u = x[(x >= 0) & (x <= 1)]
     g8 = np.zeros_like(u)
-    oracle.orc_srgb_oetf(ptr(u), C.c_int64(len(u)), ptr(g8))
+    oracle.orc_srgb_oetf(ptr(u), len(u), ptr(g8))
     code32 = np.floor(g8.astype(np.float64) * 255 + 0.5)
     code64 = np.floor(srgb_oetf(u) * 255 + 0.5)
     assert np.abs(code32 - code64).max() <= 1
@@ -171,7 +171,7 @@ def test_tonemappers(oracle, tm, saturation, agx_exp):
     rgb[:8] = [[0, 0, 0], [1, 1, 1], [1e4, 0, 0], [0, 5, 0], [0.18, 0.18, 0.18], [0.5, 0.2, 0.9], [100, 100, 100], [2, 0.01, 0.3]]
     got = np.zeros_like(rgb)
     p = disp_params(tm, 0, saturation, agx_exp)
-    oracle.orc_tonemap(ptr(rgb), C.c_int64(len(rgb)), C.byref(p), ptr(lut), ptr(got))
+    oracle.orc_tonemap(ptr(rgb), len(rgb), C.byref(p), ptr(lut), ptr(got))
     want = tonemap(rgb.astype(np.float64), tm, lut, saturation, agx_exp)
     # what reaches the display: saturate (NaN -> 0 as HLSL's saturate does)
     g = np.clip(np.nan_to_num(got.astype(np.float64), nan=0.0), 0, 1)
@@ -185,7 +185,7 @@ def test_agx_matrices_are_applied_as_row_vector_times_matrix(oracle):
     rgb = np.array([[x, 0, 0], [0, x, 0], [0, 0, x]], dtype=np.float32)
     got = np.zeros_like(rgb)
     p = disp_params(AGX_DEFAULT, 0)
-    oracle.orc_tonemap(ptr(rgb), C.c_int64(3), C.byref(p), None, ptr(got))
+    oracle.orc_tonemap(ptr(rgb), 3, C.byref(p), None, ptr(got))
     want_row = agx(rgb.astype(np.float64))
     want_col = agx(rgb.astype(np.float64), m=AGX_MAT.T, m_inv=AGX_MAT_INV.T)          # M applied to a column vector
     assert np.abs(got - want_row).max() < 1e-5
@@ -194,7 +194,7 @@ def test_agx_matrices_are_applied_as_row_vector_times_matrix(oracle):
 
 def _check_bins(oracle, rgba, p, tol=1e-3):
     got = np.zeros(len(rgba), dtype=np.uint32)
-    oracle.orc_lum_bins(ptr(rgba), C.c_int64(len(rgba)), C.byref(p), ptr(got))
+    oracle.orc_lum_bins(ptr(rgba), len(rgba), C.byref(p), ptr(got))
     want, t254, lum = bins64(rgba, p)
     # float32 and float64 may straddle a bin edge or the 1e-4 threshold only within rounding distance of it
     safe = (np.abs(t254 - np.round(t254)) > tol) & (np.abs(lum - 1e-4) > 1e-9) | np.isnan(lum)
@@ -225,7 +225,7 @@ def test_bin_mapping_edges(oracle):
     rgba[5, 0] = np.nan
     rgba[6, 0] = np.inf
     got = np.zeros(7, dtype=np.uint32)
-    oracle.orc_lum_bins(ptr(rgba), C.c_int64(7), C.byref(p), ptr(got))
+    oracle.orc_lum_bins(ptr(rgba), 7, C.byref(p), ptr(got))
     assert got[0] == 0                  # lum <= 1e-4
     assert got[1] == 1                  # just above: below MinLum saturates to 0 -> bin 1
     assert got[2] == 1                  # exactly MinLum
@@ -234,7 +234,7 @@ def test_bin_mapping_edges(oracle):
     assert got[5] == 1                  # NaN: saturate(NaN) = 0
     assert got[6] == 255                # +inf
     hist = np.zeros(256, dtype=np.uint32)
-    oracle.orc_lum_histogram(ptr(rgba), C.c_uint32(1), C.c_uint32(0), C.c_uint32(7), C.byref(p), ptr(hist))
+    oracle.orc_lum_histogram(ptr(rgba), 1, 0, 7, C.byref(p), ptr(hist))
     assert hist.sum() == 7 and hist[0] == 1 and hist[1] == 3 and hist[255] == 3
 
 
@@ -247,7 +247,7 @@ def test_exposure_sequence(oracle, prm):
     prev64 = 0.0
     for dt in (1 / 60, 1 / 30, 0.0, 0.25, 1e-3, 1 / 144):
         hist = rng.multinomial(W * H, rng.dirichlet(np.ones(256) * 0.3)).astype(np.uint32)
-        oracle.orc_exposure(ptr(hist), C.c_uint32(W * H), C.byref(p), C.c_float(dt), ptr(state))
+        oracle.orc_exposure(ptr(hist), W * H, C.byref(p), dt, ptr(state))
         exp64, adapted64 = exposure64(hist, W * H, p, np.float32(dt), prev64)
         assert abs(state[1] / adapted64 - 1) < 2e-5, (dt, state, adapted64)
         assert abs(state[0] / exp64 - 1) < 5e-5, (dt, state, exp64)
@@ -256,7 +256,7 @@ def test_exposure_sequence(oracle, prm):
     state = np.zeros(2, dtype=np.float32)
     hist = np.zeros(256, dtype=np.uint32)
     hist[0] = W * H
-    oracle.orc_exposure(ptr(hist), C.c_uint32(W * H), C.byref(p), C.c_float(10.0), ptr(state))
+    oracle.orc_exposure(ptr(hist), W * H, C.byref(p), 10.0, ptr(state))
     assert abs(state[1] / p.min_lum - 1) < 1e-6
 
 

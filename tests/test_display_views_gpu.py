@@ -45,7 +45,6 @@ class Frame:
         self.gb, self.gpass = GBuffers(w, h), GBufferRT()
         self.orc = OracleScene(flat)
         self.o = self.orc.o
-        self.o.orc_gbuffer_pick.restype = C.c_uint32
 
     def render(self, fc):
         from zetaray_b200 import _lib, lib, check
@@ -68,7 +67,7 @@ class Frame:
         out = np.zeros(n, dtype=np.uint32) if base is None else base.copy()
         if view:
             core, _, me, coat, _ = self.gb.download()
-            self.o.orc_display_view(ptr(core), ptr(me), ptr(coat), self.w, y0, y1, view, C.c_float(th), C.c_float(fc.CameraNear), ptr(out))
+            self.o.orc_display_view(ptr(core), ptr(me), ptr(coat), self.w, y0, y1, view, th, fc.CameraNear, ptr(out))
         if len(picks):
             mask = self.mask(fc, picks)
             self.o.orc_outline(ptr(mask), self.w, self.h, y0, y1, ptr(out))

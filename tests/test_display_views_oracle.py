@@ -15,11 +15,7 @@ OUTLINE = (0.913098693, 0.332451582, 0.048171822)
 
 @pytest.fixture(scope="module")
 def o():
-    lib = orc.load()
-    lib.orc_gbuffer_pick.restype = C.c_uint32
-    lib.orc_pack_r11g11b10.restype = C.c_uint32
-    lib.orc_pack_r11g11b10.argtypes = [C.c_float] * 3
-    return lib
+    return orc.load()
 
 
 def srgb8(c):
@@ -108,7 +104,7 @@ def test_views_match_numpy(o, view):
     core, me, coat = gbuffer_records(o, W * H, view)
     for th in (0.0, 0.5, 1.0):
         out = np.zeros(W * H, dtype=np.uint32)
-        o.orc_display_view(ptr(core), ptr(me), ptr(coat), W, 0, H, view, C.c_float(th), C.c_float(0.2), ptr(out))
+        o.orc_display_view(ptr(core), ptr(me), ptr(coat), W, 0, H, view, th, 0.2, ptr(out))
         got = out.view(np.uint8).reshape(-1, 4).astype(np.int64)
         want = views_numpy(core, me, coat, view, th, np.float32(0.2))
         assert np.abs(got - want).max() <= 1, (view, th)

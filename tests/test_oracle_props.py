@@ -5,18 +5,11 @@ import os
 import numpy as np
 import pytest
 
-from tests.orc import ptr
-
-
-class Surf(C.Structure):
-    _fields_ = [("normal", C.c_float * 3), ("wo", C.c_float * 3), ("metallic", C.c_uint32), ("roughness", C.c_float),
-                ("baseColor", C.c_float * 3), ("eta_curr", C.c_float), ("eta_next", C.c_float), ("specTr", C.c_uint32),
-                ("trDepth", C.c_float), ("subsurface", C.c_float), ("coat_weight", C.c_float), ("coat_color", C.c_float * 3),
-                ("coat_roughness", C.c_float), ("coat_ior", C.c_float)]
+from tests.orc import SurfaceDesc, ptr
 
 
 def surf(roughness=0.5, metallic=0, base=(0.8, 0.8, 0.8), spec_tr=0, coat=0.0, coat_rough=0.1, wo=(0.3, 0.2, 0.93), subsurface=0.0):
-    s = Surf()
+    s = SurfaceDesc()
     s.normal[:] = (0, 0, 1)
     w = np.array(wo, dtype=np.float64); w /= np.linalg.norm(w)
     s.wo[:] = tuple(w)
@@ -34,7 +27,6 @@ def o(oracle):
     from tests import scene_util
     lut = scene_util.rho_lut()       # process-wide instance: the oracle keeps a bare pointer
     oracle.orc_set_rho_lut(ptr(lut))
-    oracle.orc_bsdf_sampler_pdf.restype = C.c_float
     return oracle
 
 
@@ -53,13 +45,13 @@ def test_octahedral_roundtrip_1e6(o):
 def test_storage_codecs(o):
     out = (C.c_float * 3)()
     for rgb in [(0, 0, 0), (1, 0.5, 0.25), (20, 15.5, 12.3), (65000, 1e-3, 3.3)]:
-        p = o.orc_pack_r11g11b10(C.c_float(rgb[0]), C.c_float(rgb[1]), C.c_float(rgb[2]))
+        p = o.orc_pack_r11g11b10(rgb[0], rgb[1], rgb[2])
         o.orc_unpack_r11g11b10(p, out)
         for a, b, tol in zip(rgb, out, (1 / 64, 1 / 64, 1 / 32)):
             assert b <= a + 1e-12 and (a == 0 or (a - b) / a <= tol + 1e-6)     # truncation, 6/6/5 mantissa bits
     out2 = (C.c_float * 2)()
     for xy in [(0, 0), (0.5, -0.5), (1, -1), (3, -3), (1e-3, -2e-5)]:
-        o.orc_unpack_snorm16x2(o.orc_pack_snorm16x2(C.c_float(xy[0]), C.c_float(xy[1])), out2)
+        o.orc_unpack_snorm16x2(o.orc_pack_snorm16x2(xy[0], xy[1]), out2)
         for a, b in zip(xy, out2):
             assert abs(np.clip(a, -1, 1) - b) <= 0.5 / 32767 + 1e-9
 
@@ -142,7 +134,7 @@ def test_plain_path_tracer_is_the_ground_truth_for_both_restir_integrators():
 
     def run(mode, nframes=36):
         R = rpt_util.OracleRenderer(scene_util.cornell(), w, h)
-        R.gi_params.update(stochastic_multi_bounce=0)
+        R.gi_params.stochastic_multi_bounce = 0
         seq = rpt_util.FrameSequence(w, h)
         means = []
         for fr in range(nframes):

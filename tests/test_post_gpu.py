@@ -80,7 +80,7 @@ def test_taa_three_frames(oracle, w, h):
             me[:, 0] = 0      # static frame: motion vectors zero
         signal = synth.synth_hdr(w, h, 200 + frame)
         ref = np.zeros((w * h, 2), dtype=np.uint32)
-        oracle.orc_taa(C.byref(fc), ptr(core), ptr(me), ptr(signal), ptr(prev), ptr(ref), C.c_float(0.1), valid)
+        oracle.orc_taa(C.byref(fc), ptr(core), ptr(me), ptr(signal), ptr(prev), ptr(ref), 0.1, valid)
         d_core, d_depth, d_me, d_sig = dev(core), dev(depth), dev(me), dev(signal)
         fi = _frame_inputs(fc, d_core, d_depth, d_me)
         check(lib.zr_taa_pass_render(p, C.byref(fi), dptr(d_sig), stream()))

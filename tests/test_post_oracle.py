@@ -118,7 +118,7 @@ def oracle_firefly(oracle, fc, core, comp):
 def oracle_taa(oracle, w, h, core, me, sig, prev, bw=0.1, valid=1):
     fc = synth.look_at_frame_constants(w, h, frame=2)
     out = np.zeros((w * h, 2), dtype=np.uint32)
-    oracle.orc_taa(C.byref(fc), ptr(core), ptr(me), ptr(sig), ptr(prev), ptr(out), C.c_float(bw), int(valid))
+    oracle.orc_taa(C.byref(fc), ptr(core), ptr(me), ptr(sig), ptr(prev), ptr(out), bw, int(valid))
     return out
 
 

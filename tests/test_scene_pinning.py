@@ -19,14 +19,6 @@ HASHED = ("oct32", "emissive")
 STRUCTS = (("MeshInstance", zs.MESH_INSTANCE), ("EmissiveTriangle", zs.EMISSIVE_TRI), ("Material", zs.MATERIAL))
 
 
-def load_ref_lib(so):
-    lib = C.CDLL(so)
-    lib.ref_oct32.restype = C.c_uint32
-    lib.ref_half.restype = C.c_uint16
-    lib.ref_rgb8.restype = C.c_uint32
-    return lib
-
-
 def oct_half_rgb8_inputs():
     rng = np.random.default_rng(0)
     n = rng.normal(size=(30000, 3))
@@ -93,20 +85,20 @@ def reference_scene_outputs(ref):
     ref.ref_scene_sizes(sz)
     out["sizes"] = np.array(list(sz), dtype=np.int32)
     n, x, c = oct_half_rgb8_inputs()
-    out["oct32"] = np.array([ref.ref_oct32(C.c_float(a), C.c_float(b), C.c_float(cc)) for a, b, cc in n], dtype=np.uint32)
-    out["half"] = np.array([ref.ref_half(C.c_float(v)) for v in x], dtype=np.uint16)
-    out["rgb8"] = np.array([ref.ref_rgb8(C.c_float(v[0]), C.c_float(v[1]), C.c_float(v[2])) for v in c], dtype=np.uint32)
+    out["oct32"] = np.array([ref.ref_oct32(a, b, cc) for a, b, cc in n], dtype=np.uint32)
+    out["half"] = np.array([ref.ref_half(v) for v in x], dtype=np.uint16)
+    out["rgb8"] = np.array([ref.ref_rgb8(v[0], v[1], v[2]) for v in c], dtype=np.uint32)
     mats = np.zeros(1500, dtype=zs.MATERIAL)
     for k, (p, ds, tw) in enumerate(material_inputs()):
-        ref.ref_material(p.ctypes.data_as(C.c_void_p), C.c_uint32(int(ds) | (int(tw) << 1)), mats[k:k + 1].ctypes.data_as(C.c_void_p))
+        ref.ref_material(p.ctypes.data_as(C.c_void_p), int(ds) | (int(tw) << 1), mats[k:k + 1].ctypes.data_as(C.c_void_p))
     out["materials"] = mats
     V0, V1, V2, uv, ids, strength = emissive_inputs()
     tris = np.zeros(len(ids), dtype=zs.EMISSIVE_TRI)
     for k in range(len(ids)):
         vv = np.concatenate([V0[k], V1[k], V2[k]]).astype(np.float32)
         uu = np.concatenate([uv[0][k], uv[1][k], uv[2][k]]).astype(np.float32)
-        ref.ref_emissive_triangle(vv.ctypes.data_as(C.c_void_p), uu.ctypes.data_as(C.c_void_p), C.c_uint32(0x9dc6ff), C.c_uint32(zs.INVALID_ID),
-                                  C.c_uint16(strength), C.c_uint32(int(ids[k])), 1, tris[k:k + 1].ctypes.data_as(C.c_void_p))
+        ref.ref_emissive_triangle(vv.ctypes.data_as(C.c_void_p), uu.ctypes.data_as(C.c_void_p), 0x9dc6ff, zs.INVALID_ID,
+                                  strength, int(ids[k]), 1, tris[k:k + 1].ctypes.data_as(C.c_void_p))
     # TriIDPatchedBit: set when the scene patches ID / world position (SceneCore.cpp:199-235); ours are stored patched
     tris["PackedA"] |= np.uint32(1 << 24)
     out["emissive"] = tris

@@ -21,10 +21,9 @@ def main():
     if reflib is None:
         raise SystemExit("oracle/_ref/libref_alias.so is missing: build it from the reference tree first")
     np.savez_compressed(test_alias_oracle.GOLDEN_REF, **test_alias_oracle.reference_alias_outputs(reflib))
-    scene_so = os.path.join(ROOT, "oracle", "_ref", "libref_scene.so")
-    if not os.path.exists(scene_so):
+    ref = orc.load_ref_scene()
+    if ref is None:
         raise SystemExit("oracle/_ref/libref_scene.so is missing: build it from the reference tree first")
-    ref = test_scene_pinning.load_ref_lib(scene_so)
     np.savez_compressed(test_scene_pinning.GOLDEN, **test_scene_pinning.reference_scene_outputs(ref))
     for p in (test_alias_oracle.GOLDEN_REF, test_scene_pinning.GOLDEN):
         print("wrote", os.path.relpath(p, ROOT), os.path.getsize(p), "bytes")

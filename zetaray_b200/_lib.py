@@ -38,40 +38,43 @@ class _NoLibrary:
 
 u32, u64, f32, vp, i32 = C.c_uint32, C.c_uint64, C.c_float, C.c_void_p, C.c_int32
 
-# Parameter and return types of the ZR_API prototypes. Besides these, every pointer parameter (T*, T**, T[N]) and every
+# Parameter and return types of the exported prototypes. Besides these, every pointer parameter (T*, T**, T[N]) and every
 # function-pointer typedef is a c_void_p, which takes byref(), pointer(), arrays, None, ints and CFUNCTYPE instances;
 # every enum typedef is a c_int.
-ARG_TYPES = {"uint32_t": u32, "uint64_t": u64, "size_t": C.c_size_t, "float": f32, "int": C.c_int}
-RET_TYPES = {"zr_status": i32, "void": None, "uint32_t": u32, "uint64_t": u64, "const char*": C.c_char_p}
+ARG_TYPES = {"uint16_t": C.c_uint16, "uint32_t": u32, "uint64_t": u64, "int64_t": C.c_int64, "size_t": C.c_size_t,
+             "float": f32, "int": C.c_int}
+RET_TYPES = {"zr_status": i32, "void": None, "int": C.c_int, "uint16_t": C.c_uint16, "uint32_t": u32, "uint64_t": u64,
+             "float": f32, "void*": vp, "const char*": C.c_char_p}
 
 
-def prototypes(text=None):
-    """{name: (restype, [argtypes])} for every ZR_API function of include/zr_abi.h (or of the header text `text`).
-    A declaration that does not parse or uses a type outside the maps above raises ZRError naming it."""
+def prototypes(text=None, macro="ZR_API", prefix="zr_"):
+    """{name: (restype, [argtypes])} for every `macro` function named `prefix`... in the header text `text` (by default
+    every ZR_API function of include/zr_abi.h). A declaration that does not parse or uses a type outside the maps above
+    raises ZRError naming it."""
     if text is None:
         with open(HEADER) as f:
             text = f.read()
     text = re.sub(r"/\*.*?\*/", " ", text, flags=re.S)
-    text = re.sub(r"^\s*#.*$", "", text, flags=re.M)          # the ZR_API definition itself
+    text = re.sub(r"^\s*#.*$", "", text, flags=re.M)          # the export macro's definition itself
     args = dict(ARG_TYPES)
     args.update((e, C.c_int) for e in re.findall(r"typedef\s+enum\b[^{;]*\{[^}]*\}\s*(\w+)\s*;", text))
     args.update((fn, vp) for fn in re.findall(r"typedef\s+[\w\s*]+\(\s*\*\s*(\w+)\s*\)", text))
     out = {}
-    for decl in re.findall(r"\bZR_API\b([^;]*);", text):
+    for decl in re.findall(r"\b%s\b([^;]*);" % macro, text):
         decl = " ".join(decl.split())
-        m = re.fullmatch(r"(.+?) ?\b(zr_\w+) ?\((.*)\)", decl)
+        m = re.fullmatch(r"(.+?) ?\b(%s\w+) ?\((.*)\)" % prefix, decl)
         if m is None:
-            raise ZRError("zr_abi.h: cannot parse the declaration %r" % decl)
+            raise ZRError("%s: cannot parse the declaration %r" % (macro, decl))
         ret, name, params = m.groups()
         ret = ret.replace(" *", "*")
         if ret not in RET_TYPES:
-            raise ZRError("zr_abi.h: %s returns %r, which has no ctypes type" % (decl, ret))
+            raise ZRError("%s: %s returns %r, which has no ctypes type" % (macro, decl, ret))
         argtypes = []
         for p in ([] if params == "void" else params.split(",")):
             p = p.strip()
             t = vp if "*" in p or "[" in p else args.get(p.rsplit(" ", 1)[0])
             if t is None:
-                raise ZRError("zr_abi.h: %s takes %r, which has no ctypes type" % (decl, p))
+                raise ZRError("%s: %s takes %r, which has no ctypes type" % (macro, decl, p))
             argtypes.append(t)
         out[name] = (RET_TYPES[ret], argtypes)
     return out
@@ -82,14 +85,15 @@ def declared_symbols():
     return sorted(prototypes())
 
 
-def _declare(dll):
-    for name, (restype, argtypes) in prototypes().items():
+def declare(dll, protos):
+    """Set every function of `protos` (from prototypes()) on the CDLL `dll`; returns `dll`."""
+    for name, (restype, argtypes) in protos.items():
         f = getattr(dll, name)
         f.restype, f.argtypes = restype, argtypes
     return dll
 
 
-lib = _NoLibrary() if os.environ.get("ZETARAY_B200_STRUCTS_ONLY") == "1" else _declare(_load())
+lib = _NoLibrary() if os.environ.get("ZETARAY_B200_STRUCTS_ONLY") == "1" else declare(_load(), prototypes())
 
 
 class FrameConstants(C.Structure):
