@@ -54,7 +54,8 @@ ZR_API const char* zr_last_error(void);
  * zr_renderer_set_display / get_display_output and zr_comm_allreduce_u32. 1.7 added zr_comm_create_transport (zr_comm_transport). 1.8
  * added zr_svgf_pass_set_rows / set_halo_exchange, and zr_renderer_set_shard runs the SVGF stage sharded instead of refusing it. 1.9
  * added zr_scene_update_materials and zr_scene_get_tables. 1.10 added pixel picking (zr_gbuffer_pass_pick / get_pick), the Display
- * pass's G-buffer debug views (zr_display_pass_set_view) and the outline of picked instances (zr_display_pass_set_picked). */
+ * pass's G-buffer debug views (zr_display_pass_set_view) and the outline of picked instances (zr_display_pass_set_picked). 1.11
+ * added the ReSTIR PT debug views (zr_indirect_pass_set_debug_view). */
 ZR_API uint32_t zr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -536,6 +537,23 @@ ZR_API zr_status zr_indirect_pass_set_halo_exchange(zr_indirect_pass* p, zr_halo
 ZR_API zr_status zr_indirect_pass_set_cost_map(zr_indirect_pass* p, void* d_cycles);
 ZR_API zr_status zr_indirect_pass_set_schedule_costs(zr_indirect_pass* p, const double* h_tile_cost, uint32_t tiles_x, uint32_t tiles_y);
 ZR_API void zr_indirect_pass_destroy(zr_indirect_pass* p);
+/* ReSTIR PT debug views (RPT_DEBUG_VIEW, IndirectLighting_Common.h:58-67, same order; IndirectLighting::DebugViewCallback,
+ * IndirectLighting.cpp:1233, 1543-1549). A view other than NONE replaces the indirect output (ZR_INDIRECT_FINAL) by
+ * RPT_Util::DebugColor (ReSTIR_PT/Util.hlsli:69-139) of the reconnection in the reservoir that produces it: the reconnection vertex's
+ * index k, its case, whether there is one, the BSDF lobe before or after x_k. The colour is written where the reference writes it --
+ * the path-trace output with temporal reuse off (ReSTIR_PT_PathTrace.hlsl:540-556), temporal reuse's output without spatial reuse
+ * (Reconnect_TtC.hlsl:386-388), else each spatial pass's output (Reconnect_StC.hlsl:348-351) -- and every other output write of those
+ * stages is black while a view is on (Util.hlsli:141-160): no reusable neighbour, no temporal history, a history without a
+ * reconnection. An empty reconnection is black, and so is case 3 in CONNECTION_LOBE_K. Accumulation, invalid and emissive pixels
+ * behave as without a view, and reservoirs, target, neighbour and thread-map planes are the same bytes with and without one. Debug
+ * frames launch one more kernel per write stage and hold 80 bytes per pixel more (freed when the view returns to NONE). Default
+ * NONE; the view survives resize and reset_temporal. A view > CONNECTION_LOBE_K or a NULL pass is ZR_ERR_INVALID_ARG. */
+typedef enum zr_rpt_debug_view
+{
+    ZR_RPT_DEBUG_VIEW_NONE = 0, ZR_RPT_DEBUG_VIEW_K, ZR_RPT_DEBUG_VIEW_CASE, ZR_RPT_DEBUG_VIEW_FOUND_CONNECTION,
+    ZR_RPT_DEBUG_VIEW_CONNECTION_LOBE_K_MIN_1, ZR_RPT_DEBUG_VIEW_CONNECTION_LOBE_K
+} zr_rpt_debug_view;
+ZR_API zr_status zr_indirect_pass_set_debug_view(zr_indirect_pass* p, uint32_t view);
 
 /* ---- IndirectLighting, INTEGRATOR::ReSTIR_GI (IndirectLighting.cpp:277-368; ReSTIR_GI shaders) ----
  * One kernel per frame: a path-traced initial candidate (second path vertex + outgoing radiance), temporal reuse with one

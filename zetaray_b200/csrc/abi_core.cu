@@ -93,7 +93,7 @@ extern "C"
     //        allocation failures return ZR_ERR_OUT_OF_MEMORY
     // 1.4: - the stage-limited ReSTIR PT render and its stage enum (nothing called them)
     // 1.3: - zr_indirect_pass_set_execution, zr_compositing_pass_render_unfused (measurement and test hooks; nothing else called them)
-    uint32_t zr_abi_version(void) { return (1u << 16) | 10u; }    // 1.10: + zr_gbuffer_pass_pick / get_pick, zr_display_pass_set_view / set_picked; 1.9: + zr_scene_update_materials, zr_scene_get_tables; 1.8: + zr_svgf_pass_set_rows / set_halo_exchange, sharded SVGF stage; 1.7: + zr_comm_create_transport; 1.6: + AutoExposure and Display passes, zr_renderer_set_display, zr_comm_allreduce_u32; 1.2: + SVGF pass, zr_comm, sharded renderer, zr_gi_pass_set_rows / set_halo_exchange; 1.1: + zr_bvh_build_host, zr_renderer_set_integrator / get_gi_pass / apply_scene_settings, zr_gi_pass_set_method
+    uint32_t zr_abi_version(void) { return (1u << 16) | 11u; }    // 1.11: + zr_indirect_pass_set_debug_view; 1.10: + zr_gbuffer_pass_pick / get_pick, zr_display_pass_set_view / set_picked; 1.9: + zr_scene_update_materials, zr_scene_get_tables; 1.8: + zr_svgf_pass_set_rows / set_halo_exchange, sharded SVGF stage; 1.7: + zr_comm_create_transport; 1.6: + AutoExposure and Display passes, zr_renderer_set_display, zr_comm_allreduce_u32; 1.2: + SVGF pass, zr_comm, sharded renderer, zr_gi_pass_set_rows / set_halo_exchange; 1.1: + zr_bvh_build_host, zr_renderer_set_integrator / get_gi_pass / apply_scene_settings, zr_gi_pass_set_method
     uint64_t zr_kernel_launch_count(void) { return zr::g_launches.load(); }
 
     zr_status zr_profile_enable(int on)

@@ -518,6 +518,107 @@ namespace
             writeOutput(dxs[i], dys[i], (int)(rank & 31), (int)(rank >> 5), result[i]);
         }
     }
+
+    // -------------------------------------------------------------------------------------------
+    // Debug views (RPT_DEBUG_VIEW, IndirectLighting_Common.h:58-67)
+    // -------------------------------------------------------------------------------------------
+    // RPT_Util::DebugColor (ReSTIR_PT/Util.hlsli:69-139) of the reconnection packed in a record's meta word, constants as the
+    // reference has them (GLOSSY_R is 0.4284 in one lobe view and 0.284 in the other). A record's k is 2..16 or EMPTY and every
+    // non-empty reconnection is one of the three cases, so the colour never falls through to the radiance.
+    ZR_D float3 DebugColor(uint32_t view, uint32_t meta)
+    {
+        Reservoir r;
+        r.UnpackMetadata(meta);
+        const Reconnection& rc = r.rc;
+        if (rc.Empty())
+            return f3(0);
+        if (view == ZR_RPT_DEBUG_VIEW_K)
+            return rc.k == 2 ? f3(0.1f, 0.25f, 0.88f) : rc.k == 3 ? f3(0.13f, 0.55f, 0.14f) : rc.k == 4 ? f3(0.69f, 0.45f, 0.1f) :
+                f3(0.88f, 0.08f, 0.1f);
+        if (view == ZR_RPT_DEBUG_VIEW_CASE)
+            return rc.IsCase1() ? f3(0.85f, 0.096f, 0.1f) : rc.IsCase2() ? f3(0.13f, 0.6f, 0.14f) : f3(0.1f, 0.27f, 0.888f);
+        if (view == ZR_RPT_DEBUG_VIEW_FOUND_CONNECTION)
+            return f3(0.234f, 0.12f, 0.2134f);
+        if (view == ZR_RPT_DEBUG_VIEW_CONNECTION_LOBE_K_MIN_1)
+        {
+            const BSDF::LOBE l = rc.lobe_k_min_1;
+            return l == BSDF::DIFFUSE_R ? f3(0.384f, 0.12f, 0.2134f) : l == BSDF::GLOSSY_R ? f3(0.12f, 0.4284f, 0.2134f) :
+                l == BSDF::GLOSSY_T ? f3(0.1134f, 0.12f, 0.634f) : l == BSDF::DIFFUSE_T ? f3(0.25f, 0.25f, 0.25f) : f3(0.55f, 0.55f, 0.0f);
+        }
+        if (rc.IsCase3())
+            return f3(0);
+        const BSDF::LOBE l = rc.lobe_k;
+        return l == BSDF::DIFFUSE_R ? f3(0.384f, 0.12f, 0.2134f) : l == BSDF::GLOSSY_R ? f3(0.12f, 0.284f, 0.2134f) :
+            l == BSDF::GLOSSY_T ? f3(0.1134f, 0.12f, 0.634f) : l == BSDF::DIFFUSE_T ? f3(0.25f, 0.25f, 0.0f) : f3(0.25f, 0.25f, 0.25f);
+    }
+
+    // The frame's writes of the indirect output, in the reference's order; each is followed by k_rpt_debug_view in a debug frame.
+    enum DebugStage : uint32_t { DV_PATHTRACE, DV_TEMPORAL, DV_SPATIAL };
+
+    // Overwrites what one stage (k_pathtrace, k_temporal_merge or one k_spatial_merge) just wrote to FINAL with the debug view, for
+    // the pixels that stage wrote. Where the reference colours the output (ReSTIR_PT_PathTrace.hlsl:548, Reconnect_TtC.hlsl:386,
+    // Reconnect_StC.hlsl:349) the colour is DebugColor of the reservoir the stage left in resOut; every other write of the stage is
+    // WriteOutputColor with the filter on (Util.hlsli:141-160), so black. The branch is recovered from planes the stage leaves:
+    //   DV_TEMPORAL  black unless the temporal flag is set and the previous frame's reservoir (resGate) at the reprojected pixel holds
+    //                a reconnection
+    //   DV_SPATIAL   black unless the pixel has a neighbour and the neighbour's input reservoir (resGate) holds a reconnection; the
+    //                pixels are the ones k_spatial_merge visits, thread position (x, y) -> pixel through the StC thread map
+    // prevFinal is FINAL as it was before the stage; it is read only where the stage accumulates. The alpha channel is left as the
+    // stage wrote it. One thread per pixel of rows [y0, ...): for DV_SPATIAL y0 is the first row of the strip's first 32x32 tile.
+    __global__ void __launch_bounds__(256) k_rpt_debug_view(FrameView f, RptParams prm, uint32_t view, uint32_t stage, uint32_t y0,
+        const zr_rpt_reservoir* __restrict__ resOut, const zr_rpt_reservoir* __restrict__ resGate, const uint8_t* __restrict__ tflags,
+        const uint16_t* __restrict__ neighbor, const uint16_t* __restrict__ threadMap, const float4* __restrict__ prevFinal,
+        float4* __restrict__ finalImg)
+    {
+        const zr_frame_constants& fc = f.fc;
+        int x = (int)(blockIdx.x * 32 + (threadIdx.x & 31));
+        int y = (int)(y0 + blockIdx.y * 8 + (threadIdx.x >> 5));
+        if (x >= (int)f.W || y >= (int)f.H) return;
+        if (stage == DV_SPATIAL && prm.sortSpatial)
+        {
+            const uint32_t enc = __ldg(&threadMap[(size_t)y * f.W + x]);
+            if (enc & (1u << 15)) return;
+            const int lx = (x & 31) + (int)(enc & 0x3f) - 31, ly = (y & 31) + (int)((enc >> 7) & 0x3f) - 31;
+            if ((uint32_t)lx >= 32u || (uint32_t)ly >= 32u) return;
+            x = (x & ~31) + lx; y = (y & ~31) + ly;
+            if (x >= (int)f.W || y >= (int)f.H) return;
+        }
+        if (y < (int)prm.rowBegin || y >= (int)prm.rowEnd) return;
+        const size_t idx = (size_t)y * f.W + x;
+        const GFlags flags = FlagsAt(f.core, f.W, x, y);
+        if (flags.invalid || flags.emissive) return;
+
+        bool colour = true;
+        if (stage == DV_TEMPORAL)
+        {
+            int ppx = 0, ppy = 0;
+            colour = (__ldg(&tflags[idx]) & TF_OK) != 0;
+            if (colour)
+            {
+                PrevPixel(f, x, y, ppx, ppy);
+                colour = (__ldg(&resGate[(size_t)ppy * f.W + ppx].meta) & 0xf) != Reconnection::EMPTY;
+            }
+        }
+        else if (stage == DV_SPATIAL)
+        {
+            int nx = 0, ny = 0;
+            colour = NeighborOf(f, neighbor, x, y, nx, ny) && (__ldg(&resGate[(size_t)ny * f.W + nx].meta) & 0xf) != Reconnection::EMPTY;
+        }
+        const float3 c = colour ? DebugColor(view, __ldg(&resOut[idx].meta)) : f3(0);
+        // the path-trace write accumulates whenever the camera is static, WriteOutputColor from the second static frame on
+        const bool accumulate = fc.Accumulate && fc.CameraStatic && (stage == DV_PATHTRACE || fc.NumFramesCameraStatic > 1);
+        float4 o = finalImg[idx];
+        if (accumulate)
+        {
+            const float4 prev = prevFinal[idx];
+            o.x = prev.x + c.x; o.y = prev.y + c.y; o.z = prev.z + c.z;
+        }
+        else
+        {
+            o.x = c.x; o.y = c.y; o.z = c.z;
+        }
+        finalImg[idx] = o;
+    }
 }
 } // namespace zr
 
@@ -539,6 +640,17 @@ struct zr_indirect_pass
         zr::SpatialQueued queued;
     } sz;
     zr::ShiftStreams shiftStreams;
+    // Debug view (zr_rpt_debug_view) and what its frames need besides the pass's planes, allocated by the first frame with a view at
+    // a size: the reservoirs k_pathtrace writes when temporal reuse is off (it keeps none then), and FINAL before the stage that
+    // writes it, where that stage accumulates.
+    uint32_t debugView = ZR_RPT_DEBUG_VIEW_NONE;
+    struct DebugPlanes
+    {
+        zr::Planes planes{ "zr_indirect_pass" };
+        size_t n = 0;
+        zr_rpt_reservoir* d_res = nullptr;
+        float4* d_prevFinal = nullptr;
+    } dbg;
     int currTemporalIdx = 0;
     bool isTemporalReservoirValid = false;
     bool resetTemporalTextures = true;
@@ -592,6 +704,18 @@ struct zr_indirect_pass
         return ZR_OK;
     }
 
+    zr_status FitDebugPlanes()
+    {
+        const size_t n = (size_t)width * height;
+        if (dbg.n == n) return ZR_OK;
+        DebugPlanes next;
+        ZR_TRY(next.planes.Alloc(next.d_res, n, false));
+        ZR_TRY(next.planes.Alloc(next.d_prevFinal, n, false));
+        next.n = n;
+        dbg = std::move(next);
+        return ZR_OK;
+    }
+
     zr_status LoadPattern()
     {
         if (patternLoaded) return ZR_OK;
@@ -633,14 +757,66 @@ struct zr_indirect_pass
         int cur = currTemporalIdx;
         const uint32_t dispX = (width + 15) / 16, dispY = (height + 7) / 8;
         const bool plain = (in->scene->materialFeatures & BSDF::MF_ALL) == 0;
+
+        // Debug frames: each stage that writes FINAL is followed by k_rpt_debug_view over the pixels it wrote. Nothing else changes:
+        // a frame without a view launches exactly the kernels above and below.
+        const bool view = debugView != ZR_RPT_DEBUG_VIEW_NONE;
+        if (view)
+        {
+            st = FitDebugPlanes();
+            if (st != ZR_OK) return st;
+        }
+        const zr_frame_constants& fc = f.fc;
+        const bool accumPathTrace = fc.Accumulate && fc.CameraStatic, accumReuse = accumPathTrace && fc.NumFramesCameraStatic > 1;
+        auto snapshot = [&](bool accumulate) -> zr_status
+        {
+            if (accumulate)
+            {
+                const size_t first = (size_t)prm.rowBegin * width;
+                ZR_CUDA(cudaMemcpyAsync(dbg.d_prevFinal + first, sz.d_final + first, (size_t)rows * width * sizeof(float4),
+                    cudaMemcpyDeviceToDevice, stream));
+            }
+            return ZR_OK;
+        };
+        auto debugPass = [&](DebugStage stage, const zr_rpt_reservoir* resOut, const zr_rpt_reservoir* resGate) -> zr_status
+        {
+            const uint32_t y0 = stage == DV_SPATIAL ? prm.rowBegin / 32 * 32 : prm.rowBegin;
+            const uint32_t y1 = stage == DV_SPATIAL ? std::min(height, (prm.rowEnd + 31) / 32 * 32) : prm.rowEnd;
+            ZR_PROF("k_rpt_debug_view", stream);
+            k_rpt_debug_view<<<dim3((width + 31) / 32, (y1 - y0 + 7) / 8), 256, 0, stream>>>(f, prm, debugView, stage, y0, resOut, resGate,
+                sz.queued.d_flags, sz.d_neighbor, sz.d_threadMap, dbg.d_prevFinal, sz.d_final);
+            ZR_LAUNCH_CHECK();
+            return ZR_OK;
+        };
+
+        // With temporal reuse off k_pathtrace writes no reservoir after the first frame; a debug frame has it write them to a plane of
+        // its own, so the pass's reservoirs stay as they would be without the view.
+        zr_rpt_reservoir* ptRes = sz.d_res[cur];
+        RptParams ptPrm = prm;
+        if (view && !doTemporal)
+        {
+            if (!prm.resetTemporal)
+            {
+                ptRes = dbg.d_res;
+                ptPrm.resetTemporal = 1;
+            }
+            ZR_TRY(snapshot(accumPathTrace));
+        }
         ZR_PROF("k_pathtrace", stream);
-        (plain ? k_pathtrace<BSDF::MF_NONE> : k_pathtrace<BSDF::MF_ALL>)<<<strip.sched[0].count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY,
+        (plain ? k_pathtrace<BSDF::MF_NONE> : k_pathtrace<BSDF::MF_ALL>)<<<strip.sched[0].count, ZR_PT_THREADS, PT_SMEM_BYTES, stream>>>(in->scene->dev, f, ptPrm, ptRes, sz.d_target, sz.d_final, dispX, dispY,
             strip.sched[0].d_order);
         ZR_LAUNCH_CHECK();
+        if (view && !doTemporal)
+            ZR_TRY(debugPass(DV_PATHTRACE, ptRes, nullptr));
         if (doTemporal)
         {
+            const bool temporalWrites = view && !doSpatial;
+            if (temporalWrites)
+                ZR_TRY(snapshot(accumReuse));
             st = sz.queued.RunTemporal(shiftStreams, in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, plain, stream);
             if (st != ZR_OK) return st;
+            if (temporalWrites)
+                ZR_TRY(debugPass(DV_TEMPORAL, sz.d_res[cur], sz.d_res[1 - cur]));
         }
         // reservoirs written so far are read by neighbours (spatial pass) and by the next frame's temporal pass
         strip.Exchange(sz.d_res[cur], width, height, 64u, stream);
@@ -662,8 +838,12 @@ struct zr_indirect_pass
                     k_sort<<<dim3(sx, ty1 - ty0), 256, 0, stream>>>(f, 3, 1u, rin, nullptr, sz.d_neighbor, sz.d_threadMap, sx, sy, ty0);
                     ZR_LAUNCH_CHECK();
                 }
+                if (view)
+                    ZR_TRY(snapshot(accumReuse));
                 st = sz.queued.Run(shiftStreams, in->scene->dev, f, prm, rin, rout, sz.d_target, sz.d_final, sz.d_neighbor, sz.d_threadMap, plain, stream);
                 if (st != ZR_OK) return st;
+                if (view)
+                    ZR_TRY(debugPass(DV_SPATIAL, rout, rin));
                 strip.Exchange(rout, width, height, 64u, stream);
             }
         }
@@ -690,6 +870,19 @@ extern "C"
             return ZR_ERR_INVALID_ARG;
         }
         p->params = *params;
+        return ZR_OK;
+    }
+    zr_status zr_indirect_pass_set_debug_view(zr_indirect_pass* p, uint32_t view)
+    {
+        if (!p) return ZR_ERR_INVALID_ARG;
+        if (view > ZR_RPT_DEBUG_VIEW_CONNECTION_LOBE_K)
+        {
+            zr::set_error("zr_indirect_pass_set_debug_view: view %u out of range (0..%u)", view, (uint32_t)ZR_RPT_DEBUG_VIEW_CONNECTION_LOBE_K);
+            return ZR_ERR_INVALID_ARG;
+        }
+        p->debugView = view;
+        if (view == ZR_RPT_DEBUG_VIEW_NONE)
+            p->dbg = zr_indirect_pass::DebugPlanes();       // frees them
         return ZR_OK;
     }
     zr_status zr_indirect_pass_render(zr_indirect_pass* p, const zr_frame_inputs* in, void* stream)

@@ -16,7 +16,6 @@ namespace zr
 namespace
 {
     using namespace RPT;
-    enum : uint8_t { TF_OK = 1, TF_REPLAY_OK = 2 };
 
     __global__ void __launch_bounds__(256) k_temporal_classify(SceneDev sc, FrameView f, RptParams prm, const zr_rpt_reservoir* __restrict__ resCurr,
         const zr_rpt_reservoir* __restrict__ resPrev, uint8_t* __restrict__ tflags, uint32_t* __restrict__ queue, uint32_t* __restrict__ counters,

@@ -44,6 +44,9 @@ struct ShiftStreams
 // SetupShifts<true>: the temporal pass's shift kernels are instantiated in rpt_temporal.cu
 zr_status SetupTemporalShifts();
 
+// bits of SpatialQueued::d_flags
+enum : uint8_t { TF_OK = 1, TF_REPLAY_OK = 2 };
+
 // The queues, shift results and tensor maps of one frame size. Temporal reuse runs through the same queues, counters and shift-result
 // plane (the two passes never overlap in a frame).
 struct SpatialQueued

@@ -274,6 +274,14 @@ class IndirectLighting(_Pass):
     prefix = "zr_indirect_pass"
     Params = _lib.IndirectParams
     output_ids = True
+    # zr_rpt_debug_view (RPT_DEBUG_VIEW)
+    (DEBUG_VIEW_NONE, DEBUG_VIEW_K, DEBUG_VIEW_CASE, DEBUG_VIEW_FOUND_CONNECTION, DEBUG_VIEW_CONNECTION_LOBE_K_MIN_1,
+     DEBUG_VIEW_CONNECTION_LOBE_K) = range(6)
+
+    def SetDebugView(self, view):
+        """DebugViewCallback: the indirect output shows each pixel's reconnection (its k, case, whether there is one, or the
+        lobe before or after it) instead of radiance; DEBUG_VIEW_NONE returns to radiance."""
+        self._call("set_debug_view", int(view))
 
 
 class IndirectLightingGI(_Pass):
