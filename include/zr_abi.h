@@ -55,7 +55,9 @@ ZR_API const char* zr_last_error(void);
  * added zr_svgf_pass_set_rows / set_halo_exchange, and zr_renderer_set_shard runs the SVGF stage sharded instead of refusing it. 1.9
  * added zr_scene_update_materials and zr_scene_get_tables. 1.10 added pixel picking (zr_gbuffer_pass_pick / get_pick), the Display
  * pass's G-buffer debug views (zr_display_pass_set_view) and the outline of picked instances (zr_display_pass_set_picked). 1.11
- * added the ReSTIR PT debug views (zr_indirect_pass_set_debug_view). */
+ * added the ReSTIR PT debug views (zr_indirect_pass_set_debug_view). The sky (zr_sky_pass_*, zr_direct_pass_set_sky,
+ * zr_compositing_pass_set_sky, zr_renderer_set_sky) was added without a minor of its own: the version still reads 1.11, so
+ * detect those entry points by symbol. */
 ZR_API uint32_t zr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -445,7 +447,7 @@ ZR_API void zr_gbuffer_free(zr_gbuffer* g);
 typedef enum zr_resource_id
 {
     ZR_RES_GBUFFER_CURR = 1, ZR_RES_GBUFFER_PREV, ZR_RES_SCENE_BVH, ZR_RES_ALIAS_TABLE,
-    ZR_RES_DI_FINAL, ZR_RES_INDIRECT_FINAL, ZR_RES_COMPOSITED, ZR_RES_TAA_OUT
+    ZR_RES_DI_FINAL, ZR_RES_INDIRECT_FINAL, ZR_RES_COMPOSITED, ZR_RES_TAA_OUT, ZR_RES_SKY_VIEW_LUT
 } zr_resource_id;
 typedef struct zr_resource_use { uint32_t id; uint32_t write; } zr_resource_use;
 
@@ -500,6 +502,12 @@ ZR_API zr_status zr_direct_pass_set_cost_map(zr_direct_pass* p, void* d_cycles);
 ZR_API zr_status zr_direct_pass_set_schedule_costs(zr_direct_pass* p, const double* h_tile_cost, uint32_t tiles_x, uint32_t tiles_y);
 ZR_API zr_status zr_direct_pass_get_output(zr_direct_pass* p, zr_direct_output id, zr_image2d* out);
 ZR_API zr_status zr_direct_pass_describe_io(zr_direct_pass* p, zr_resource_use* uses, int* n);
+/* The sky in accumulating frames (ReSTIR_DI_Temporal.hlsl:274-285): with a LUT set (zr_sky_pass_get_output), each render with
+ * Accumulate && CameraStatic copies FINAL's rows before it runs and afterwards sets every pixel without geometry to that copy
+ * (kept only when NumFramesCameraStatic > 1) plus Le_SkyWithSunDisk, so Compositing's division by the frame count averages the
+ * sky like any other pixel. Other frames leave those pixels at 0, as without a LUT. The copy is allocated only while a LUT is set.
+ * lut == NULL turns it off; an image that is not a non-empty unpadded 4-byte-texel plane is refused. The pass does not own the LUT. */
+ZR_API zr_status zr_direct_pass_set_sky(zr_direct_pass* p, const zr_image2d* lut);
 ZR_API void zr_direct_pass_destroy(zr_direct_pass* p);
 
 /* ---- IndirectLighting (ReSTIR PT, IndirectLighting/IndirectLighting.h:72-108) ---- */
@@ -598,6 +606,20 @@ ZR_API zr_status zr_gi_pass_render(zr_gi_pass* p, const zr_frame_inputs* in, voi
 ZR_API zr_status zr_gi_pass_get_output(zr_gi_pass* p, zr_gi_output id, zr_image2d* out);
 ZR_API void zr_gi_pass_destroy(zr_gi_pass* p);
 
+/* ---- Sky (Sky/Sky.h, Sky.cpp:120-147): the sky-view LUT (Sky/SkyViewLUT.hlsl) ----
+ * create(lut_w, lut_h): a lut_w x lut_h LUT (the renderer's is 256 x 128, DefaultRendererImpl.h:165-166). render reads only
+ * in->frame: the sun (SunDir, SunIlluminance) and the atmosphere (PlanetRadius, AtmosphereAltitude, Rayleigh / Mie / ozone
+ * coefficients, g), and refuses non-finite values or a PlanetRadius or AtmosphereAltitude <= 0. Each texel is the sun's light
+ * scattered once towards a viewer 0.2 km above the ground (Volumetric.hlsli EstimateLs, 32 steps; 8 towards the sun), at
+ * longitude 2 pi x / lut_w and latitude pi/2 +- 2 pi (y / lut_h - 1/2)^2. get_output (GetOutput(SKY_VIEW_LUT)): R11G11B10F texels
+ * as uint32, pitch = 4 * lut_w. No sizes beyond the create; inscattering is not part of this pass. */
+typedef struct zr_sky_pass zr_sky_pass;
+ZR_API zr_status zr_sky_pass_create(uint32_t lut_w, uint32_t lut_h, zr_sky_pass** out);
+ZR_API zr_status zr_sky_pass_render(zr_sky_pass* p, const zr_frame_inputs* in, void* stream);
+ZR_API zr_status zr_sky_pass_get_output(zr_sky_pass* p, zr_image2d* out);
+ZR_API zr_status zr_sky_pass_describe_io(zr_sky_pass* p, zr_resource_use* uses, int* n);
+ZR_API void zr_sky_pass_destroy(zr_sky_pass* p);
+
 /* ---- Compositing + FireflyFilter (Compositing/Compositing.cpp:83-145) ---- */
 typedef struct zr_compositing_pass zr_compositing_pass;
 typedef struct zr_compositing_params { uint32_t emissive_di; uint32_t indirect; uint32_t firefly_filter; } zr_compositing_params;
@@ -609,6 +631,11 @@ ZR_API zr_status zr_compositing_pass_render(zr_compositing_pass* p, const zr_fra
     const void* d_direct, const void* d_indirect, void* stream);
 ZR_API zr_status zr_compositing_pass_set_rows(zr_compositing_pass* p, uint32_t y0, uint32_t y1);
 ZR_API zr_status zr_compositing_pass_get_output(zr_compositing_pass* p, zr_image2d* out);
+/* The sky behind geometry in frames that do not accumulate (Compositing.hlsl:43-47): with a LUT set, pixels without geometry show
+ * Light::Le_SkyWithSunDisk (LightSource.hlsli:178-199) when emissive_di is on and 0 when it is off; NULL returns to 0 everywhere.
+ * Accumulating frames take the sky from DirectLighting's output (zr_direct_pass_set_sky). Refuses what zr_direct_pass_set_sky
+ * refuses; the pass does not own the LUT. */
+ZR_API zr_status zr_compositing_pass_set_sky(zr_compositing_pass* p, const zr_image2d* lut);
 ZR_API void zr_compositing_pass_destroy(zr_compositing_pass* p);
 
 /* ------------------------------------------------------------------------------------------
@@ -807,6 +834,12 @@ ZR_API zr_status zr_renderer_get_output(zr_renderer* r, zr_image2d* out);      /
  * gather the display image on rank 0 along with the TAA image. out_ae / out_display may be NULL. */
 ZR_API zr_status zr_renderer_set_display(zr_renderer* r, int enable, zr_auto_exposure_pass** out_ae, zr_display_pass** out_display);
 ZR_API zr_status zr_renderer_get_display_output(zr_renderer* r, zr_image2d* out);      /* RGBA8; ZR_ERR_NOT_INITIALIZED when disabled */
+/* The sky (Sky::Render, PathTracer.cpp:165-185, 343-362): enable != 0 creates a 256 x 128 sky pass whose LUT every frame recomputes
+ * on DirectLighting's stream before DirectLighting, and hands that LUT to zr_direct_pass_set_sky and zr_compositing_pass_set_sky, so
+ * pixels without geometry show the sky and the sun disk. Strip-sharded, every rank computes the whole LUT. 0 detaches the LUT and
+ * frees the pass and the DirectLighting copy it needed; frames are then those of a renderer that never enabled it. *out_pass (may
+ * be NULL) is the pass, or NULL when the sky is off. Off by default. */
+ZR_API zr_status zr_renderer_set_sky(zr_renderer* r, int enable, zr_sky_pass** out_pass);
 ZR_API zr_status zr_renderer_get_passes(zr_renderer* r, zr_gbuffer_pass** gbuffer, zr_direct_pass** direct,
     zr_indirect_pass** indirect, zr_compositing_pass** compositing, zr_taa_pass** taa);
 ZR_API zr_status zr_renderer_get_gbuffer(zr_renderer* r, int previous, zr_gbuffer* out);

@@ -10,7 +10,7 @@
  * and sm_90a (nvcc, -fmad=false). Nothing here restates the reference's algorithms; it plays
  * the role "the same libm on both sides" plays in a CPU-vs-CPU comparison.
  *
- * Accuracy: sin/cos <= 2 ulp on [-2pi, 4pi]; exp/log <= 2 ulp on normal range.
+ * Accuracy: sin/cos <= 2 ulp on [-2pi, 4pi]; exp/log <= 2 ulp on normal range; atan2 <= 2 ulp.
  */
 #ifndef ZR_FPMATH_H
 #define ZR_FPMATH_H
@@ -124,6 +124,50 @@ ZR_HD float zr_logf(float x)
     y = fmaf(fe, -2.12194440e-4f, y);
     y = fmaf(-0.5f, z, y);
     return fmaf(fe, 0.693359375f, m + y);
+}
+
+/* ---- atan2: octant reduction to t = min/max in [0, 1], t > tan(pi/8) folded to (num-den)/(num+den), degree-5 polynomial in t^2
+   (least-squares fit on [0, tan(pi/8)]); pi/4, pi/2 and pi are added as hi + lo pairs so the final subtraction does not lose the last bits.
+   IEEE special cases: signed zeros and the axes give +-0, +-pi/2 and +-pi; a NaN gives NaN. ---- */
+ZR_HD float zr_atan2f(float y, float x)
+{
+    if (x != x || y != y) return x + y;
+    const float ax = fabsf(x), ay = fabsf(y);
+    const float PIO4_HI = 7.8539818525e-01f, PIO4_LO = -2.1855694e-08f;
+    const float PIO2_HI = 1.5707963705e+00f, PIO2_LO = -4.3711388e-08f;
+    const float PI_HI = 3.1415927410e+00f, PI_LO = -8.7422777e-08f;
+    float r;
+    if (ax == 0.0f && ay == 0.0f)
+        r = 0.0f;
+    else if (ax == ay)      /* including both infinite */
+        r = PIO4_HI;
+    else
+    {
+        const int swap = ay > ax;
+        const float num = swap ? ax : ay, den = swap ? ay : ax;
+        float a = num, b = den;
+        float off_hi = 0.0f, off_lo = 0.0f;
+        if (num > 0.41421356237f * den)
+        {
+            /* scaling both by 1/4 is exact and keeps num + den finite */
+            const float k = den > 1e38f ? 0.25f : 1.0f;
+            a = num * k - den * k;
+            b = num * k + den * k;
+            off_hi = PIO4_HI; off_lo = PIO4_LO;
+        }
+        const float t = a / b;                      /* 0 when num is finite and den infinite */
+        const float t_lo = b > 3.40282347e38f ? 0.0f : fmaf(-t, b, a) / b;      /* the division's rounding error (none when b is infinite) */
+        const float z = t * t;
+        float p = fmaf(5.055331811e-2f, z, -8.627819270e-2f);
+        p = fmaf(p, z, 1.107185036e-1f);
+        p = fmaf(p, z, -1.428418159e-1f);
+        p = fmaf(p, z, 1.999997795e-1f);
+        p = fmaf(p, z, -3.333333433e-1f);
+        r = off_hi + ((fmaf(p * z, t, t_lo) + t) + off_lo);
+        if (swap) r = PIO2_HI - (r - PIO2_LO);
+    }
+    if (zr_f2u(x) >> 31) r = PI_HI - (r - PI_LO);
+    return (zr_f2u(y) >> 31) ? -r : r;
 }
 
 ZR_HD float zr_log2f(float x) { return zr_logf(x) * 1.44269504088896341f; }

@@ -31,7 +31,34 @@ def look_at_frame_constants(w, h, frame=1, jitter=(0.0, 0.0), prev_jitter=(0.0, 
     fc.NumFramesCameraStatic = 0
     fc.CameraStatic = 0
     fc.Accumulate = 0
+    set_default_atmosphere(fc)
     return fc
+
+
+def set_default_atmosphere(fc):
+    """The reference's sun and atmosphere (DefaultRenderer.cpp:274-307 with DefaultRendererImpl.h:29-36): distances in km, Hillaire's
+    (2020) Rayleigh / Mie / ozone coefficients in 1/km, Rayleigh and ozone stored as a unit colour times a scale. Only the sky
+    (zr_renderer_set_sky) reads these fields."""
+    f = np.float32
+    sun = np.array([0.6565358, -0.0560669, 0.752208233], dtype=np.float64)
+    sun = (sun / np.linalg.norm(sun)).astype(np.float32)
+    fc.SunDir[0], fc.SunDir[1], fc.SunDir[2] = (float(v) for v in sun)
+    fc.SunIlluminance = 20.0
+    cos_r = f(np.cos(np.float64(np.radians(f(0.5) * f(0.526)))))
+    fc.SunCosAngularRadius = float(cos_r)
+    fc.SunSinAngularRadius = float(np.sqrt(f(1.0) - cos_r * cos_r))
+    fc.AtmosphereAltitude = 100.0
+    fc.PlanetRadius = 6360.0
+    fc.g = 0.8
+    for name, v in (("RayleighSigmaS", (5.802e-3, 13.558e-3, 33.1e-3)), ("OzoneSigmaA", (0.65e-3, 1.881e-3, 0.085e-3))):
+        v = np.array(v, dtype=np.float32)
+        scale = f(np.sqrt(np.float64(v @ v)))
+        color = v * (f(1.0) / scale)
+        arr = getattr(fc, name + "Color")
+        arr[0], arr[1], arr[2] = (float(c) for c in color)
+        setattr(fc, name + "Scale", float(scale))
+    fc.MieSigmaA = 4.4e-3
+    fc.MieSigmaS = 3.996e-3
 
 
 

@@ -11,6 +11,7 @@
 // place (the reference's in-place UAV update races with its own neighbour reads).
 #include "zr_common.cuh"
 #include "zr_planes.h"
+#include "zr_sky.cuh"
 #include "zr_schedule.h"
 
 namespace zr
@@ -27,12 +28,26 @@ namespace
         uint32_t rowBegin, rowEnd;      // rows this device owns (strip-sharded frames); the whole image by default
     };
 
+    // The sky behind geometry (zr_compositing_pass_set_sky); only the SKY instantiations read it
+    struct SkyArgs
+    {
+        Sky::LutView lut;
+        uint32_t emissiveDI;
+        zr_frame_constants fc;
+    };
+
+    // SKY: invalid pixels of non-accumulating frames show Le_SkyWithSunDisk when emissive direct lighting is on (Compositing.hlsl:43-47)
+    template<bool SKY>
     ZR_D float3 composite_px(const uint4* __restrict__ core, const float4* __restrict__ direct,
-        const float4* __restrict__ indirect, size_t i, const PostParams& p)
+        const float4* __restrict__ indirect, size_t i, const PostParams& p, const SkyArgs& sky, uint32_t x, uint32_t y)
     {
         const uint32_t flags = __ldg(&core[i].w) & 0xffu;
         if ((flags & ZR_GBUFFER_FLAG_INVALID) && !p.accumulate)
+        {
+            if constexpr (SKY)
+                return sky.emissiveDI ? Sky::Le_SkyWithSunDisk(sky.fc, sky.lut, x, y) : f3(0);
             return f3(0);
+        }
         float3 color = f3(0);
         if (direct)
         {
@@ -47,14 +62,15 @@ namespace
         return color / (float)p.numFramesAccumulated;
     }
 
+    template<bool SKY>
     __global__ void __launch_bounds__(256) k_compositing(const uint4* __restrict__ core,
-        const float4* __restrict__ direct, const float4* __restrict__ indirect, float4* __restrict__ out, PostParams p)
+        const float4* __restrict__ direct, const float4* __restrict__ indirect, float4* __restrict__ out, PostParams p, SkyArgs sky)
     {
         const uint32_t x = blockIdx.x * 32 + (threadIdx.x & 31);
         const uint32_t y = p.rowBegin + blockIdx.y * 8 + (threadIdx.x >> 5);
         if (x >= p.W || y >= p.rowEnd) return;
         const size_t i = (size_t)y * p.W + x;
-        float3 c = composite_px(core, direct, indirect, i, p);
+        float3 c = composite_px<SKY>(core, direct, indirect, i, p, sky, x, y);
         out[i] = f4(c.x, c.y, c.z, 0.0f);
     }
 
@@ -65,8 +81,9 @@ namespace
     // reference's tap order, so the result is bit-identical to the oracle. Rows are read as contiguous 34-pixel segments
     // (coalesced 128-bit loads).
     constexpr int FF_TW = 32, FF_TH = 16, FF_SW = FF_TW + 2, FF_SH = FF_TH + 2;
+    template<bool SKY>
     __global__ void __launch_bounds__(FF_TW * FF_TH) k_firefly_tiled(const uint4* __restrict__ core, const float* __restrict__ depth,
-        const float4* __restrict__ direct, const float4* __restrict__ indirect, float4* __restrict__ out, PostParams p)
+        const float4* __restrict__ direct, const float4* __restrict__ indirect, float4* __restrict__ out, PostParams p, SkyArgs sky)
     {
         __shared__ float4 tile[FF_SH][FF_SW];           // xyz = (composited) colour, w = its luminance
         __shared__ uint8_t geom[FF_SH][FF_SW];          // 1 = inside the image and depth != FLT_MAX
@@ -82,7 +99,7 @@ namespace
             if ((uint32_t)gx < (uint32_t)W && (uint32_t)gy < (uint32_t)H)
             {
                 const size_t i = (size_t)gy * W + gx;
-                const float3 c = composite_px(core, direct, indirect, i, p);
+                const float3 c = composite_px<SKY>(core, direct, indirect, i, p, sky, (uint32_t)gx, (uint32_t)gy);
                 v = f4(c.x, c.y, c.z, Math::Luminance(c));
                 g = __ldg(&depth[i]) != FLT_MAX_ ? 1 : 0;
             }
@@ -332,6 +349,7 @@ struct zr_compositing_pass
     } sz;
     zr_compositing_params params{ 1, 1, 1 };
     zr::StripRows strip{ "zr_compositing_pass" };
+    zr::Sky::LutView sky{ nullptr, 0, 0 };     // zr_compositing_pass_set_sky; not owned
 
     zr_status Setup() { return ZR_OK; }
     zr_status OnWindowResized(uint32_t w, uint32_t h)
@@ -357,19 +375,25 @@ struct zr_compositing_pass
         const float4* direct = params.emissive_di ? (const float4*)d_direct : nullptr;
         const float4* indirect = params.indirect ? (const float4*)d_indirect : nullptr;
         p.rowBegin = strip.rowBegin; p.rowEnd = strip.ClampedRowEnd(height);
+        const bool withSky = sky.texels != nullptr;
+        SkyArgs skyArgs;
+        skyArgs.lut = sky;
+        skyArgs.emissiveDI = params.emissive_di;
+        skyArgs.fc = in->frame;
         if (params.firefly_filter)
         {
             const dim3 tgrid((width + FF_TW - 1) / FF_TW, (p.rowEnd - p.rowBegin + FF_TH - 1) / FF_TH);
             ZR_PROF("k_firefly", stream);
-            k_firefly_tiled<<<tgrid, FF_TW * FF_TH, 0, stream>>>((const uint4*)in->curr.d_core, (const float*)in->curr.d_depth,
-                direct, indirect, sz.d_composited, p);
+            (withSky ? k_firefly_tiled<true> : k_firefly_tiled<false>)<<<tgrid, FF_TW * FF_TH, 0, stream>>>((const uint4*)in->curr.d_core,
+                (const float*)in->curr.d_depth, direct, indirect, sz.d_composited, p, skyArgs);
             ZR_LAUNCH_CHECK();
         }
         else
         {
             ZR_PROF("k_compositing", stream);
             const dim3 grid((width + 31) / 32, (p.rowEnd - p.rowBegin + 7) / 8);
-            k_compositing<<<grid, 256, 0, stream>>>((const uint4*)in->curr.d_core, direct, indirect, sz.d_composited, p);
+            (withSky ? k_compositing<true> : k_compositing<false>)<<<grid, 256, 0, stream>>>((const uint4*)in->curr.d_core, direct, indirect,
+                sz.d_composited, p, skyArgs);
             ZR_LAUNCH_CHECK();
         }
         return ZR_OK;
@@ -436,6 +460,11 @@ extern "C"
         if (!p || !params) return ZR_ERR_INVALID_ARG;
         p->params = *params;
         return ZR_OK;
+    }
+    zr_status zr_compositing_pass_set_sky(zr_compositing_pass* p, const zr_image2d* lut)
+    {
+        if (!p) return ZR_ERR_INVALID_ARG;
+        return zr::Sky::ViewOf("zr_compositing_pass_set_sky", lut, p->sky);
     }
     zr_status zr_compositing_pass_render(zr_compositing_pass* p, const zr_frame_inputs* in, const void* d_direct,
         const void* d_indirect, void* stream)

@@ -13,6 +13,7 @@
 #include "zr_schedule.h"
 
 #include "zr_rdi.cuh"
+#include "zr_sky.cuh"
 
 namespace zr
 {
@@ -281,6 +282,24 @@ namespace
         const Reservoir rs = pairwiseMIS.r_s;
         WriteFinal(fc, finalImg, idx, rs.target * rs.W);
     }
+
+    // The sky behind geometry in accumulating frames (ReSTIR_DI_Temporal.hlsl:274-281), after k_di_temporal / k_di_spatial, which leave
+    // invalid pixels at 0: each invalid pixel of rows [rowBegin, rowEnd) becomes its value before the frame, kept only past the first
+    // accumulated frame, plus Le_SkyWithSunDisk. `before` is FINAL as it was before k_di_temporal.
+    __global__ void __launch_bounds__(256) k_di_sky(zr_frame_constants fc, const uint4* __restrict__ core, Sky::LutView lut,
+        const float4* __restrict__ before, float4* __restrict__ finalImg, uint32_t rowBegin, uint32_t rowEnd)
+    {
+        const uint32_t x = blockIdx.x * 32 + (threadIdx.x & 31);
+        const uint32_t y = rowBegin + blockIdx.y * 8 + (threadIdx.x >> 5);
+        const uint32_t W = fc.RenderWidth;
+        if (x >= W || y >= rowEnd) return;
+        const size_t i = (size_t)y * W + x;
+        if (!(__ldg(&core[i].w) & ZR_GBUFFER_FLAG_INVALID)) return;
+        const float4 b = before[i];
+        const float3 prev = f3(b.x, b.y, b.z);
+        const float3 c = prev * (float)(fc.NumFramesCameraStatic > 1) + Sky::Le_SkyWithSunDisk(fc, lut, x, y);
+        finalImg[i] = f4(c.x, c.y, c.z, b.w);
+    }
 }
 } // namespace zr
 
@@ -303,6 +322,13 @@ struct zr_direct_pass
     bool patternLoaded = false;
     zr_direct_params params = Defaults();
     zr::LightingStrip strip{ "zr_direct_pass" };     // sched[0]: k_di_temporal, sched[1]: k_di_spatial (8x8-group blocks)
+    // zr_direct_pass_set_sky: the LUT (not owned) and, only while it is set, FINAL's copy from before the accumulating frame
+    zr::Sky::LutView sky{ nullptr, 0, 0 };
+    struct SkyCopy
+    {
+        zr::Planes planes{ "zr_direct_pass" };
+        float4* d_before = nullptr;
+    } skyCopy;
 
     static zr_direct_params Defaults()
     {
@@ -328,7 +354,10 @@ struct zr_direct_pass
         ZR_TRY(next.planes.Alloc(next.d_target, n));
         ZR_TRY(next.planes.Alloc(next.d_final, n));
         ZR_TRY(next.planes.Clear());
+        SkyCopy nextSky;
+        if (sky.texels) ZR_TRY(nextSky.planes.Alloc(nextSky.d_before, n, false));
         sz = std::move(next);
+        skyCopy = std::move(nextSky);
         width = w; height = h;
         strip.ForgetSize();
         ResetFlags();
@@ -339,6 +368,16 @@ struct zr_direct_pass
     {
         ZR_TRY(sz.planes.Clear());
         ResetFlags();
+        return ZR_OK;
+    }
+    zr_status SetSky(const zr_image2d* lut)
+    {
+        zr::Sky::LutView view;
+        ZR_TRY(zr::Sky::ViewOf("zr_direct_pass_set_sky", lut, view));
+        SkyCopy next;
+        if (view.texels && !skyCopy.d_before) ZR_TRY(next.planes.Alloc(next.d_before, (size_t)width * height, false));
+        if (!view.texels || !skyCopy.d_before) skyCopy = std::move(next);
+        sky = view;
         return ZR_OK;
     }
     zr_status LoadPattern()
@@ -378,6 +417,13 @@ struct zr_direct_pass
         const BlockSchedule& schedT = strip.sched[0];
         const BlockSchedule& schedS = strip.sched[1];
         const bool plain = (in->scene->materialFeatures & BSDF::MF_ALL) == 0;
+        const bool skyAccumulates = sky.texels && in->frame.Accumulate && in->frame.CameraStatic;
+        if (skyAccumulates)
+        {
+            const size_t rowBytes = (size_t)width * sizeof(float4), first = (size_t)prm.rowBegin * width;
+            ZR_CUDA(cudaMemcpyAsync(skyCopy.d_before + first, sz.d_final + first, (prm.rowEnd - prm.rowBegin) * rowBytes,
+                cudaMemcpyDeviceToDevice, stream));
+        }
         ZR_PROF("k_di_temporal", stream);
         (plain ? k_di_temporal<BSDF::MF_NONE> : k_di_temporal<BSDF::MF_ALL>)<<<schedT.count, ZR_RDI_TEMPORAL_THREADS, DI_TEMPORAL_SMEM_BYTES, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_res[1 - cur], sz.d_target, sz.d_final, dispX, dispY, schedT.d_order);
         ZR_LAUNCH_CHECK();
@@ -387,6 +433,13 @@ struct zr_direct_pass
         {
             ZR_PROF("k_di_spatial", stream);
             (plain ? k_di_spatial<BSDF::MF_NONE> : k_di_spatial<BSDF::MF_ALL>)<<<schedS.count, ZR_RDI_SPATIAL_THREADS, 0, stream>>>(in->scene->dev, f, prm, sz.d_res[cur], sz.d_target, sz.d_final, dispX, dispY, schedS.d_order);
+            ZR_LAUNCH_CHECK();
+        }
+        if (skyAccumulates)
+        {
+            const dim3 grid((width + 31) / 32, (prm.rowEnd - prm.rowBegin + 7) / 8);
+            ZR_PROF("k_di_sky", stream);
+            k_di_sky<<<grid, 256, 0, stream>>>(in->frame, f.core, sky, skyCopy.d_before, sz.d_final, prm.rowBegin, prm.rowEnd);
             ZR_LAUNCH_CHECK();
         }
         isTemporalReservoirValid = true;
@@ -409,6 +462,7 @@ extern "C"
         p->params = *params;
         return ZR_OK;
     }
+    zr_status zr_direct_pass_set_sky(zr_direct_pass* p, const zr_image2d* lut) { return p ? p->SetSky(lut) : ZR_ERR_INVALID_ARG; }
     zr_status zr_direct_pass_render(zr_direct_pass* p, const zr_frame_inputs* in, void* stream)
     {
         if (!p) return ZR_ERR_INVALID_ARG;

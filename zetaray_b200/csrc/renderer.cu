@@ -11,6 +11,7 @@
 //                     DirectLighting                              `side` stream, the least priority, after GBufferRT
 //                     Compositing (+ firefly filter) -> [SVGF denoise, zr_renderer_set_denoiser] -> TAA
 //                     with zr_renderer_set_display: AutoExposure on the TAA input before TAA, Display on its output after it
+//                     with zr_renderer_set_sky: the sky-view LUT on `side`, before DirectLighting
 //
 // Streams (two_streams != 0; otherwise every pass runs on the caller's stream in the order above). `chain` is forked from the caller's
 // stream by an event and holds the frame's critical path: GBufferRT and IndirectLighting, whose shift stages fork two more streams of
@@ -47,6 +48,7 @@ struct zr_renderer
     zr_svgf_pass* svgf = nullptr;                   // optional denoise stage between Compositing and TAA (BASELINE config 3)
     zr_auto_exposure_pass* ae = nullptr;            // optional post-processing (PostProcessor.cpp): both or neither
     zr_display_pass* display = nullptr;
+    zr_sky_pass* sky = nullptr;                     // optional sky-view LUT, read by DirectLighting and Compositing (zr_renderer_set_sky)
     cudaStream_t chain = nullptr;           // GBufferRT + IndirectLighting when twoStreams, the greatest priority
     cudaStream_t side = nullptr;            // DirectLighting when twoStreams, the least priority
     cudaEvent_t evFork = nullptr, evGBuffer = nullptr, evChain = nullptr, evDirect = nullptr;
@@ -115,8 +117,18 @@ struct zr_renderer
         ae = nullptr; display = nullptr;
     }
 
+    // detaches the LUT from the passes that read it, then frees it
+    void ReleaseSky()
+    {
+        if (direct) zr_direct_pass_set_sky(direct, nullptr);
+        if (compositing) zr_compositing_pass_set_sky(compositing, nullptr);
+        if (sky) zr_sky_pass_destroy(sky);
+        sky = nullptr;
+    }
+
     void Release()
     {
+        ReleaseSky();
         if (gbufferPass) zr_gbuffer_pass_destroy(gbufferPass);
         if (direct) zr_direct_pass_destroy(direct);
         if (indirect) zr_indirect_pass_destroy(indirect);
@@ -222,6 +234,12 @@ extern "C"
         s = r->integrator != ZR_INTEGRATOR_RESTIR_PT ? zr_gi_pass_render(r->gi, &in, chainStream)
                                                      : zr_indirect_pass_render(r->indirect, &in, chainStream);
         if (s != ZR_OK) return s;
+        if (r->sky)
+        {
+            // the LUT follows the frame's sun and atmosphere, so it is recomputed every frame (PathTracer.cpp:343-362)
+            s = zr_sky_pass_render(r->sky, &in, directStream);
+            if (s != ZR_OK) return s;
+        }
         s = zr_direct_pass_render(r->direct, &in, directStream);
         if (s != ZR_OK) return s;
         if (r->twoStreams)
@@ -351,6 +369,26 @@ extern "C"
         if (!enable) r->ReleaseDisplay();
         if (out_ae) *out_ae = r->ae;
         if (out_display) *out_display = r->display;
+        return s;
+    }
+    // Sky (PathTracer.cpp:165-185): enable != 0 creates a 256 x 128 sky-view LUT (DefaultRendererImpl.h:165-166) that every frame
+    // recomputes before DirectLighting, on DirectLighting's stream, and that DirectLighting and Compositing read for the background of
+    // pixels without geometry; 0 detaches it and frees it. A strip-sharded frame computes the whole LUT on every rank.
+    zr_status zr_renderer_set_sky(zr_renderer* r, int enable, zr_sky_pass** out_pass)
+    {
+        if (!r) return ZR_ERR_INVALID_ARG;
+        zr_status s = ZR_OK;
+        if (enable && !r->sky)
+        {
+            zr_image2d lut{};
+            s = zr_sky_pass_create(256, 128, &r->sky);
+            if (s == ZR_OK) s = zr_sky_pass_get_output(r->sky, &lut);
+            if (s == ZR_OK) s = zr_direct_pass_set_sky(r->direct, &lut);
+            if (s == ZR_OK) s = zr_compositing_pass_set_sky(r->compositing, &lut);
+            if (s != ZR_OK) r->ReleaseSky();
+        }
+        if (!enable) r->ReleaseSky();
+        if (out_pass) *out_pass = r->sky;
         return s;
     }
     zr_status zr_renderer_get_display_output(zr_renderer* r, zr_image2d* out)

@@ -264,10 +264,20 @@ class GBufferRT(_Pass):
         return int(_d2h((np.zeros(1, dtype=np.uint32), img.d_ptr))[0][0])
 
 
+def _lut_arg(lut):
+    """A set_sky argument: the LUT image (a SkyPass's GetOutput()) by reference, or None for off."""
+    return None if lut is None else C.byref(lut)
+
+
 class DirectLighting(_Pass):
     prefix = "zr_direct_pass"
     Params = _lib.DirectParams
     output_ids = True
+
+    def SetSky(self, lut):
+        """The sky in accumulating frames: pixels without geometry accumulate Le_SkyWithSunDisk from the sky-view LUT `lut` (a
+        SkyPass's GetOutput(), which must outlive its use here); None turns it off."""
+        self._call("set_sky", _lut_arg(lut))
 
 
 class IndirectLighting(_Pass):
@@ -305,6 +315,20 @@ class Compositing(_Pass):
 
     def Render(self, fi, d_direct, d_indirect, stream=None):
         self._call("render", C.byref(fi), d_direct, d_indirect, stream)
+
+    def SetSky(self, lut):
+        """The sky behind geometry in frames that do not accumulate (with emissive_di on), from the sky-view LUT `lut`; None
+        turns it off."""
+        self._call("set_sky", _lut_arg(lut))
+
+
+class SkyPass(_Pass):
+    """Sky (zr_sky_pass, csrc/sky.cu): the lut_w x lut_h sky-view LUT of the frame's sun and atmosphere, R11G11B10F texels as
+    uint32 (GetOutput)."""
+    prefix = "zr_sky_pass"
+
+    def Render(self, fi, stream=None):
+        self._call("render", C.byref(fi), stream)
 
 
 class TAA(_Pass):
@@ -434,7 +458,7 @@ class Renderer:
         check(lib.zr_renderer_get_passes(self.handle, *[C.byref(x) for x in hs]))
         self.gbuffer, self.direct, self.indirect, self.compositing, self.taa = (
             cls._borrow(hnd) for cls, hnd in zip((GBufferRT, DirectLighting, IndirectLighting, Compositing, TAA), hs))
-        self.gi = self.svgf = self.auto_exposure = self.display = None
+        self.gi = self.svgf = self.auto_exposure = self.display = self.sky = None
 
     @staticmethod
     def _wrapper(current, cls, handle):
@@ -480,6 +504,13 @@ class Renderer:
         self.display = self._wrapper(self.display, Display, disp)
         if enable and lut is not None:
             self.display.SetLUT(lut)
+
+    def SetSky(self, enable=True):
+        """The sky behind geometry: a 256 x 128 SkyPass recomputed every frame before DirectLighting, read by DirectLighting and
+        Compositing. False frees it."""
+        h = C.c_void_p()
+        check(lib.zr_renderer_set_sky(self.handle, int(enable), C.byref(h)))
+        self.sky = self._wrapper(self.sky, SkyPass, h)
 
     def Pick(self, x, y):
         """DefaultRenderer::Pick: the next Render reports the instance under pixel (x, y) (GBufferRT.Pick)."""
